@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py — Groth16 prove throughput on B200 (the driver's contract).
+"""bench.py — Groth16 prove throughput on H100 (the driver's contract).
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload prove|g1msm|g2msm|verify]
-                    [--logn L] [--with-qap]
+                    [--logn L] [--with-qap] [--dump-outputs DIR]
 
 Default workload (BASELINE.json's metric): one step = one groth16.GenerateProofs (groth16/groth16.go:225-278) on the
 synthetic R1CS shape of SURVEY §8(d): n = 2^20 constraints, m = n+2 signals, NPublic = 1, full-width witness.
@@ -24,6 +24,10 @@ Other workloads (BASELINE.json configs 3 and 5; never the default line):
 `--impl reference` times the reference's own algorithm (oracle/ref_c.c: per-term MSB-first double-and-add + add-2007-bl
 accumulate, exactly groth16.go:243-271) on the host cores, on a fixed-size sample of the same workload; nothing of the
 GPU library is loaded in that arm.
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy (float64; every 254-bit
+field element as 8 little-endian 32-bit limbs, each exact in float64; points in affine form), so two builds can be compared
+output for output on the same seeded inputs.
 """
 import argparse
 import ctypes
@@ -51,7 +55,7 @@ R_MOD = 218882428718392752222464057452572750885483644004160343436982041865758084
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps (--impl reference: timed repeats of the CPU sample)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="prove", choices=["prove", "g1msm", "g2msm", "verify"])
@@ -66,12 +70,19 @@ def parse():
                          "latency chains of one proof overlap the accumulation of the other; 1 = one proof at a time)")
     ap.add_argument("--pairing-kernel", type=int, default=None, choices=[0, 1, 2], help="A/B (verify workload): b200_pairing_batch with one thread (1) / one warp (2) per pairing")
     ap.add_argument("--tma-staging", type=int, default=None, choices=[0, 1, 2], help="A/B: staged backward pass off / all rounds / rounds >= 2")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64 32-bit limbs, <= 64 MB in all)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU arm computed; --impl reference has no such outputs")
+    return args
 
 
 # --------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -267,7 +278,7 @@ def run_reference(args):
     ref = CpuReference()
     for _ in range(args.warmup):
         ref.per_term()
-    v, info = reference_value(ref, args.workload, n, max(args.steps, 5))
+    v, info = reference_value(ref, args.workload, n, args.steps)
     if args.workload != "prove":
         v = v * n / 1e6                      # MSMs per second -> Mscalar-mul/s
     info["value"], info["unit"] = v, unit
@@ -359,46 +370,54 @@ def timed(c, fn, steps, wall=False, profile=False, extra_streams=()):
 
 
 def peaks_hbm():
+    """HBM bandwidth the roofline fraction is taken against: the measured figure of MEASURED_PEAKS.json (hbm_gbs) where the
+    machine provides one, else NVIDIA's data-sheet figure for the H100 SXM (80 GB HBM3), which is not a measurement."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return json.load(f).get("hbm_gbs", 6650.0), "MEASURED_PEAKS.json hbm_gbs (of measured)"
-    except Exception:
-        return 6650.0, "fallback 6650 GB/s (of fallback)"
+            return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
+    except (OSError, ValueError, KeyError, TypeError):
+        return 3350.0, "H100 SXM data sheet, 3.35 TB/s (not measured)"
 
 
-def measured_traffic():
-    """Per-term DRAM bytes of the G1 accumulation phase from this round's ncu --set full capture (profiles/traffic.json,
-    regenerated by tools/ncu_traffic.py from profiles/r2_ncu_*.csv); None when that capture does not exist."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return None
+# ------------------------------------------------------------------- --dump-outputs
+DUMP_LIMIT = 64 << 20
 
 
-# measured on B200 with ncu (profiles/r2_notes.md): an IMAD.WIDE.U32 warp instruction occupies the fmaheavy pipe for 4
-# cycles per SM sub-partition => 32 wide multiply-accumulates / clk / SM; 148 SMs at 1.965 GHz.
-IMAD_WIDE_PEAK = 148 * 32 * 1.965e9
+def limbs32(a):
+    """(..., 4) uint64 little-endian limbs -> (..., 8) float64 of 32-bit limbs (exact: every limb < 2^53)."""
+    a = np.ascontiguousarray(np.asarray(a, dtype=np.uint64))
+    return a.view(np.uint32).reshape(*a.shape[:-1], 2 * a.shape[-1]).astype(np.float64)
 
 
-def _nwin(n):
-    """Windows per scalar the library uses for an n-term base set (mirror of pick_window_bits, csrc/capi.cu)."""
-    best, best_cost = 8, float("inf")
-    for cbits in range(8, 19):
-        cost = ((255 + cbits - 1) // cbits) * float(n) * 10.0 + 2.0 * float(1 << (cbits - 1)) * 14.0 * 4.0
-        if cost < best_cost:
-            best, best_cost = cbits, cost
-    return (255 + best - 1) // best
+def affine_g1_limbs(flat):
+    """Flattened Jacobian G1 points (k x 12 u64, standard form) -> (k, 2, 8) affine x, y in 32-bit limbs (infinity: 0, 0)."""
+    from gosnark_b200._lib import ints_to_limbs
+    from gosnark_b200.bn128 import _unflatten_g1
+    from oracle import ref_py as o
+    aff = [o.BN.G1.affine(p) for p in _unflatten_g1(np.asarray(flat, dtype=np.uint64).reshape(-1))]
+    vals = [c for p in aff for c in (p[0], p[1])] if aff else []
+    return limbs32(ints_to_limbs(vals).reshape(len(aff), 2, 4))
 
 
-def alu_model(terms_per_launch, ms_per_launch, fq_mults_per_add, wide_per_mult=137.5):
-    macs = fq_mults_per_add * wide_per_mult * _nwin(terms_per_launch) * terms_per_launch / (ms_per_launch * 1e-3)
-    return {"achieved": macs, "peak": IMAD_WIDE_PEAK, "unit": "32x32+64 multiply-accumulates/s", "frac": macs / IMAD_WIDE_PEAK,
-            "windows_per_term": _nwin(terms_per_launch),
-            "note": f"one bucket add per term and window; {fq_mults_per_add} F_q multiplies per batched-affine add x {wide_per_mult} "
-                    "IMAD.WIDE-equivalent fmaheavy slots each (SASS of fp_mul_outlined, profiles/r2_sass_fp_mul.txt: 120 IMAD.WIDE x 4 cycles + 35 "
-                    "IMAD / IMAD.HI / IMAD.X / IMAD.MOV x 2 cycles); peak = 32 "
-                    "IMAD.WIDE / clk / SM (ncu: sm__pipe_fmaheavy_cycles_active, profiles/r2_notes.md) x 148 SMs x 1.965 GHz"}
+def affine_g2_limbs(flat):
+    """Flattened Jacobian G2 points (k x 24 u64) -> (k, 2, 2, 8): affine x, y as F_q2 (c0, c1) in 32-bit limbs."""
+    from gosnark_b200._lib import ints_to_limbs
+    from gosnark_b200.bn128 import _unflatten_g2
+    from oracle import ref_py as o
+    aff = [o.BN.G2.affine(p) for p in _unflatten_g2(np.asarray(flat, dtype=np.uint64).reshape(-1))]
+    vals = [c for p in aff for xy in (p[0], p[1]) for c in xy]
+    return limbs32(ints_to_limbs(vals).reshape(len(aff), 2, 2, 4))
+
+
+def dump_outputs(dirname, arrays):
+    """Write each array as dirname/<name>.npy (float32 / float64 only, <= DUMP_LIMIT bytes in all)."""
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        raise SystemExit(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT}-byte limit")
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 def run_prove(args, c):
@@ -415,7 +434,7 @@ def run_prove(args, c):
     if n_fly > 1 and world > 1:    # latency hidden by the second proof: every shard takes the batched-affine tree (6 vs 10 multiplies per add)
         check(L.b200_config(_lib.CFG_SHARD_AFFINE_MIN_G1, 1))
         check(L.b200_config(_lib.CFG_SHARD_AFFINE_MIN_G2, 1))
-        # partition weights for that mode (profiles/r2_notes.md section 16, every rank of the 2 / 4 / 8-way split timed on one GPU):
+        # partition weights for that mode (every rank of the 2 / 4 / 8-way split timed on one GPU):
         # the C||PTD ranks also run the division, so their terms weigh more — A / B1 terms 0.85, G2 terms 2.75 of a C||PTD term
         check(L.b200_config(_lib.CFG_SHARD_W_AB, 85))
         check(L.b200_config(_lib.CFG_SHARD_W_G2, 275))
@@ -512,6 +531,9 @@ def run_prove(args, c):
     prof0 = (ctypes.c_double * 8)()
     check(L.b200_profile_read(prof0))          # reset counters
     ms_total = timed(c, step_in_flight, args.steps, profile=args.profile_region, extra_streams=fly_streams[1:])
+    if args.dump_outputs and rank == 0:      # the proof of the last timed step, before later measurements reuse its buffer
+        last = d_outs[(fly_ctr[0] - 1) % n_fly].cpu().numpy().view(np.uint64)
+        dumped = {"pi_a": affine_g1_limbs(last[:12])[0], "pi_b": affine_g2_limbs(last[24:])[0], "pi_c": affine_g1_limbs(last[12:24])[0]}
     prof = (ctypes.c_double * 8)()
     check(L.b200_profile_read(prof))
     check(L.b200_profile(0))
@@ -599,9 +621,6 @@ def run_prove(args, c):
     g1_ms, g1_l, g1_terms = prof_x[0], max(prof_x[1], 1), prof_x[2]      # exclusive (serialised) timings, this rank
     g2_ms, g2_l, g2_terms = prof_x[3], max(prof_x[4], 1), prof_x[5]
     ach = 96.0 * (g1_terms / g1_l) / (g1_ms / g1_l * 1e-3) / 1e9 if g1_ms > 0 else None
-    tr = measured_traffic()
-    per_term = (tr or {}).get("g1_accumulation_dram_bytes_per_term")
-    traffic = per_term * (g1_terms / g1_l) if per_term and g1_ms > 0 else None
     metric, unit = metric_of("prove")
     line = {
         "metric": metric, "value": value, "unit": unit, "n_gpus": world,
@@ -627,18 +646,15 @@ def run_prove(args, c):
             "bound": "hbm", "kernel": "G1 bucket accumulation phase (k_affine_forward / k_affine_invert / k_affine_backward<Fq> rounds; "
                                       "k_accumulate<Fq> below the affine threshold)",
             "achieved": ach, "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None, "peak_source": peak_src,
-            "traffic": traffic,
-            "traffic_source": (tr or {}).get("source", "not measured in this run: no profiles/traffic.json from this round's ncu capture"),
+            "traffic": None, "traffic_source": "not measured",
             "launches_per_step": prof_x[1] / ser_steps, "avg_launch_ms": g1_ms / g1_l,
             "timing": "CUDA events around each phase on its stream, measured with the proof's MSMs serialised on one stream "
                       f"(b200_profile(3)); serialised step = {ms_serial:.3f} ms, overlapped step = {ms_step:.3f} ms",
             "share_of_serial_step": (g1_ms / ser_steps) / ms_serial if ms_serial else None,
-            "note": "bound by the integer multiply pipe (fmaheavy: IMAD.WIDE occupies it 4 cycles per warp; ncu on the dominant "
-                    "kernel: sm__pipe_fmaheavy_cycles_active 76.7 %, DRAM 25 %), not by HBM: the HBM fraction is reported "
-                    "because the contract asks for it (SURVEY H8)",
+            "note": "the accumulation is field-multiply work (integer multiply-adds) over gathered points; the HBM fraction of "
+                    "its algorithmic bytes is reported because the contract asks for it (SURVEY H8)",
             "g2": {"avg_launch_ms": g2_ms / g2_l, "share_of_serial_step": (g2_ms / ser_steps) / ms_serial if ms_serial else None,
                    "achieved": 160.0 * (g2_terms / g2_l) / (g2_ms / g2_l * 1e-3) / 1e9 if g2_ms > 0 else None},
-            "alu": alu_model(g1_terms / g1_l, g1_ms / g1_l, 6) if g1_ms > 0 else None,
             "overlapped": {"g1_avg_ms": prof[0] / max(prof[1], 1), "g2_avg_ms": prof[3] / max(prof[4], 1)}},
         "algorithmic_bytes_per_proof": syn.algorithmic_bytes(),
         "per_rank": per_rank,
@@ -647,7 +663,7 @@ def run_prove(args, c):
         line["verified_under_real_vk"] = verified
     if not args.no_extras and world == 1 and not args.with_qap:
         try:
-            line["g1_msm_2p20"] = side_g1_msm(c)
+            line["g1_msm_2p20"] = side_g1_msm(c, steps=args.steps, warmup=args.warmup)
         except Exception as e:   # a side measurement must never take the bench line down
             line["g1_msm_2p20"] = {"error": str(e)}
     if not args.no_extras and world == 1:
@@ -659,11 +675,13 @@ def run_prove(args, c):
             line["cpu_baseline"] = cinfo
         except Exception as e:   # the checker must never take the bench line down
             line["cpu_baseline"] = {"error": str(e)}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumped)
     print(json.dumps(line))
     return 0
 
 
-def side_g1_msm(c, logn=20, steps=10, warmup=3):
+def side_g1_msm(c, steps, warmup, logn=20):
     """The other half of BASELINE.json's metric inside the default line: a stand-alone BN128 G1 MSM of 2^logn random scalars /
     points (config 3), device-resident — two MSMs in flight on two base-set objects, and one at a time."""
     torch, L = c.torch, c.L
@@ -802,6 +820,11 @@ def run_msm(args, c):
     torch.cuda.synchronize()
     ms = timed(c, step_in_flight, args.steps, profile=args.profile_region, extra_streams=fly_streams[1:]) / args.steps
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs:                    # the whole MSM of the last timed step (world > 1: summed over every rank's partial)
+        src = d_alls if world > 1 else d_parts
+        check((L.b200_g1_sum_partials if group == 1 else L.b200_g2_sum_partials)(src[(fly_ctr[0] - 1) % n_fly].data_ptr(), world,
+                                                                                 ptr(out), st))
+        dumped = {"msm": (affine_g1_limbs if group == 1 else affine_g2_limbs)(out)[0]}
     # one MSM at a time (its latency), with CUDA events around its accumulation phase for the roofline
     check(L.b200_profile(1))
     prof = (ctypes.c_double * 8)()
@@ -841,8 +864,7 @@ def run_msm(args, c):
             "whole_msm_hbm_algorithmic_GBps": bpt * n / (ms * 1e-3) / 1e9,
             "roofline": {"bound": "hbm", "kernel": f"G{group} bucket accumulation phase of this rank's shard", "achieved": ach, "peak": peak,
                          "unit": "GB/s", "frac": (ach / peak) if ach else None, "peak_source": peak_src, "traffic": None,
-                         "avg_launch_ms": acc_ms / acc_l,
-                         "alu": alu_model(acc_terms / acc_l, acc_ms / acc_l, 6 if group == 1 else 6 * 2.6) if acc_ms > 0 else None}}
+                         "avg_launch_ms": acc_ms / acc_l}}
     if not args.no_extras and world == 1:
         try:
             ref = CpuReference()
@@ -852,6 +874,8 @@ def run_msm(args, c):
             line["cpu_baseline"] = cinfo
         except Exception as e:
             line["cpu_baseline"] = {"error": str(e)}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumped)
     print(json.dumps(line))
     return 0
 
@@ -903,6 +927,10 @@ def run_verify(args, c):
         step()
     ms = timed(c, step, args.steps, wall=True) / args.steps
     clk = clocks.stop()
+    if args.dump_outputs:                    # a fixed, seeded sample of the pairings (F_q^12 = 12 F_q coefficients each)
+        rows = np.sort(np.random.default_rng(0x5EED0007).choice(n, size=min(n, 4096), replace=False))
+        dump_outputs(args.dump_outputs, {"pairing": limbs32(out[rows].reshape(len(rows), 12, 4)),
+                                         "pairing_rows": rows.astype(np.float64)})
     # groth16.VerifyProof latency on a real instance
     syn = CircuitGroth16(6)
     pk = syn.load_pk()

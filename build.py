@@ -1,13 +1,11 @@
-"""Build helpers: everything is compiled IN-TREE with explicit commands so the
-built .so files travel to the GPU box with the gpurun snapshot.
+"""Build helpers: everything is compiled IN-TREE with explicit commands, so the
+package is importable from the repository tree after build().
 
-  build_cuda()        nvcc -> go-snark-study_b200/lib/libb200snark.so   (the product: sm_100a only)
+  build_cuda()        nvcc -> go-snark-study_b200/lib/libb200snark.so   (the product: sm_90a only)
   build_host_arith()  g++  -> go-snark-study_b200/lib/libb200_host_arith.so (CPU unit-test vehicle)
   build_oracle()      gcc  -> oracle/_build/liboracle.so             (test infrastructure)
-  stage_ref_binary()  copies the reference's prebuilt Go CLI to oracle/_ref/ when /root/reference exists
 """
 import os
-import shutil
 import subprocess
 import sys
 
@@ -20,7 +18,7 @@ HOSTTEST = os.path.join(ROOT, "tests", "host")     # CPU test vehicles for the k
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CUDA_SOURCES = ["capi.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 
@@ -112,23 +110,7 @@ def build_oracle(force=False):
     return target
 
 
-def stage_ref_binary():
-    """The reference is Go (no toolchain here), but it ships a prebuilt CLI
-    (go-snark-cli, build-cli.sh:3-4).  Stage it under oracle/_ref/ (git-ignored,
-    NOT gpurun-ignored) so GPU-box tests can have real Go code verify our proofs."""
-    src = "/root/reference/go-snark-cli"
-    dst_dir = os.path.join(ORACLE, "_ref")
-    dst = os.path.join(dst_dir, "go-snark-cli")
-    if os.path.exists(src):
-        os.makedirs(dst_dir, exist_ok=True)
-        if not os.path.exists(dst) or os.path.getsize(dst) != os.path.getsize(src):
-            shutil.copy(src, dst)
-            os.chmod(dst, 0o755)
-    return dst if os.path.exists(dst) else None
-
-
 if __name__ == "__main__":
     print(build_host_arith(force=True))
     print(build_oracle(force=True))
-    print(stage_ref_binary())
     print(build_cuda(force=True))

@@ -1,4 +1,4 @@
-"""go-snark-study_b200 — B200-native Groth16 / Pinocchio prove path.
+"""go-snark-study_b200 — H100-native Groth16 / Pinocchio prove path.
 
 Host-side mirror of the reference's Go package API for the prove path
 (bn128.G1/G2, r1csqap.PolynomialField, groth16.GenerateProofs,

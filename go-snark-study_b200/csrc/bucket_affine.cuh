@@ -3,7 +3,7 @@
 // An affine addition costs 1 inversion + 2M + 1S; with Montgomery's trick a batch
 // of denominators shares one inversion at 3M each, so a bucket add costs ~6.5 field
 // multiplications instead of the 10 (8M + 2S) of the XYZZ mixed add — and the
-// multiply pipe (IMAD.WIDE, quarter rate on sm_100) is what bounds this kernel
+// integer multiply pipe (IMAD.WIDE) is what bounds this kernel
 // (DESIGN.md §4).
 //
 // Shape.  Buckets are cut into slices of exactly S = 2^R leaf slots (the tail of a
@@ -22,7 +22,7 @@
 //                      peeling 1/d off the running inverse, and writes the sums
 // After R rounds every slice is one affine point; k_merge_slices_affine folds the
 // slices of a bucket into the XYZZ bucket array consumed by the weighted reduction.
-// Measured and dropped (profiles/r2_notes.md): register-staged and L2-prefetch software pipelines of the operand
+// Measured and dropped: register-staged and L2-prefetch software pipelines of the operand
 // fetches, an inlined multiply, a backward pass ordered for short live ranges, a thread-per-slice variant with the
 // rounds fused, fewer pairs per thread in the late rounds, an XYZZ tail after a few affine rounds.
 #pragma once
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(kAffBlock, MINB) k_affine_forward(AffineRound<
 }
 
 // One warp per block total, lane 0 working: the binary-Euclid inversion has data-dependent control flow, and this
-// launch is pure latency (a few thousand inversions between two machine-filling passes) -- 182 us with a^(p-2).
+// launch is pure latency (a few thousand inversions between two machine-filling passes), far longer with a^(p-2).
 template <class F>
 __global__ void __launch_bounds__(128) k_affine_invert(F* btot, uint32_t nblocks_live) {
   uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -522,8 +522,7 @@ __global__ void __launch_bounds__(kAffBlock, MINB) k_affine_backward_staged(Affi
 // A thread folds up to kMergeSeq slices itself; only buckets beyond that (skewed scalar distributions) take the warp path.
 // bases_create picks S so that the MEAN bucket holds 6..12 slices, and the population spreads around it: with the bound at 12
 // (rounds 1-2 of this kernel) nearly half the buckets of a set whose mean sat just under 12 slices went down the warp path,
-// one after the other — a 832 k-term G1 MSM took 4.89 ms where a 845 k-term one (next S, 6 slices) took 3.67
-// (profiles/r2_slice_cliff.log).  Twice the largest mean leaves the warp path to the genuinely skewed buckets.
+// one after the other, so a G1 MSM just below the next S was far slower than one just above it (tools/slice_cliff.py).  Twice the largest mean leaves the warp path to the genuinely skewed buckets.
 constexpr uint32_t kMergeSeq = 24;
 template <class F>
 __global__ void __launch_bounds__(128)

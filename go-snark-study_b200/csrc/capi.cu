@@ -53,7 +53,7 @@ Comm g_comm;  // NCCL communicator of this process (b200_comm_init); world 1 = n
 // b200_config: bucket-accumulation kernel of base sets / proving keys created afterwards
 // (0 auto: batched affine where the bucket population and the shard size amortise its rounds, else XYZZ; 1, 2 force)
 int g_acc_mode = 0;
-// partition tuning (b200_config keys 10..13; defaults = the measured best, profiles/r2_notes.md §8)
+// partition tuning (b200_config keys 10..13; defaults = the measured best for one proof at a time)
 int g_w_ab = 100, g_w_g2 = 280, g_aff_min_g1 = 700000, g_aff_min_g2 = 400000;
 int g_tma_staging = 0;   // B200_CFG_TMA_STAGING: 1 staged backward pass in every round, 2 only in the contiguous rounds (>= 2)
 
@@ -217,7 +217,7 @@ int check_err_flag(const char* what, cudaStream_t st = nullptr, std::unique_lock
 
 // prefer_affine: batched-affine bucket accumulation (6 multiplies per add instead of 10) whenever the buckets are
 // populated enough to amortise its per-round launches; since the per-round inversion became a binary-Euclid warp
-// (182 -> ~45 us) it also wins for a stand-alone MSM (2^20: G1 4.40 vs 4.46 ms, G2 9.26 vs 11.80 ms XYZZ).  A proving-key
+// it also wins for a stand-alone MSM.  A proving-key
 // shard that leaves a rank only a small MSM passes false (prove_host.cuh); B200_ACC_MODE=xyzz|affine forces either.
 template <class F>
 int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_ptr<Bases>& out_b, bool prefer_affine = true) {
@@ -312,8 +312,8 @@ Bases* find_bases(b200_bases_t h, int group) {
 
 // Enqueue one MSM on `st`; result XYZZ written to d_out (device).
 // Accumulate launch: LPB lanes per bucket slice (2 / 4 / 8 by mean bucket population).  Register budget:
-// G1 runs at 128 regs (4 CTAs/SM); occupancy / prefetch variants measured within 2% of each other
-// (profiles/r1_notes.md) — the kernel is bound by the IMAD.WIDE issue rate, not by latency hiding.
+// G1 runs at 128 regs (4 CTAs/SM); occupancy / prefetch variants were no faster — the kernel is bound by the
+// IMAD.WIDE issue rate, not by latency hiding.
 template <class F, int LPB>
 void launch_accumulate_l(const Affine<F>* table, const uint32_t* entries, SliceTables stb, uint32_t m,
                          XYZZ<F>* out, uint32_t max_slices, cudaStream_t st) {
@@ -405,7 +405,7 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
   XYZZ<F>* partials = b->partials.as<XYZZ<F>>();
   SliceTables stb = ss.tables();
   // The out-of-line F_q multiply wins here: the fully inlined madd body (~38 KB of SASS) thrashes the
-  // instruction caches (measured 5.85 ms vs 4.80 ms at 2^20, profiles/r1_notes.md).
+  // instruction caches.
   ProfRec pr{};
   if (g_prof) {
     pr = ProfRec{prof_event(), prof_event(), b->group, n_terms};
@@ -442,8 +442,8 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
       ar.out = bufs[(r - 1) & 1];
       uint64_t npairs_max = nsl_bound << ar.q_log;
       unsigned nb = (unsigned)((npairs_max + kAffBlock * kAffPairs - 1) / (kAffBlock * kAffPairs));
-      // CTAs/SM bounds = register caps (ptxas -v: forward 64 / 128 registers, backward 96 / 128, G1 / G2; measured
-      // sweep in profiles/r1_notes.md: forward 8 + backward 5 CTAs/SM for G1, 4 + 4 for G2)
+      // CTAs/SM bounds = register caps (forward 8 + backward 5 CTAs/SM for G1, 4 + 4 for G2); chosen by a sweep on an
+      // earlier target and not re-swept on the H100
       if (sizeof(F) == 32) {
         k_affine_forward<F, kAffPairs, 8><<<nb, kAffBlock, 0, st>>>(ar);
         k_affine_invert<F><<<nblocks((size_t)nb * 32, 128), 128, 0, st>>>(ar.btot, nb);
@@ -917,7 +917,7 @@ __global__ void k_ic_sum(const Fq* ic, const Jacobian<Fq>* terms, size_t npub, F
 // Final exponentiation: Devegili-Scott-Dahab (easy part + hard part by the BN parameter), the SAME F_q^12 value as the
 // reference's plain f^((q^12-1)/r) square-and-multiply (bn128.go:400-421) with ~13x fewer operations: validated on the
 // GPU against the snarkjs golden vk_alfabeta_12 (K8), the bn128_test.go literal and the oracle (tests/test_gpu_verify.py,
-// profiles/r2_notes.md).  The plain routine stays in pairing.cuh as the step-by-step restatement used by the host tests.
+// tests/test_host_pairing.py).  The plain routine stays in pairing.cuh as the step-by-step restatement used by the host tests.
 constexpr bool kFastFinalExp = true;
 int pairing_batch_host(const uint64_t* g1, const uint64_t* g2, size_t n, uint64_t* out) {
   if (!g1 || !g2 || !out) return fail(B200_EINVAL, "pairing_batch: null pointer");
@@ -928,8 +928,8 @@ int pairing_batch_host(const uint64_t* g1, const uint64_t* g2, size_t n, uint64_
   CU(dout.alloc(n * 6 * sizeof(Fq2)));
   CU(cudaMemcpyAsync(d1.p, g1, n * 3 * sizeof(Fq), cudaMemcpyHostToDevice, g_stream));
   CU(cudaMemcpyAsync(d2.p, g2, n * 3 * sizeof(Fq2), cudaMemcpyHostToDevice, g_stream));
-  // auto: a warp per pairing has the 5x shorter latency (3.4 vs 17 ms) and wins up to ~3 500 pairings per call; above that the
-  // thread-per-pairing kernel keeps more pairings resident and has twice the throughput (462 k vs 204 k pairings/s at 2^16)
+  // auto: a warp per pairing has the much shorter latency and wins for small calls; above that the thread-per-pairing
+  // kernel keeps more pairings resident and has the higher throughput
   const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
   if (thread_kernel) k_pairing_batch<kFastFinalExp><<<nblk(n, 32), 32, 0, g_stream>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
   else k_pairing_batch_warp<<<nblk(n, kPairWarps), 32 * kPairWarps, 0, g_stream>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);

@@ -11,7 +11,7 @@
 namespace b200 {
 
 // BN254's endomorphism phi(x, y) = (beta*x, y) acts as multiplication by lambda, and every k splits as k1 + k2*lambda (mod r)
-// with |k1|, |k2| < 2^128 (glv_decompose below, on the host).  A 254-bit double-and-add in a lone thread is ~2 ms of dependent
+// with |k1|, |k2| < 2^128 (glv_decompose below, on the host).  A 254-bit double-and-add in a lone thread is a long chain of dependent
 // field multiplications and sits on the critical path of a small proof and of every verification: here sixteen lanes share
 // one product (glv_mul_halfwarp).  Constants derived and checked against the oracle (tools/glv_constants.py).
 struct GlvScalars {

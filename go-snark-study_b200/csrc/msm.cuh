@@ -5,14 +5,14 @@
 // Data layout in HBM (DESIGN.md §3):
 //   table   [nwin][n]  Affine<F>, Montgomery form: table[w][i] = 2^(c*w) * P_i
 //                      (64 B per G1 point, 128 B per G2 point, 32 B-aligned so a
-//                      point is 2 / 4 LDG.256 sector-exact loads)
+//                      point is 4 / 8 sector-exact 128-bit loads)
 //   scalars [n]        4 x u64 standard form (or Montgomery if produced by the
 //                      NTT pipeline)
 //   entries [nwin*n]   u32: (w*n + i) << 1 | sign, counting-sorted by bucket
 //   buckets [B]        XYZZ<F>, B = 2^(c-1) (signed digits)
 //
-// Because every window's multiple is precomputed (the CRS is static; 180 GB of
-// HBM makes a 16x table affordable), all windows feed ONE bucket set and the
+// Because every window's multiple is precomputed (the CRS is static; a 2^20-term
+// G1 table is ~1 GB, so 80 GB of HBM holds the tables of several keys), all windows feed ONE bucket set and the
 // final result is a single sum_b b * S_b — no per-window reduction, no Horner
 // doublings on the critical path.
 //
@@ -33,11 +33,13 @@
 namespace b200 {
 
 // ------------------------------------------------------------ vector loads
-// 256-bit global loads (sm_100+: LDG.E.ENL2.256) for 32 B-aligned field elements.
+// A 32 B-aligned field element as two 128-bit global loads (sm_90 has no 256-bit load; both halves hit the same
+// 32-byte sector).
 __device__ __forceinline__ void ld256(const void* p, uint32_t* o) {
   uint64_t a, b, c, d;
 #ifdef __CUDA_ARCH__
-  asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+  asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(a), "=l"(b) : "l"(p));
+  asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%2+16];" : "=l"(c), "=l"(d) : "l"(p));
 #else  // g++ test vehicle (csrc/host_stub)
   const uint64_t* q = static_cast<const uint64_t*>(p);
   a = q[0]; b = q[1]; c = q[2]; d = q[3];
@@ -47,12 +49,13 @@ __device__ __forceinline__ void ld256(const void* p, uint32_t* o) {
   o[4] = (uint32_t)c; o[5] = (uint32_t)(c >> 32);
   o[6] = (uint32_t)d; o[7] = (uint32_t)(d >> 32);
 }
-// Same, for random gathers of 64-byte points: ask L2 to fetch only the 64 B it needs (LDG...LTC64B);
-// the default pulls the whole 128-byte line from HBM (ncu: 2.1 GB read for 1.07 GB of points).
+// Same, for random gathers of 64-byte points: ask L2 to fetch only the 64 B it needs (LDG...LTC64B)
+// rather than the whole 128-byte line.
 __device__ __forceinline__ void ld256_g64(const void* p, uint32_t* o) {
   uint64_t a, b, c, d;
 #ifdef __CUDA_ARCH__
-  asm volatile("ld.global.nc.L2::64B.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+  asm volatile("ld.global.nc.L2::64B.v2.u64 {%0,%1}, [%2];" : "=l"(a), "=l"(b) : "l"(p));
+  asm volatile("ld.global.nc.L2::64B.v2.u64 {%0,%1}, [%2+16];" : "=l"(c), "=l"(d) : "l"(p));
 #else
   const uint64_t* q = static_cast<const uint64_t*>(p);
   a = q[0]; b = q[1]; c = q[2]; d = q[3];
@@ -236,7 +239,7 @@ __global__ void __launch_bounds__(1024) k_scan(const uint32_t* __restrict__ coun
                                                uint32_t* offsets, uint32_t* cursor, SliceTables st) {
   // One block walks the m counters in coalesced tiles of blockDim.x; (entry count, slice count) are packed into one
   // 64-bit value so a single warp-shuffle scan + a scan of the warp totals serves both prefix sums.  (The first version
-  // gave every thread 64 consecutive counters: uncoalesced and serial, 140 us for 2^16 buckets.)
+  // gave every thread 64 consecutive counters: uncoalesced and serial.)
   __shared__ unsigned long long wsum[32];
   __shared__ unsigned long long carry_s;
   const uint32_t t = threadIdx.x, T = blockDim.x, lane = t & 31u, warp = t >> 5, nwarps = T >> 5;
@@ -304,7 +307,7 @@ __global__ void k_fill_slices(const uint32_t* __restrict__ counts, const uint32_
 // l, l+LPB, ... (coalesced reads of `entries`), gathers the precomputed affine
 // points and mixed-adds them; a warp-shuffle tree then merges the LPB partials.
 // (A software-prefetch variant — next point fetched before the current add — and 80..154-register builds were
-// measured within 2 % of this one: the kernel is bound by the multiply pipe, profiles/r1_notes.md.)
+// no faster: the kernel is bound by the multiply pipe.)
 template <class F, int LPB, int MINB = 1>
 __global__ void __launch_bounds__(128, MINB)
 k_accumulate(const Affine<F>* __restrict__ table, const uint32_t* __restrict__ entries, SliceTables st,
@@ -431,7 +434,7 @@ k_sum_points(const XYZZ<F>* __restrict__ in, uint32_t count, uint32_t per_block,
 // (3) k_tail_horner: the c-1 planes of the combined weight (low kl bits from the columns, high bits from the rows) in one
 //     Horner chain of c-1 doublings and additions, plus the plain sum.
 // Depth: ~(K/32 + 5) + (K/32 + 5) + 2(c-1) dependent group operations instead of 2*seg + 16 doublings + ... per thread
-// followed by two more tree levels — 0.59 -> ~0.2 ms on a 2^16-bucket set, which is the serial tail of every MSM
+// followed by two more tree levels, on the serial tail of every MSM
 // (stand-alone MSM latency, and the per-rank critical path when a proof is sharded over 8 GPUs).
 template <class F>
 __device__ __forceinline__ XYZZ<F> warp_sum_xyzz(XYZZ<F> acc) {

@@ -1,7 +1,7 @@
 // Optimal-ate pairing, ONE WARP per pairing (bn128/bn128.go:179-421; the thread-per-pairing restatement is pairing.cuh).
 //
-// A pairing is ~25 000 dependent F_q multiplications when one thread walks the tower; a dependent multiplication in a
-// lone thread costs ~0.4 us, so a verification (groth16.go:281-305: four pairings) took ~20 ms however idle the GPU was.
+// A pairing is ~25 000 dependent F_q multiplications when one thread walks the tower, so a verification
+// (groth16.go:281-305: four pairings) is a long latency chain however idle the GPU is.
 // Here the F_q^12 accumulator and every temporary live in SHARED memory and the 32 lanes of a warp share the work of
 // each tower operation:
 //   F_q^12 product   Karatsuba over F_q^6 (3 products) x schoolbook inside F_q^6 (9 F_q^2 products each) = 27 F_q^2

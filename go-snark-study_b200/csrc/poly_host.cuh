@@ -61,7 +61,7 @@ struct NttPlan {
 
 struct PolyCtx {
   // Transforms of >= 2^10 points run as fused shared-memory passes (ntt.cuh: k_ntt_fused; 3 passes instead of 21 stage
-  // launches at 2^21 points: 19.36 -> 18.88 ms per 2^20 proof, profiles/r2_notes.md); bit-identical to the stage kernels.
+  // launches at 2^21 points); bit-identical to the stage kernels.
   static constexpr bool fused() { return true; }
   unsigned long long* launch_counter = nullptr;
   void note(unsigned n) { if (launch_counter) *launch_counter += n; }

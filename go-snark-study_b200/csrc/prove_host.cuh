@@ -173,7 +173,7 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   const size_t n_c_full = pk->n_c_full = m - l1;
   const size_t len[4] = {m, m, m, n_c_full + n_ptd};
   // Cost weights of the line partition, in G1 terms of the C||PTD set: a G2 term (B2), and a term of A / B1 — whose ranks
-  // also pay the two GLV products s*A_part + r*B1_part (1 ms of single-warp latency) on their critical path when sharded.
+  // also pay the two GLV products s*A_part + r*B1_part (single-warp latency) on their critical path when sharded.
   const double w_ab = world > 1 ? g_w_ab / 100.0 : 1.0;
   const double wgt[4] = {w_ab, w_ab, g_w_g2 / 100.0, 1.0};
   std::vector<ShardCut> cuts((size_t)world);
@@ -185,11 +185,10 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   }
   // a set whose end falls exactly on a cut: the rank holding its last element owns the tail (checked above);
   // if no rank holds elements of it (len == 0) the last rank does.
-  // Accumulation kernel per SET of this rank (profiles/r2_notes.md §8).  Stand-alone, G2 sets win with the batched-affine
-  // tree from 2^18 terms (3.82 vs 4.21 ms; 5.20 vs 6.54 at 2^19) and G1 sets from ~2^19.5 (2.53 vs 2.45 ms at 2^19, 3.96 vs 4.12
-  // at 2^20); inside a sharded proof a 318 k-term G2 shard was still faster on the XYZZ kernel (4.81 vs 5.69 ms per rank), a
-  // 524 k-term one on the affine tree — hence 4e5 / 7e5.  A single-GPU key always takes the affine tree: its four MSMs cover
-  // each other's gaps.
+  // Accumulation kernel per SET of this rank.  The batched-affine tree pays off once a set is large enough to amortise its
+  // per-round launches (G2 sets earlier than G1 sets); below g_aff_min_g1 / g_aff_min_g2 terms a shard takes the XYZZ
+  // kernel, whose single launch has the shorter latency chain.  A single-GPU key always takes the affine tree: its four
+  // MSMs cover each other's gaps.
   auto set_terms = [&](int k) { return (double)(pk->hi[k] - pk->lo[k]); };
   auto affine_for = [&](int k) { return world == 1 || set_terms(k) >= (double)(k == 2 ? g_aff_min_g2 : g_aff_min_g1); };
   // sets that consume identical scalar slices share one digit sort
@@ -381,7 +380,7 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
   if (pk->g[0] || pk->g[1]) {
     k_groth16_products<<<1, 32, 0, s1>>>(res, glv, prod);
   } else {   // a rank that holds no part of A or B1: both products are the point at infinity (all-zero XYZZ) — skip the
-    // 1 ms single-warp chain (it sat on the critical path of 5 of the 8 ranks of an 8-way proof)
+    // single-warp chain (it would sit on the critical path of most ranks of an 8-way proof)
     CU(cudaMemsetAsync(prod, 0, 2 * sizeof(XYZZ<Fq>), s1));
   }
   EV_REC(e_prod, s1);

@@ -5,7 +5,7 @@
 // The sets lie end to end on a line weighted by cost per term (wgt[k], in G1 terms of the C||PTD set) and the line is
 // cut into `world` equal pieces: rank g holds whole sets where it can and an index range where it must; rank g's `lo`
 // is rank g-1's `hi`, so every set is tiled exactly once.
-// (Measured and dropped, profiles/r2_notes.md section 16: a fixed cost per piece with greedy filling to the smallest
+// (Measured and dropped: a fixed cost per piece with greedy filling to the smallest
 // common capacity.  The ranks that hold two pieces are the FAST ones — their two MSMs fill each other's gaps.)
 #pragma once
 #include <cstddef>

@@ -1,6 +1,6 @@
 // Package b200 is the cgo binding of libb200snark (include/b200snark.h): the marshalling layer a
 // maintainer of arnaucube/go-snark-study links under groth16.GenerateProofs / snark.GenerateProofs /
-// r1csqap.PolynomialField / bn128.G1,G2 to run the prove path on a B200.
+// r1csqap.PolynomialField / bn128.G1,G2 to run the prove path on an H100.
 //
 // NOT COMPILED IN THIS REPOSITORY: neither the build image nor the GPU box has a Go toolchain
 // (`go version`: not found).  The identical marshalling is exercised through ctypes by the Python
@@ -132,8 +132,7 @@ func (k *Groth16Key) Free() { C.b200_pk_free(k.h) }
 // LoadGroth16Pair uploads the same groth16.Pk under the library's two prove contexts (B200_CFG_PK_CONTEXT 0 and 1: own
 // tables, scratch, streams).  Two goroutines — one per key — may then call Prove concurrently: a call enqueues under the
 // library mutex and waits for its proof with the mutex released, so the sort / bucket-tail / blinding-product chains of one
-// proof overlap the bucket accumulation of the other (a proof server's steady state: +4 % proofs/s at 2^20 constraints,
-// +30 % at 2^16, bench.py `proofs_in_flight`).  cgo releases the goroutine's OS thread for the duration of the call.
+// proof overlap the bucket accumulation of the other (a proof server's steady state; bench.py `proofs_in_flight`).  cgo releases the goroutine's OS thread for the duration of the call.
 func LoadGroth16Pair(at, b1 [][3]*big.Int, b2 [][3][2]*big.Int, bacDelta, ptd [][3]*big.Int, z []*big.Int,
 	alpha1, beta1, delta1 [3]*big.Int, beta2, delta2 [3][2]*big.Int, nVars, nPublic int) (keys [2]*Groth16Key, err error) {
 	for ctx := 0; ctx < 2; ctx++ {
@@ -389,7 +388,7 @@ func CommDestroy() error { return check(C.b200_comm_destroy()) }
 
 // TuneShardsForTwoInFlight sets the partition of sharded keys loaded AFTERWARDS the way bench.py does when it keeps two
 // proofs in flight (LoadGroth16Pair on every rank): every shard on the batched-affine tree, an A / B1 term 0.85 and a G2
-// term 2.75 of a C||PTD term (profiles/r2_notes.md sections 11 and 16).  The defaults suit one proof at a time.
+// term 2.75 of a C||PTD term.  The defaults suit one proof at a time.
 func TuneShardsForTwoInFlight() error {
 	for _, kv := range [][2]C.int{{C.B200_CFG_SHARD_AFFINE_MIN_G1, 1}, {C.B200_CFG_SHARD_AFFINE_MIN_G2, 1},
 		{C.B200_CFG_SHARD_W_AB, 85}, {C.B200_CFG_SHARD_W_G2, 275}} {

@@ -1,4 +1,4 @@
-/* libb200snark — C ABI of the B200-native Groth16 / Pinocchio prove path.
+/* libb200snark — C ABI of the H100-native Groth16 / Pinocchio prove path.
  *
  * The reference (arnaucube/go-snark-study) has no FFI: its boundary is the
  * exported Go package API.  Each entry point below names the Go function(s)
@@ -56,8 +56,7 @@ int b200_version(void);
 #define B200_CFG_ACC_MODE 1
 /* B200_CFG_TMA_STAGING: the batched-affine backward pass with its operands staged into shared memory — TMA bulk
  * copies (cp.async.bulk + per-warp mbarrier) in the contiguous rounds, cp.async gathers in round 1.  0 (default) the
- * register-load kernel: measured FASTER (18.92 vs 20.17 ms per 2^20 proof, profiles/r2_notes.md: the kernel is bound by
- * the multiply pipe, not by the fetch); 1 staged in every round, 2 staged in rounds >= 2 only.  Same results.          */
+ * register-load kernel (the kernel is bound by the multiply pipe, not by the fetch); 1 staged in every round, 2 staged in rounds >= 2 only.  Same results.          */
 #define B200_CFG_TMA_STAGING 2
 /* B200_CFG_PK_CONTEXT: prove context (0 or 1) of proving keys loaded AFTERWARDS.  The two contexts own separate side
  * streams and polynomial workspaces, so a device-resident proof on a context-1 key (b200_groth16_prove_device on the
@@ -66,13 +65,13 @@ int b200_version(void);
  * `proofs_in_flight`; the keys are independent objects, each with its own tables and scratch).                       */
 #define B200_CFG_PK_CONTEXT 4
 /* B200_CFG_PAIRING_KERNEL: b200_pairing_batch with one THREAD per pairing (1: the step-by-step restatement of
- * bn128.go:179-421, ~10 ms of dependent multiplications per pairing) or one WARP per pairing (2: F_q^12 in shared
- * memory, 27 F_q^2 products of a tower multiplication on 27 lanes; csrc/pairing_warp.cuh: 3.4 ms); 0 = auto: a warp per
- * pairing up to 2048 pairings per call (latency), a thread per pairing above (462 k vs 204 k pairings/s at 2^16).
- * Bit-identical F_q^12 values.  b200_groth16_verify always runs four warps (4.2 ms per verification, was 20).          */
+ * bn128.go:179-421, a long chain of dependent multiplications per pairing) or one WARP per pairing (2: F_q^12 in shared
+ * memory, 27 F_q^2 products of a tower multiplication on 27 lanes; csrc/pairing_warp.cuh); 0 = auto: a warp per
+ * pairing up to 2048 pairings per call (latency), a thread per pairing above (throughput).
+ * Bit-identical F_q^12 values.  b200_groth16_verify always runs four warps.          */
 #define B200_CFG_PAIRING_KERNEL 5
-/* Partition tuning of SHARDED proving keys loaded afterwards (defaults = the measured best for one proof at a time,
- * profiles/r2_notes.md section 8): cost weight x100 of an A / B1 term (10) and of a G2 term (11) in C||PTD terms, and the
+/* Partition tuning of SHARDED proving keys loaded afterwards (defaults = the measured best for one proof at a time):
+ * cost weight x100 of an A / B1 term (10) and of a G2 term (11) in C||PTD terms, and the
  * smallest per-rank set that still takes the batched-affine tree, in G1 (12) / G2 (13) terms — below it the set runs
  * the XYZZ kernel, whose single launch has the shorter latency chain.  With two proofs in flight (B200_CFG_PK_CONTEXT)
  * that latency is hidden and the affine tree's 6 multiplications per add win at every shard size: set 12 and 13 to 1. */

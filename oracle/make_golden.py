@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
 """Generate tests/golden/*.json by running the REFERENCE's own prebuilt Go
-binary (/root/reference/go-snark-cli, built by build-cli.sh:3-4 from
+binary (go-snark-cli at the root of the reference tree, built by build-cli.sh:3-4 from
 cli/main.go).  Test infrastructure only.
 
-Run in the build container (the GPU box has no /root/reference):
-    python oracle/make_golden.py
+Run where a checkout of the reference exists:
+    python oracle/make_golden.py      (GOSNARK_REFERENCE overrides where the checkout is looked for, oracle/ref_binary.py)
 
 For each circuit it runs, in a scratch dir, the CLI workflow of
 cli/main.go:28-78:
@@ -25,7 +25,8 @@ import subprocess
 import sys
 import tempfile
 
-REF_BIN = "/root/reference/go-snark-cli"
+import ref_binary
+
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 CIRCUITS = {
@@ -60,10 +61,11 @@ def load(path):
 
 
 def main():
+    ref = ref_binary.require_reference_dir()
     os.makedirs(OUT, exist_ok=True)
     tmp = tempfile.mkdtemp(prefix="gsc_")
     binary = os.path.join(tmp, "gsc")
-    shutil.copy(REF_BIN, binary)
+    shutil.copy(os.path.join(ref, "go-snark-cli"), binary)
     os.chmod(binary, 0o755)
     for name, c in CIRCUITS.items():
         d = os.path.join(tmp, name)
@@ -101,7 +103,7 @@ def main():
     shutil.rmtree(tmp)
     # K8: the snarkjs-generated Groth16 fixture the reference verifies in
     # externalVerif/circomVerifier_test.go:9-13 (data files, stored verbatim).
-    cdir = "/root/reference/externalVerif/circom-test"
+    cdir = os.path.join(ref, "externalVerif", "circom-test")
     circom = {k: load(os.path.join(cdir, f)) for k, f in
               (("vk", "verification_key.json"), ("proof", "proof.json"), ("public", "public.json"))}
     with open(os.path.join(OUT, "circom_groth16.json"), "w") as f:

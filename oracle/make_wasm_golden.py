@@ -1,12 +1,13 @@
 #!/usr/bin/env python3
 """Extract the string-form fixtures of the reference's wasm demo (wasm/index.js:2-8: inputs, CircuitString, the
 Pinocchio SetupString in the older top-level-G1T layout, px strings) into tests/golden/wasm_index_strings.json.
-Run in the build container (needs /root/reference); the tests read only the committed JSON."""
+Needs a checkout of the reference (located as in oracle/ref_binary.py); the tests read only the committed JSON."""
 import json
 import os
 import re
 
-SRC = "/root/reference/wasm/index.js"
+import ref_binary
+
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "wasm_index_strings.json")
 
 
@@ -16,7 +17,7 @@ def const(src, name):
 
 
 def main():
-    src = open(SRC).read()
+    src = open(os.path.join(ref_binary.require_reference_dir(), "wasm", "index.js")).read()
     i = src.index("const inputs = ")
     inputs_txt = src[i + len("const inputs = "):src.index("};", i) + 1]
     inputs = json.loads(re.sub(r"(\w+):", r'"\1":', inputs_txt))

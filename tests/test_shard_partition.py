@@ -65,7 +65,7 @@ def test_cpp_partition_equals_python_mirror_and_tiles(cpart, w_ab, w_g2):
 
 
 def test_shard_ranges_defaults_are_the_recorded_partition():
-    """The default weights reproduce the cuts recorded in profiles/r2_scale_n8_final.json (per_rank.witness_ranges)."""
+    """The default weights reproduce the recorded cuts of the 8-rank split of a 2^20-constraint key (witness ranges)."""
     from gosnark_b200 import shard
     m = (1 << 20) + 2
     s1 = shard.shard_ranges(m, 1, (1 << 20) + 1, 1, 8)["sets"]

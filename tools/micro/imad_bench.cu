@@ -1,8 +1,13 @@
 // Microbenchmark: per-SM throughput of the integer multiply instructions the
-// Montgomery kernels are built from (B200, sm_100a).  Development aid.
+// Montgomery kernels are built from.  Development aid:
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/imad_bench tools/micro/imad_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+
+// SM count and peak SM clock of device 0 (the rates below are per SM and per clock at that peak clock).
+static int dev_sms() { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, 0); return v; }
+static double dev_clk_hz() { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrClockRate, 0); return v * 1e3; }
 
 template <int MODE>
 __global__ void k(uint32_t* out, uint32_t a0, uint32_t b0, int iters) {
@@ -41,7 +46,7 @@ __global__ void k(uint32_t* out, uint32_t a0, uint32_t b0, int iters) {
 template <int MODE>
 void run(const char* name, int ops_per_iter) {
   uint32_t* d;
-  int blocks = 148 * 4, threads = 512, iters = 20000;
+  int blocks = dev_sms() * 4, threads = 512, iters = 20000;
   cudaMalloc(&d, blocks * threads * 4);
   k<MODE><<<blocks, threads>>>(d, 3, 5, 100);
   cudaEvent_t e0, e1;
@@ -52,9 +57,8 @@ void run(const char* name, int ops_per_iter) {
   cudaEventSynchronize(e1);
   float ms; cudaEventElapsedTime(&ms, e0, e1);
   double ops = (double)blocks * threads * iters * ops_per_iter;   // thread-level ops
-  int clk; cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
-  double per_sm_clk = ops / (ms * 1e-3) / 148 / (1.965e9);
-  printf("%-28s %8.3f ms  %7.2f Tops/s  %6.1f thread-ops/clk/SM (at 1965 MHz)\n", name, ms, ops / ms / 1e9, per_sm_clk);
+  double per_sm_clk = ops / (ms * 1e-3) / dev_sms() / dev_clk_hz();
+  printf("%-28s %8.3f ms  %7.2f Tops/s  %6.1f thread-ops/clk/SM (at %.0f MHz)\n", name, ms, ops / ms / 1e9, per_sm_clk, dev_clk_hz() / 1e6);
   cudaFree(d);
 }
 

@@ -1,4 +1,4 @@
-// Microbenchmark (development aid): throughput of the two Montgomery multiplications of fp.cuh on a B200 —
+// Microbenchmark (development aid): throughput of the two Montgomery multiplications of fp.cuh —
 // mul_impl (8 x 32-bit limbs, IMAD.WIDE.U32.X carry chains) against mul29_impl (nine 29-bit limbs, carry-free IMAD.WIDE.U32) —
 // as out-of-line device functions called from a dependent chain per thread (the shape of the bucket kernels' inner loops),
 // at several occupancies, plus a bit-for-bit comparison of the two on random operands.
@@ -8,12 +8,16 @@
 #include "fp.cuh"
 using namespace b200;
 
+// SM count and peak SM clock of device 0 (the rates below are per SM and per clock at that peak clock).
+static int dev_sms() { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, 0); return v; }
+static double dev_clk_hz() { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrClockRate, 0); return v * 1e3; }
+
 // ---- the experiment: carry-free Montgomery multiplication on nine 29-bit limbs (same result as Fq::mul_impl) -------------
 // A 64-bit column accumulator holds 18 products of 29-bit limbs without overflowing, so no partial product needs a carry
 // flag.  The reduction takes eight 29-bit digits and one 24-bit digit (232 + 24 = 256: R stays 2^256); the quotient columns then
-// sit at bit offsets 5 + 29 k and are packed straight into 32-bit words.  MEASURED SLOWER (profiles/r2_notes.md section 10):
-// ptxas splits every mad.wide.u32 with a 64-bit addend into IMAD.WIDE.U32 (RZ addend) + a 3-input IADD3 / IADD3.X pair, the
-// multiplier pipe takes 4 cycles per IMAD.WIDE.U32 with or without carry flags, and 81 + 81 products replace 64 + 64.
+// sit at bit offsets 5 + 29 k and are packed straight into 32-bit words.  ptxas splits every mad.wide.u32 with a 64-bit
+// addend into IMAD.WIDE.U32 (RZ addend) + a 3-input IADD3 / IADD3.X pair, and 81 + 81 products replace 64 + 64.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I go-snark-study_b200/csrc -o tools/micro/mul29_bench tools/micro/mul29_bench.cu
 __device__ __constant__ uint32_t kQ29[9] = {0x187cfd47u, 0x010460b6u, 0x1c72a34fu, 0x02d522d0u, 0x1585d978u, 0x02db40c0u, 0x00a6e141u, 0x0e5c2634u, 0x0030644eu};
 __device__ __forceinline__ uint64_t mad_wide64(uint32_t a, uint32_t b, uint64_t c) {
   uint64_t r;
@@ -96,7 +100,7 @@ __global__ void k_cmp(const Fq* in, int n, int* bad) {
 }
 
 int main() {
-  const int max_threads = 148 * 16 * 128;
+  const int max_threads = dev_sms() * 16 * 128;
   Fq* d;
   cudaMalloc(&d, sizeof(Fq) * 2 * max_threads);
   // operands: arbitrary reduced values (top limb small)
@@ -119,7 +123,7 @@ int main() {
   for (int cta_per_sm : {2, 4, 5, 8, 12, 16}) {
     float ms[2];
     for (int v = 0; v < 2; v++) {
-      int blocks = 148 * cta_per_sm;
+      int blocks = dev_sms() * cta_per_sm;
       cudaMemcpy(d, h, sizeof(Fq) * 2 * max_threads, cudaMemcpyHostToDevice);
       if (v == 0) k_chain<0><<<blocks, 128>>>(d, 10); else k_chain<1><<<blocks, 128>>>(d, 10);
       cudaEvent_t e0, e1;
@@ -130,8 +134,8 @@ int main() {
       cudaEventSynchronize(e1);
       cudaEventElapsedTime(&ms[v], e0, e1);
     }
-    double muls = 148.0 * cta_per_sm * 128 * iters * 2;
-    auto cyc = [&](float m) { return m * 1e-3 * 1.965e9 * 148 * 4 / (muls / 32); };   // SMSP-cycles per warp-level multiply
+    double muls = (double)dev_sms() * cta_per_sm * 128 * iters * 2;
+    auto cyc = [&](float m) { return m * 1e-3 * dev_clk_hz() * dev_sms() * 4 / (muls / 32); };   // SMSP-cycles per warp-level multiply
     printf("%2d CTAs/SM (%2d warps/SMSP): mul_impl %7.3f ms = %5.0f SMSP-cycles/warp-mul (%.1f Gmul/s)   mul29_impl %7.3f ms = %5.0f (%.1f Gmul/s)   x%.2f\n",
            cta_per_sm, cta_per_sm, ms[0], cyc(ms[0]), muls / ms[0] / 1e6, ms[1], cyc(ms[1]), muls / ms[1] / 1e6, ms[0] / ms[1]);
   }

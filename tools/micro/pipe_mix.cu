@@ -1,4 +1,4 @@
-// Microbenchmark (development aid, B200 sm_100a): do the integer-multiply pipe (IMAD.WIDE.X carry chains — what the
+// Microbenchmark (development aid; nvcc -gencode arch=compute_90a,code=sm_90a -O3): do the integer-multiply pipe (IMAD.WIDE.X carry chains — what the
 // Montgomery kernels are made of) and the FP64 pipe (DFMA, the Emmart-style 52-bit-limb route) + the ALU pipe (64-bit
 // integer adds of the DFMA results) run CONCURRENTLY when different warps of an SM execute them?
 //   mode 0: every warp runs the IMAD.WIDE.X chain        mode 1: every warp runs DFMA(+DADD) + int64 adds
@@ -8,6 +8,10 @@
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+
+// SM count and peak SM clock of device 0 (the rates below are per SM and per clock at that peak clock).
+static int dev_sms() { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, 0); return v; }
+static double dev_clk_hz() { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrClockRate, 0); return v * 1e3; }
 
 __device__ __forceinline__ void imad_chain(uint32_t (&r)[8], uint32_t a, uint32_t& b) {
   asm volatile(
@@ -85,7 +89,7 @@ __global__ void __launch_bounds__(512) k(uint32_t* out, uint32_t a0, double d0, 
 }
 
 float run(int mode, int iters, uint32_t* d) {
-  int blocks = 148 * 4, threads = 512;
+  int blocks = dev_sms() * 4, threads = 512;
   k<<<blocks, threads>>>(d, 3, 5.0, 64, mode);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -99,12 +103,12 @@ float run(int mode, int iters, uint32_t* d) {
 
 int main() {
   uint32_t* d;
-  cudaMalloc(&d, 148 * 4 * 512 * 4);
+  cudaMalloc(&d, dev_sms() * 4 * 512 * 4);
   const int iters = 20000;
-  const double warps = 148.0 * 4 * 16, clk = 1.965e9;
+  const double sms = dev_sms(), warps = sms * 4 * 16, clk = dev_clk_hz();
   float t0 = run(0, iters, d), t1 = run(1, iters, d), t2 = run(2, iters, d), t3 = run(3, iters, d), t4 = run(4, iters, d), t5 = run(5, iters, d);
   // per-SMSP cycles per warp-instruction group
-  auto cyc = [&](float ms, double warp_ops) { return ms * 1e-3 * clk * 148 * 4 / warp_ops; };
+  auto cyc = [&](float ms, double warp_ops) { return ms * 1e-3 * clk * sms * 4 / warp_ops; };
   printf("mode 0 IMAD.WIDE.X chains      %8.3f ms   %.2f SMSP-cycles per wide MAC warp-instr (8 per iteration)\n", t0, cyc(t0, warps * iters * 8));
   printf("mode 5 IMAD.WIDE (no carry)    %8.3f ms   %.2f SMSP-cycles per wide MAC warp-instr (8 per iteration)\n", t5, cyc(t5, warps * iters * 8));
   printf("mode 3 DFMA only               %8.3f ms   %.2f SMSP-cycles per DFMA warp-instr (8 + 2 DMUL per iteration)\n", t3, cyc(t3, warps * iters * 10));

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Stand-alone G1 MSM either side of the slice-size step of bases_create (development aid, profiles/r2_notes.md section 16):
+"""Stand-alone G1 MSM either side of the slice-size step of bases_create (development aid):
 at c = 17 the mean bucket population crosses 192 at 838 861 terms — below it S = 16, above it S = 32."""
 import sys
 
