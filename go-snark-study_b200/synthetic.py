@@ -160,29 +160,51 @@ class SyntheticCircuit:
         return out
 
 
-class CircuitGroth16(SyntheticGroth16):
+class CircuitQAP:
+    """What a real trusted setup of SyntheticCircuit(n) starts from, shared by CircuitGroth16 and CircuitPinocchio: the R1CS
+    resident on the device, the satisfying witness (limbs in ``w``), Z = prod_{i=1..n}(x - i) (groth16.go:122-132,
+    snark.go:210-221), and the QAP evaluated at the toxic T for every signal — at_s / bt_s / ct_s = Eval(alphas[i], T) etc.
+    through the sparse A^T l(T) of b200_qap_eval_at, and zt = Z(T) — as Python ints.  Any n >= 2."""
+
+    def __init__(self, n, t):
+        from .r1csqap import SparseR1CS
+        assert n >= 2
+        self.n, self.m, self.npublic = n, n + 2, 1
+        self.logn = n.bit_length() - 1 if n & (n - 1) == 0 else None
+        self.circuit = SyntheticCircuit(n)
+        self.r1cs = SparseR1CS(n, self.m, self.circuit.csr)
+        at_l, bt_l, ct_l, self.zt = self.r1cs.EvalAt(t)
+        self.at_s, self.bt_s, self.ct_s = limbs_to_ints(at_l), limbs_to_ints(bt_l), limbs_to_ints(ct_l)
+        self.w = ints_to_limbs(self.circuit.witness)
+        self.z = np.zeros((n + 1, 4), dtype=np.uint64)
+        check(lib().b200_zero_poly(n, ptr(self.z)))
+
+    def px_of(self, w_limbs):
+        """px = A(x) B(x) - C(x) of a witness of this R1CS (r1csqap.go:191-210), from the sparse front end (b200_qap_px)."""
+        return self.r1cs.combine_limbs(w_limbs, want_abc=False)[3]
+
+
+def _size(logn, n):
+    assert (logn is None) != (n is None), "give logn or n"
+    return 1 << logn if n is None else n
+
+
+class CircuitGroth16(CircuitQAP, SyntheticGroth16):
     """A REAL Groth16 instance at benchmark sizes: SyntheticCircuit's R1CS, a satisfying witness, and the CRS that
     groth16.GenerateTrustedSetup (groth16/groth16.go:94-222) yields for seeded toxic values — every point is still
-    k*G with a known k (k = Eval(alphas[i], tau) etc., obtained through the sparse A^T l(tau) of b200_qap_eval_at), so
+    k*G with a known k (k = Eval(alphas[i], tau) etc., see CircuitQAP), so
     the known-discrete-log parity check of SyntheticGroth16 keeps working AND the proof verifies under the real Vk.
     px comes from the sparse QAP front end (b200_qap_px); the expected proof is computed in the exponent from the QAP
-    identity  h(tau) Z(tau) = A(tau) B(tau) - C(tau)  — independently of the GPU's px and h."""
+    identity  h(tau) Z(tau) = A(tau) B(tau) - C(tau)  — independently of the GPU's px and h.  Sized by 2^logn or by n."""
 
-    def __init__(self, logn, mint=True):
-        from .r1csqap import SparseR1CS
-        self.logn = logn
-        n = self.n = 1 << logn
-        m = self.m = n + 2
-        self.npublic = 1
-        self.n_ptd = m - 1
-        self.circuit = SyntheticCircuit(n)
-        self.r1cs = SparseR1CS(n, m, self.circuit.csr)
+    def __init__(self, logn=None, mint=True, n=None):
         tox = [x % R for x in limbs_to_ints(rand_limbs(5, SEED_TOXIC))]
         self.toxic = dict(zip(("T", "Kalpha", "Kbeta", "Kgamma", "Kdelta"), tox))
         t, ka, kb, kg, kd = tox
-        at_l, bt_l, ct_l, zt = self.r1cs.EvalAt(t)
-        at, bt, ct = limbs_to_ints(at_l), limbs_to_ints(bt_l), limbs_to_ints(ct_l)
-        self.at_s, self.bt_s, self.ct_s, self.zt = at, bt, ct, zt
+        super().__init__(_size(logn, n), t)
+        m = self.m
+        self.n_ptd = m - 1
+        at, bt, ct, zt = self.at_s, self.bt_s, self.ct_s, self.zt
         inv_d, inv_g = pow(kd, -1, R), pow(kg, -1, R)
         l1 = self.npublic + 1
         kc = [0] * l1 + [inv_d * ((at[i] * kb + bt[i] * ka + ct[i]) % R) % R for i in range(l1, m)]      # :181-200
@@ -193,11 +215,8 @@ class CircuitGroth16(SyntheticGroth16):
             cur = cur * t % R
         self.k_at, self.k_b, self.k_c, self.k_ptd = (ints_to_limbs(v) for v in (at, bt, kc, ptd))
         self.k_alpha, self.k_beta, self.k_delta, self.k_gamma = (ints_to_limbs([v]) for v in (ka, kb, kd, kg))
-        self.w = ints_to_limbs(self.circuit.witness)
         rs = limbs_to_ints(rand_limbs(2, SEED_RS))
         self.r, self.s = rs[0] >> 13, rs[1] >> 13
-        self.z = np.zeros((n + 1, 4), dtype=np.uint64)
-        check(lib().b200_zero_poly(n, ptr(self.z)))                  # Z = prod_{i=1..m-2}(x - i), groth16.go:122-132
         if mint:
             self.mint()
 
@@ -210,7 +229,7 @@ class CircuitGroth16(SyntheticGroth16):
         self.alpha1, self.beta1, self.delta1 = (mint_points(1, k) for k in (self.k_alpha, self.k_beta, self.k_delta))
         self.beta2, self.delta2, self.gamma2 = (mint_points(2, k) for k in (self.k_beta, self.k_delta, self.k_gamma))
         self.ic = mint_points(1, ints_to_limbs(self.k_ic))
-        _, _, _, self.px = self.r1cs.combine_limbs(self.w, want_abc=False)
+        self.px = self.px_of(self.w)
 
     def expected_dlogs(self):
         w = self.circuit.witness
@@ -239,3 +258,88 @@ class CircuitGroth16(SyntheticGroth16):
         check(lib().b200_groth16_verify(ptr(self.ic), self.npublic + 1, ptr(self.alpha1), ptr(self.beta2), ptr(self.gamma2),
                                         ptr(self.delta2), ptr(pi_a), ptr(pi_b), ptr(pi_c), ptr(pub), 1, ctypes.byref(ok)))
         return bool(ok.value)
+
+
+PINOCCHIO_TOXIC = ("T", "Ka", "Kb", "Kc", "Kbeta", "Kgamma", "RhoA", "RhoB")
+
+
+def pinocchio_toxic(seed=SEED_TOXIC):
+    """Seeded toxic values of snark.GenerateTrustedSetup (snark.go:98-251), keyed as its Toxic struct (RhoC is derived)."""
+    return dict(zip(PINOCCHIO_TOXIC, (x % R for x in limbs_to_ints(rand_limbs(len(PINOCCHIO_TOXIC), seed)))))
+
+
+def pinocchio_key_dlogs(at, bt, ct, zt, toxic, npublic):
+    """Discrete logs (w.r.t. the generators) of every point of the Pinocchio key and Vk that snark.GenerateTrustedSetup
+    (snark.go:98-251) makes from at / bt / ct = Eval(alphas[i], T) etc. over all signals and zt = Z(T).  Pure ints:
+    A, Ap, Bp, C, Cp, Kp, G1T and Vkb, G1Kbg are in G1; B and Vka, Vkc, G2Kbg, G2Kg, Vkz in G2; IC = A[0..NPublic]."""
+    t, ka, kb, kc, kbeta, kgamma, rho_a, rho_b = (toxic[k] % R for k in PINOCCHIO_TOXIC)
+    rho_c = rho_a * rho_b % R                                    # :150
+    kbg = kbeta * kgamma % R
+    a = [rho_a * x % R for x in at]                              # :171-207
+    b = [rho_b * x % R for x in bt]
+    c = [rho_c * x % R for x in ct]
+    g1t, cur = [], 1                                             # G1T[j] = T^j, j = 0 .. len(Z) - 1 (:230-237)
+    for _ in range(len(at) - 1):
+        g1t.append(cur)
+        cur = cur * t % R
+    return {"A": a, "Ap": [ka * x % R for x in a], "B": b, "Bp": [kb * x % R for x in b], "C": c,
+            "Cp": [kc * x % R for x in c], "Kp": [kbeta * (x + y + z) % R for x, y, z in zip(a, b, c)], "G1T": g1t,
+            "Vka": ka, "Vkb": kb, "Vkc": kc, "G1Kbg": kbg, "G2Kbg": kbg, "G2Kg": kgamma, "Vkz": rho_c * zt % R,
+            "IC": a[:npublic + 1]}
+
+
+def pinocchio_proof_dlogs(at, bt, ct, zt, toxic, npublic, w):
+    """Discrete logs of the eight elements snark.GenerateProofs (snark.go:254-289) returns for witness w under the key of
+    pinocchio_key_dlogs, from the QAP identity  h(T) Z(T) = A(T) B(T) - C(T)  (A(T) = sum over ALL signals of w_i at_i),
+    independently of px and of the quotient h."""
+    _, ka, kb, kc, kbeta, _, rho_a, rho_b = (toxic[k] % R for k in PINOCCHIO_TOXIC)
+    rho_c = rho_a * rho_b % R
+    dot = lambda ks, lo=0: sum(k * x for k, x in zip(ks[lo:], w[lo:])) % R
+    A, B, C = dot(at), dot(bt), dot(ct)
+    pi_a = rho_a * dot(at, npublic + 1) % R                      # public signals excluded, :265-268
+    return {"PiA": pi_a, "PiAp": ka * pi_a % R, "PiB": rho_b * B % R, "PiBp": kb * rho_b * B % R, "PiC": rho_c * C % R,
+            "PiCp": kc * rho_c * C % R, "PiH": (A * B - C) * pow(zt, -1, R) % R,
+            "PiKp": kbeta * (rho_a * A + rho_b * B + rho_c * C) % R}
+
+
+class CircuitPinocchio(CircuitQAP):
+    """A REAL Pinocchio instance at benchmark sizes (any n >= 2): SyntheticCircuit's R1CS and witness, and the key and Vk
+    that snark.GenerateTrustedSetup (snark.go:98-251) yields for seeded toxic values.  Every point is k*G with k from
+    pinocchio_key_dlogs, minted on the GPU; the expected proof comes from pinocchio_proof_dlogs.  Key arrays are Jacobian
+    limbs in ``pk`` (A, Ap, B (G2), Bp, C, Cp, Kp, G1T), the Vk is a snark.VerifyProof dict of points in ``vk``."""
+
+    def __init__(self, n, mint=True):
+        self.toxic = pinocchio_toxic()
+        super().__init__(n, self.toxic["T"])
+        self.k = pinocchio_key_dlogs(self.at_s, self.bt_s, self.ct_s, self.zt, self.toxic, self.npublic)
+        if mint:
+            self.mint()
+
+    def mint(self):
+        from .bn128 import _unflatten_g1, _unflatten_g2
+        k = self.k
+        self.pk = {s: mint_points(2 if s == "B" else 1, ints_to_limbs(k[s])) for s in ("A", "Ap", "B", "Bp", "C", "Cp", "Kp", "G1T")}
+        g1 = ("Vkb", "G1Kbg")
+        g2 = ("Vka", "Vkc", "G2Kbg", "G2Kg", "Vkz")
+        self.vk = dict(zip(g1, _unflatten_g1(mint_points(1, ints_to_limbs([k[s] for s in g1])))))
+        self.vk.update(zip(g2, _unflatten_g2(mint_points(2, ints_to_limbs([k[s] for s in g2])))))
+        self.vk["IC"] = _unflatten_g1(self.pk["A"][: self.npublic + 1])
+        self.px = self.px_of(self.w)
+
+    def load_pk(self, rank=0, world=1, window_bits=0):
+        p = self.pk
+        h = _lib._h(0)
+        check(lib().b200_pinocchio_pk_load_shard(
+            ptr(p["A"]), ptr(p["Ap"]), ptr(p["B"]), ptr(p["Bp"]), ptr(p["C"]), ptr(p["Cp"]), ptr(p["Kp"]), self.m,
+            ptr(p["G1T"]), p["G1T"].shape[0], ptr(self.z), self.n + 1, self.npublic, window_bits, rank, world, h))
+        return h.value
+
+    def expected_dlogs(self, witness=None):
+        """Discrete logs of PiA .. PiKp, PiB for ``witness`` (ints; this instance's own unless given)."""
+        w = self.circuit.witness if witness is None else witness
+        return pinocchio_proof_dlogs(self.at_s, self.bt_s, self.ct_s, self.zt, self.toxic, self.npublic, w)
+
+    def verify(self, proof, public=None):
+        """snark.VerifyProof (snark.go:292-372) on the GPU against this instance's Vk."""
+        from . import snark
+        return snark.VerifyProof(self.vk, proof, self.circuit.public_signals if public is None else public)

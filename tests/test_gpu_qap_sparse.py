@@ -160,17 +160,19 @@ def go_groth16_verify(vk_json, proof_json, public):
         shutil.rmtree(d)
 
 
-@pytest.mark.parametrize("logn", [6, 10, 16])
-def test_real_crs_witness_to_verified_proof(mods, logn):
+@pytest.mark.timeout(600)
+@pytest.mark.parametrize("n", [1 << 6, 1 << 10, 1 << 16, (1 << 12) + 2], ids=["6", "10", "16", "4098"])   # log2 n for 2^k
+def test_real_crs_witness_to_verified_proof(mods, n):
     """Config 2 end to end with a REAL CRS (groth16.go:94-222 semantics, toxic values seeded): witness -> px on the device
     -> proof; the proof equals the one the reference's GenerateProofs would return (known discrete logs, from the QAP
     identity, independent of the GPU's px / h), verifies under the real Vk on the GPU (groth16.go:281-305) and — the
-    reference's own Go code — under `go-snark-cli groth16 verify`; a wrong public input is rejected."""
+    reference's own Go code — under `go-snark-cli groth16 verify`; a wrong public input is rejected.  n = 2^12 + 2: the
+    quotient has 2^12 + 1 coefficients, so the division and the interpolation both cross a power of two."""
     import ctypes
     from gosnark_b200._lib import check, ints_to_limbs, lib, limbs_to_ints, ptr
     from gosnark_b200.bn128 import _unflatten_g1, _unflatten_g2
     from gosnark_b200.synthetic import CircuitGroth16
-    syn = CircuitGroth16(logn)
+    syn = CircuitGroth16(n=n)
     pk = syn.load_pk()
     rr, ss = ints_to_limbs([syn.r]), ints_to_limbs([syn.s])
     outs = []
