@@ -168,6 +168,9 @@ struct Bases {
   // batched-affine accumulation (affine_S > 0): ping-pong node buffers, prefix products, per-thread / per-block products
   uint32_t affine_S = 0;
   DevBuf nodeA, nodeB, aff_pre, aff_others, aff_btot, aff_ids;
+  // error word of b200_msm_device on this set: written by the kernels, never read (the call cannot wait for it, and a
+  // later call on any object must not report it; see b200snark.h).  Host-pointer MSMs use g_d_err.
+  DevBuf d_err;
 };
 
 int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
@@ -270,6 +273,8 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   CU(b->partials.alloc(((size_t)b->nseg + 1024) * sizeof(XYZZ<F>)));
   CU(b->result.alloc(sizeof(XYZZ<F>)));
   CU(b->out_std.alloc(3 * sizeof(F)));
+  CU(b->d_err.alloc(sizeof(int)));
+  CU(cudaMemset(b->d_err.p, 0, sizeof(int)));
 
   // upload + normalise + window precompute
   DevBuf staging, state;
@@ -365,8 +370,9 @@ void launch_bucket_tail(const XYZZ<F>* buckets, uint32_t c, XYZZ<F>* scratch, XY
   g_launches += 3;
 }
 
-// Front end: signed-digit recode + counting sort of n scalars into bucket order (3 launches).
-int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, cudaStream_t st) {
+// Front end: signed-digit recode + counting sort of n scalars into bucket order (3 launches).  A standard-form scalar
+// >= r is read as 0 and sets bit 1 of *err.
+int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, int* err, cudaStream_t st) {
   if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride)
     return fail(B200_EINVAL, "msm_sort: shape mismatch");
   MsmShape sh = shape;
@@ -382,11 +388,11 @@ int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t
   }
   uint32_t* counts = ss.counts.as<uint32_t>();
   CU(cudaMemsetAsync(counts, 0, (m + 1) * sizeof(uint32_t), st));
-  if (n) k_digits_count<<<nblocks(n, 256), 256, 0, st>>>(d_scalars, sh, mont, counts, g_d_err);
+  if (n) k_digits_count<<<nblocks(n, 256), 256, 0, st>>>(d_scalars, sh, mont, counts, err);
   k_scan<<<1, 1024, 0, st>>>(counts, m, cap, fixed, ss.offsets.as<uint32_t>(), ss.cursor.as<uint32_t>(), ss.tables());
   k_fill_slices<<<nblocks(m, 256), 256, 0, st>>>(counts, ss.offsets.as<uint32_t>(), m, cap, fixed, ss.tables());
   if (n) k_digits_scatter<<<nblocks(n, 256), 256, 0, st>>>(d_scalars, sh, mont, ss.cursor.as<uint32_t>(),
-                                                           ss.entries.as<uint32_t>(), g_d_err);
+                                                           ss.entries.as<uint32_t>(), err);
   g_launches += n ? 4 : 2;
   CU(cudaGetLastError());
   return B200_OK;
@@ -496,9 +502,9 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
 }
 
 template <class F>
-int msm_enqueue(Bases* b, const Fr* d_scalars, size_t n, int mont, XYZZ<F>* d_out, cudaStream_t st) {
+int msm_enqueue(Bases* b, const Fr* d_scalars, size_t n, int mont, XYZZ<F>* d_out, int* err, cudaStream_t st) {
   if (n > b->n) return fail(B200_EINVAL, "msm: n=%zu exceeds base set size %zu", n, b->n);
-  int rc = msm_sort(b->sort, b->sh, d_scalars, n, mont, st);
+  int rc = msm_sort(b->sort, b->sh, d_scalars, n, mont, err, st);
   if (rc) return rc;
   return msm_buckets<F>(b, b->sort, n, d_out, st);
 }
@@ -509,7 +515,7 @@ int msm_host(b200_bases_t h, int group, const uint64_t* scalars, size_t n, uint6
   if (!b) return fail(B200_EINVAL, "msm: bad handle");
   if ((!scalars && n) || !out) return fail(B200_EINVAL, "msm: null pointer");
   if (n) CU(cudaMemcpyAsync(b->scalars.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  int rc = msm_enqueue<F>(b, b->scalars.as<Fr>(), n, 0, b->result.as<XYZZ<F>>(), g_stream);
+  int rc = msm_enqueue<F>(b, b->scalars.as<Fr>(), n, 0, b->result.as<XYZZ<F>>(), g_d_err, g_stream);
   if (rc) return rc;
   k_finalize<F><<<1, 32, 0, g_stream>>>(b->result.as<XYZZ<F>>(), b->out_std.as<F>());
   CU(cudaMemcpyAsync(out, b->out_std.p, 3 * sizeof(F), cudaMemcpyDeviceToHost, g_stream));
@@ -628,11 +634,13 @@ int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t
     CU(pk->h_full.ensure((pk->m + pk->n_h_bases + 4) * sizeof(Fr)));
     rc = qap_h_enqueue(rc1, pk->w_stage.as<Fr>(), pk->h_full.as<Fr>(), sq);
     if (rc) return rc;
-    rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, rc1->px_mont.as<Fr>(), 2 * rc1->n - 1, r, s, o, st, 1, pk->h_full.as<Fr>());
+    rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, rc1->px_mont.as<Fr>(), 2 * rc1->n - 1, r, s, o, st, g_d_err, 1,
+                         pk->h_full.as<Fr>());
   } else {
     rc = qap_px_enqueue(rc1, pk->w_stage.as<Fr>(), nullptr, nullptr, sq);
     if (rc) return rc;
-    rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, rc1->px_mont.as<Fr>(), 2 * rc1->n - 1, r, s, o, st, /*px_mont=*/1);
+    rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, rc1->px_mont.as<Fr>(), 2 * rc1->n - 1, r, s, o, st, g_d_err,
+                         /*px_mont=*/1);
   }
   if (rc) return rc;
   uint64_t host_out[48];
@@ -1113,7 +1121,7 @@ int b200_groth16_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const vo
   ProvingKey* p = find_pk(pk, 1);
   if (!p || !d_w || !d_px || !r || !s || !d_out) return fail(B200_EINVAL, "groth16_prove_device: bad arguments");
   return drain_on_error(groth16_enqueue(p, (const Fr*)d_w, nw, (const Fr*)d_px, npx, r, s, (Fq*)d_out,
-                         stream ? (cudaStream_t)stream : g_stream));
+                         stream ? (cudaStream_t)stream : g_stream, p->d_err.as<int>()));
 }
 int b200_comm_unique_id(uint8_t out[128]) {
   std::lock_guard<std::mutex> lk(g_mu);
@@ -1398,8 +1406,9 @@ int b200_msm_device(b200_bases_t h, const void* d_scalars, size_t n, int mont, v
   Bases* b = find_bases(h, 0);
   if (!b || !d_out || (!d_scalars && n)) return fail(B200_EINVAL, "msm_device: bad arguments");
   cudaStream_t st = stream ? (cudaStream_t)stream : g_stream;
-  if (b->group == 1) return msm_enqueue<Fq>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq>*)d_out, st);
-  return msm_enqueue<Fq2>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq2>*)d_out, st);
+  int* err = b->d_err.as<int>();
+  if (b->group == 1) return msm_enqueue<Fq>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq>*)d_out, err, st);
+  return msm_enqueue<Fq2>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq2>*)d_out, err, st);
 }
 
 int b200_g1_sum_partials(const void* d, size_t count, uint64_t out[12], void* stream) {

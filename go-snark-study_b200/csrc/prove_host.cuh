@@ -59,6 +59,9 @@ struct ProvingKey {
   DevBuf res;          // XYZZ results (8 x 256 B)
   DevBuf out_std;      // standard-form Jacobian outputs
   DevBuf rs;           // r, s on device (standard form)
+  // error word of b200_groth16_prove_device on this key: written by the kernels, never read (see b200snark.h), so an
+  // out-of-range input of one device-resident proof is reported by no later call and never by a proof on another key
+  DevBuf d_err;
 };
 
 std::map<uint64_t, std::unique_ptr<ProvingKey>> g_pks;
@@ -147,6 +150,8 @@ int pk_common_init(ProvingKey& pk, const uint64_t* z, size_t nz, size_t m) {
   CU(pk.res.alloc(8 * 256));
   CU(pk.out_std.alloc(64 * sizeof(Fq)));
   CU(pk.rs.alloc(8 * sizeof(Fr)));
+  CU(pk.d_err.alloc(sizeof(int)));
+  CU(cudaMemset(pk.d_err.p, 0, sizeof(int)));
   for (auto& e : pk.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   CU(cudaHostAlloc(reinterpret_cast<void**>(&pk.h_out), 64 * sizeof(uint64_t), cudaHostAllocDefault));
   return check_err_flag<Fr>("pk_load(Z)");
@@ -276,9 +281,10 @@ __global__ void k_groth16_combine(const uint8_t* res, const XYZZ<Fq>* prod, Fq* 
 
 // Enqueue one Groth16 proof on `st` from DEVICE-resident witness / px (standard
 // form).  d_out receives PiA (3 Fq) | PiC (3 Fq) | PiB (3 Fq2) in standard form
-// (or, for a sharded key, the 1 KB partial record).  No host synchronisation.
+// (or, for a sharded key, the 1 KB partial record).  No host synchronisation.  A witness entry or px coefficient >= r
+// is read as 0 and sets bit 1 of *err.
 int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, size_t npx, const uint64_t* r,
-                    const uint64_t* s, Fq* d_out, cudaStream_t st, int px_mont = 0, const Fr* d_h_std = nullptr) {
+                    const uint64_t* s, Fq* d_out, cudaStream_t st, int* err, int px_mont = 0, const Fr* d_h_std = nullptr) {
   // d_h_std != nullptr: the quotient h (npx - len(Z) + 1 coefficients, standard form, device) is supplied by the caller
   // (witness path: qap_h_enqueue on side stream 3) and the division is skipped; d_px is then unused.
   size_t m = pk->m;
@@ -336,13 +342,13 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
       Fr* h_dst = direct ? sCH + n_c : pk->h_full.as<Fr>();
       if (!direct && !pk->h_full.p) CU(pk->h_full.alloc((pk->m + pk->n_h_bases + 4) * sizeof(Fr)));
       if (d_h_std) CU(cudaMemcpyAsync(h_dst, d_h_std, nq * sizeof(Fr), cudaMemcpyDeviceToDevice, s3));
-      else CU(poly_div_device(pk->poly(), pk->Z, d_px, npx, px_mont, h_dst, nullptr, g_d_err, s3));
+      else CU(poly_div_device(pk->poly(), pk->Z, d_px, npx, px_mont, h_dst, nullptr, err, s3));
       size_t have = nq > p_lo ? (nq < p_hi ? nq - p_lo : n_p) : 0;   // valid h coefficients inside [p_lo, p_hi)
       if (!direct && have)
         CU(cudaMemcpyAsync(sCH + n_c, pk->h_full.as<Fr>() + p_lo, have * sizeof(Fr), cudaMemcpyDeviceToDevice, s3));
       if (n_p > have) CU(cudaMemsetAsync(sCH + n_c + have, 0, (n_p - have) * sizeof(Fr), s3));
     }
-    if ((rc = msm_enqueue<Fq>(pk->g[3].get(), sCH, nterm[3], 0, reinterpret_cast<XYZZ<Fq>*>(res + 768), s3))) return rc;
+    if ((rc = msm_enqueue<Fq>(pk->g[3].get(), sCH, nterm[3], 0, reinterpret_cast<XYZZ<Fq>*>(res + 768), err, s3))) return rc;
   }
   EV_REC(e_ch, s3);
   // --- A, B1, B2.  Sets that consume identical scalar slices (all three on one GPU; A and B1 on a rank that
@@ -354,7 +360,7 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
   cudaEvent_t e_sorted[3] = {e_w, pk->ev[7], e_prod};   // e_prod is re-recorded later; safe: waits are enqueued first
   for (int k = 0; k < 3; k++) {
     if (!pk->g[k] || pk->sort_src[k] != k) continue;
-    if ((rc = msm_sort(pk->g[k]->sort, pk->g[k]->sh, sv[k], nterm[k], 0, st))) return rc;
+    if ((rc = msm_sort(pk->g[k]->sort, pk->g[k]->sh, sv[k], nterm[k], 0, err, st))) return rc;
     EV_REC(e_sorted[k], st);
   }
   for (int k = 2; k >= 0; k--) {   // B2 first: it is the longest
@@ -464,7 +470,7 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
                        cudaMemcpyHostToDevice, g_serial ? st : pk->side()[2]));
   }
   Fq* o = pk->out_std.as<Fq>();
-  int rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st);
+  int rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st, g_d_err);
   if (rc) return rc;
   uint64_t* host_out = pk->h_out;
   CU(cudaMemcpyAsync(host_out, o, 48 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -591,7 +597,7 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
     used[2] = true;
     EV_WAIT(s3, e_in);
     CU(poly_div_device(pk->poly(), pk->Z, pk->px.as<Fr>(), npx, 0, dh, nullptr, g_d_err, s3));
-    if ((rc = msm_enqueue<Fq>(pk->g[7].get(), dh, nq, 0, slot_g1(7), s3))) return rc;
+    if ((rc = msm_enqueue<Fq>(pk->g[7].get(), dh, nq, 0, slot_g1(7), g_d_err, s3))) return rc;
   }
   // two scalar vectors: w[l+1..m) feeds PiA, PiAp (snark.go:265-268); w feeds PiB, PiBp, PiC, PiCp, PiKp (:270-278).
   // Per vector ONE digit sort (held by the first owned set of the group), the bucket phases fan out over the streams.
@@ -603,7 +609,7 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
     if (holder[gi] < 0) continue;
     const Fr* sc = gi == 0 ? dw + l1 : dw;
     const size_t cnt = gi == 0 ? m - l1 : m;
-    if ((rc = msm_sort(pk->g[holder[gi]]->sort, pk->g[holder[gi]]->sh, sc, cnt, 0, st))) return rc;
+    if ((rc = msm_sort(pk->g[holder[gi]]->sort, pk->g[holder[gi]]->sh, sc, cnt, 0, g_d_err, st))) return rc;
     EV_REC(e_sorted[gi], st);
   }
   for (int gi = 1; gi >= 0; gi--) {   // the larger group first

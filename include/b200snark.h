@@ -107,11 +107,20 @@ int b200_g2_msm(b200_bases_t h, const uint64_t* scalars, size_t n, uint64_t out_
  * XYZZ record (4 field elements, Montgomery form; 128 B for G1, 256 B for G2)
  * on `stream` (a cudaStream_t, may be NULL).  No host synchronisation.  Used by
  * the prove pipeline, by bench.py's device-resident timing and by the
- * multi-GPU path (each rank's partial record is what the NCCL gather moves).  */
+ * multi-GPU path (each rank's partial record is what the NCCL gather moves).
+ * Record layout: X | Y | ZZ | ZZZ, each F_q element 4 little-endian uint64 limbs
+ * (F_q^2: c0 then c1), Montgomery form (value * 2^256 mod q); x = X/ZZ, y = Y/ZZZ,
+ * ZZ^3 = ZZZ^2; ZZ = 0 is the point at infinity (n = 0 gives it).  n > the set's
+ * size returns B200_EINVAL.
+ * Scalars are not range-checked here: the call does not wait for the device,
+ * so it cannot return B200_ERANGE.  With scalars_mont = 0 a scalar >= r is read
+ * as 0, and neither this call nor any later one reports it.  With
+ * scalars_mont != 0 any 256-bit value v is accepted and read as v * 2^-256 mod r. */
 int b200_msm_device(b200_bases_t h, const void* d_scalars, size_t n, int scalars_mont,
                     void* d_out_xyzz, void* stream);
 /* Sum `count` XYZZ partial records (device memory, e.g. the gathered per-rank
- * partials) and normalise: out_jac = (x, y, 1) in standard form on the host.  */
+ * partials) and normalise: out_jac = (x, y, 1) in standard form on the host,
+ * infinity as all-zero.  1 <= count <= 2^20, else B200_EINVAL.  Synchronises `stream`. */
 int b200_g1_sum_partials(const void* d_xyzz, size_t count, uint64_t out_jac[12], void* stream);
 int b200_g2_sum_partials(const void* d_xyzz, size_t count, uint64_t out_jac[24], void* stream);
 
@@ -154,7 +163,10 @@ int b200_groth16_prove(b200_pk_t pk, const uint64_t* w, size_t nw, const uint64_
                        uint64_t pi_c[12]);
 /* Same with the witness and px already resident in DEVICE memory (standard form)
  * and the 48-u64 result (PiA | PiC | PiB) left in device memory on `stream`; no
- * host synchronisation.  This is the region bench.py times as `value`.            */
+ * host synchronisation.  This is the region bench.py times as `value`.
+ * As in b200_msm_device, a witness entry or a px coefficient >= r is read as 0,
+ * and neither this call nor any later one reports it (nor a proof on another
+ * key).  r and s are host values and are checked (B200_ERANGE).                   */
 int b200_groth16_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const void* d_px, size_t npx,
                               const uint64_t r[4], const uint64_t s[4], void* d_out, void* stream);
 /* Multi-GPU (one process per GPU): rank `rank` of `world` keeps the contiguous
