@@ -90,6 +90,7 @@ _SIGNATURES = {
     "b200_qap_eval_at": [_h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_interpolate": [_vp, _sz, _vp],
     "b200_groth16_prove_witness": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp, _vp],
+    "b200_groth16_prove_witness_device": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_profile": [_int],
     "b200_profile_read": [ctypes.POINTER(ctypes.c_double)],
 }

@@ -605,52 +605,52 @@ int poly_div_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, ui
 
 #include "qap_sparse_host.cuh"
 
-// groth16.GenerateProofs fed from the witness: px = CombinePolynomials(w, R1CSToQAP(a, b, c)) is computed on the device
-// from the resident sparse R1CS (never leaving HBM) and handed to the same prove pipeline.
-int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, const uint64_t* r, const uint64_t* s,
-                          uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c) {
-  ProvingKey* pk = find_pk(h, 1);
-  R1cs* rc1 = find_r1cs(hr);
-  if (!pk || !rc1) return fail(B200_EINVAL, "groth16_prove_witness: bad handle");
-  if (!w || !r || !s || !pi_a || !pi_b || !pi_c) return fail(B200_EINVAL, "groth16_prove_witness: null pointer");
-  if (nw != pk->m || nw != rc1->m) return fail(B200_EINVAL, "groth16_prove_witness: witness length %zu, NVars %zu, R1CS columns %zu", nw, pk->m, rc1->m);
-  if (pk->world != 1) return fail(B200_EINVAL, "groth16_prove_witness: sharded key");
-  cudaStream_t st = g_stream;
-  CU(pk->w_stage.ensure(nw * sizeof(Fr)));
-  CU(cudaMemcpyAsync(pk->w_stage.p, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
-  // px is only consumed by the division, which groth16_enqueue runs on side stream 3: compute it THERE, so the QAP front
-  // end (NTT passes, HBM-bound) overlaps the A / B1 / B2 bucket phases (multiply-bound) on the other streams
-  cudaStream_t sq = g_serial ? st : g_side[2];
+// groth16.GenerateProofs fed from the DEVICE-resident witness d_w (m standard-form scalars): px = CombinePolynomials(w,
+// R1CSToQAP(a, b, c)) — or the quotient h directly — is computed on the device from the resident sparse R1CS (never
+// leaving HBM) and handed to the prove pipeline, all on `st` and the key's side streams with the key's R1CS workspace,
+// so proofs on keys of the two prove contexts may be in flight together.  No host synchronisation after the first call
+// on an (R1CS, context) pair.  A sharded rank that holds no PowersTauDelta index needs no quotient and runs no QAP kernel.
+int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint64_t* r, const uint64_t* s, Fq* d_out,
+                            cudaStream_t st, int* err) {
+  if (fr_load_std(r).geq_modulus() || fr_load_std(s).geq_modulus())
+    return fail(B200_ERANGE, "groth16_prove_witness: r or s >= field order");
+  const size_t npx = 2 * r1->n - 1;
+  if (!pk_needs_px(pk)) return groth16_enqueue(pk, d_w, pk->m, nullptr, npx, r, s, d_out, st, err);
+  R1csWork* ws;
+  int rc = r1cs_work(r1, pk->ctx, &ws);
+  if (rc) return rc;
+  // the quotient is only consumed on side stream 3 (groth16_enqueue): compute it THERE, so the QAP front end (NTT passes,
+  // HBM-bound) overlaps the A / B1 / B2 bucket phases (multiply-bound) on the other streams
+  cudaStream_t sq = g_serial ? st : pk->side()[2];
   if (sq != st) {
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
   // h = (ax*bx - cx) / Z straight from the witness (no px): the shape the reference supports has Z = prod_{i<=n}(x - i)
   // (m = n + 2, SURVEY H5) — checked; anything else goes through px and the division.
-  const bool h_direct = rc1->n >= 2 && pk->Z.nb == rc1->n + 1;
-  int rc;
-  Fq* o = pk->out_std.as<Fq>();
-  if (h_direct) {
-    CU(pk->h_full.ensure((pk->m + pk->n_h_bases + 4) * sizeof(Fr)));
-    rc = qap_h_enqueue(rc1, pk->w_stage.as<Fr>(), pk->h_full.as<Fr>(), sq);
-    if (rc) return rc;
-    rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, rc1->px_mont.as<Fr>(), 2 * rc1->n - 1, r, s, o, st, g_d_err, 1,
-                         pk->h_full.as<Fr>());
-  } else {
-    rc = qap_px_enqueue(rc1, pk->w_stage.as<Fr>(), nullptr, nullptr, sq);
-    if (rc) return rc;
-    rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, rc1->px_mont.as<Fr>(), 2 * rc1->n - 1, r, s, o, st, g_d_err,
-                         /*px_mont=*/1);
+  if (r1->n >= 2 && pk->Z.nb == r1->n + 1) {
+    if ((rc = qap_h_enqueue(r1, *ws, pk->poly(), d_w, err, sq))) return rc;
+    return groth16_enqueue(pk, d_w, pk->m, nullptr, npx, r, s, d_out, st, err, 0, ws->h_std.as<Fr>());
   }
+  if ((rc = qap_px_enqueue(r1, *ws, pk->poly(), d_w, nullptr, nullptr, err, sq))) return rc;
+  return groth16_enqueue(pk, d_w, pk->m, ws->px_mont.as<Fr>(), npx, r, s, d_out, st, err, /*px_mont=*/1);
+}
+
+int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, const uint64_t* r, const uint64_t* s,
+                          uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c, std::unique_lock<std::mutex>* lk) {
+  ProvingKey* pk = find_pk(h, 1);
+  R1cs* r1 = find_r1cs(hr);
+  if (!pk || !r1) return fail(B200_EINVAL, "groth16_prove_witness: bad handle");
+  if (!w || !r || !s || !pi_a || !pi_b || !pi_c) return fail(B200_EINVAL, "groth16_prove_witness: null pointer");
+  if (nw != pk->m || nw != r1->m) return fail(B200_EINVAL, "groth16_prove_witness: witness length %zu, NVars %zu, R1CS columns %zu", nw, pk->m, r1->m);
+  int rc = check_sharded_host_call(pk, "groth16_prove_witness", "b200_groth16_prove_witness_device");
   if (rc) return rc;
-  uint64_t host_out[48];
-  CU(cudaMemcpyAsync(host_out, o, sizeof host_out, cudaMemcpyDeviceToHost, st));
-  rc = check_err_flag<Fr>("groth16_prove_witness");
-  if (rc) return rc;
-  memcpy(pi_a, host_out, 12 * 8);
-  memcpy(pi_c, host_out + 12, 12 * 8);
-  memcpy(pi_b, host_out + 24, 24 * 8);
-  return B200_OK;
+  cudaStream_t st = pk->main();
+  // the QAP front end reads the whole witness; a rank that runs none reads only its own index ranges
+  if ((rc = stage_witness(pk, w, pk_needs_px(pk), st))) return rc;
+  Fq* o = pk->out_std.as<Fq>();
+  if ((rc = groth16_witness_enqueue(pk, r1, pk->w_stage.as<Fr>(), r, s, o, st, g_d_err))) return rc;
+  return finish_host_proof(pk, o, "groth16_prove_witness", st, lk, pi_a, pi_b, pi_c);
 }
 
 // ---- dense QAP API (small n) -------------------------------------------------
@@ -1260,7 +1260,21 @@ int b200_qap_eval_at(b200_r1cs_t h, const uint64_t tau[4], size_t nz, uint64_t* 
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs) { B200_API_BODY(interpolate_host(values, n, coeffs)) }
 int b200_groth16_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, const uint64_t r[4],
                                const uint64_t s[4], uint64_t pi_a[12], uint64_t pi_b[24], uint64_t pi_c[12]) {
-  B200_API_BODY(groth16_prove_witness(pk, r1cs, w, nw, r, s, pi_a, pi_b, pi_c))
+  std::unique_lock<std::mutex> lk(g_mu);
+  NEED_INIT();
+  return drain_on_error(groth16_prove_witness(pk, r1cs, w, nw, r, s, pi_a, pi_b, pi_c, &lk));
+}
+int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, const uint64_t r[4],
+                                      const uint64_t s[4], void* d_out, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  ProvingKey* p = find_pk(pk, 1);
+  R1cs* r1 = find_r1cs(r1cs);
+  if (!p || !r1 || !d_w || !r || !s || !d_out) return fail(B200_EINVAL, "groth16_prove_witness_device: bad arguments");
+  if (nw != p->m || nw != r1->m)
+    return fail(B200_EINVAL, "groth16_prove_witness_device: witness length %zu, NVars %zu, R1CS columns %zu", nw, p->m, r1->m);
+  return drain_on_error(groth16_witness_enqueue(p, r1, (const Fr*)d_w, r, s, (Fq*)d_out,
+                                                stream ? (cudaStream_t)stream : g_stream, p->d_err.as<int>()));
 }
 int b200_fq12_mul_batch(const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) { B200_API_BODY(fq12_mul_batch_host(a, b, n, out)) }
 int b200_pairing_batch(const uint64_t* g1_jac, const uint64_t* g2_jac, size_t n, uint64_t* out) { B200_API_BODY(pairing_batch_host(g1_jac, g2_jac, n, out)) }

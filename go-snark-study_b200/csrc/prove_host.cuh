@@ -423,41 +423,70 @@ int groth16_finalize_enqueue(ProvingKey* pk, const uint8_t* d_parts, int nparts,
   return B200_OK;
 }
 
+// This rank's C||PTD slice reaches into PowersTauDelta, so its proof needs the quotient h (always, on one GPU).
+bool pk_needs_px(const ProvingKey* pk) { return pk->hi[3] > pk->n_c_full; }
+
+// Host-pointer entry points: refuse a sharded key unless the proof can be finished inside the call.
+int check_sharded_host_call(const ProvingKey* pk, const char* what, const char* device_entry) {
+  if (pk->world != 1 && !(g_comm.active() && g_comm.world == pk->world))
+    return fail(B200_EINVAL, "%s: sharded key (rank %d/%d) without a matching communicator: call b200_comm_init, "
+                             "or use %s + b200_groth16_finalize_device around your own all-gather",
+                what, pk->rank, pk->world, device_entry);
+  return B200_OK;
+}
+
+// Upload the host witness into pk->w_stage on `st`: all of it, or only the index ranges this rank's MSMs read.
+int stage_witness(ProvingKey* pk, const uint64_t* w, bool all, cudaStream_t st) {
+  CU(pk->w_stage.ensure(pk->m * sizeof(Fr)));
+  if (all) {
+    CU(cudaMemcpyAsync(pk->w_stage.p, w, pk->m * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    return B200_OK;
+  }
+  const size_t l1 = pk->npublic + 1, ncf = pk->n_c_full;
+  size_t lo[4], hi[4];
+  for (int k = 0; k < 3; k++) { lo[k] = pk->lo[k]; hi[k] = pk->hi[k]; }
+  size_t c_lo = pk->lo[3] < ncf ? pk->lo[3] : ncf, c_hi = pk->hi[3] < ncf ? pk->hi[3] : ncf;
+  lo[3] = l1 + c_lo;
+  hi[3] = l1 + c_hi;
+  for (int k = 0; k < 4; k++) {
+    if (lo[k] >= hi[k]) continue;
+    bool dup = false;
+    for (int j = 0; j < k; j++) dup = dup || (lo[j] <= lo[k] && hi[k] <= hi[j] && lo[j] < hi[j]);
+    if (dup) continue;
+    CU(cudaMemcpyAsync(pk->w_stage.as<Fr>() + lo[k], reinterpret_cast<const Fr*>(w) + lo[k], (hi[k] - lo[k]) * sizeof(Fr),
+                       cudaMemcpyHostToDevice, st));
+  }
+  return B200_OK;
+}
+
+// Copy the 48-word proof out to the key's pinned landing area and wait for it (with `lk`: the wait runs with the library
+// mutex released), then split it into the caller's PiA, PiB, PiC.
+int finish_host_proof(ProvingKey* pk, const Fq* d_proof, const char* what, cudaStream_t st, std::unique_lock<std::mutex>* lk,
+                      uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c) {
+  uint64_t* host_out = pk->h_out;
+  CU(cudaMemcpyAsync(host_out, d_proof, 48 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  int rc = check_err_flag<Fr>(what, st, lk, reinterpret_cast<int*>(host_out + 48));
+  if (rc) return rc;
+  memcpy(pi_a, host_out, 12 * 8);
+  memcpy(pi_c, host_out + 12, 12 * 8);
+  memcpy(pi_b, host_out + 24, 24 * 8);
+  return B200_OK;
+}
+
 int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px, size_t npx, const uint64_t* r,
                   const uint64_t* s, uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c, std::unique_lock<std::mutex>* lk = nullptr) {
   ProvingKey* pk = find_pk(h, 1);
   if (!pk) return fail(B200_EINVAL, "groth16_prove: bad proving-key handle");
   if (!w || !px || !r || !s || !pi_a || !pi_b || !pi_c) return fail(B200_EINVAL, "groth16_prove: null pointer");
   if (nw != pk->m) return fail(B200_EINVAL, "groth16_prove: witness length %zu != NVars %zu", nw, pk->m);
-  const bool sharded = pk->world != 1;
-  if (sharded && !(g_comm.active() && g_comm.world == pk->world))
-    return fail(B200_EINVAL, "groth16_prove: sharded key (rank %d/%d) without a matching communicator: call b200_comm_init, "
-                             "or use b200_groth16_prove_device + b200_groth16_finalize_device around your own all-gather",
-                pk->rank, pk->world);
+  int rc = check_sharded_host_call(pk, "groth16_prove", "b200_groth16_prove_device");
+  if (rc) return rc;
   if (npx < pk->Z.nb) return fail(B200_EINVAL, "groth16_prove: len(px) < len(Z)");
   cudaStream_t st = pk->main();   // context 1 keys: their own main stream (a second host thread's proof in flight)
   CU(pk->px.ensure(npx * sizeof(Fr)));
-  CU(pk->w_stage.ensure(nw * sizeof(Fr)));
-  bool need_px = true;
-  if (!sharded) {
-    CU(cudaMemcpyAsync(pk->w_stage.p, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
-  } else {   // stage only what this rank reads: its witness index ranges, and px only if it holds PowersTauDelta points
-    const size_t l1 = pk->npublic + 1, ncf = pk->n_c_full;
-    size_t lo[4], hi[4];
-    for (int k = 0; k < 3; k++) { lo[k] = pk->lo[k]; hi[k] = pk->hi[k]; }
-    size_t c_lo = pk->lo[3] < ncf ? pk->lo[3] : ncf, c_hi = pk->hi[3] < ncf ? pk->hi[3] : ncf;
-    lo[3] = l1 + c_lo;
-    hi[3] = l1 + c_hi;
-    need_px = pk->hi[3] > ncf;
-    for (int k = 0; k < 4; k++) {
-      if (lo[k] >= hi[k]) continue;
-      bool dup = false;
-      for (int j = 0; j < k; j++) dup = dup || (lo[j] <= lo[k] && hi[k] <= hi[j] && lo[j] < hi[j]);
-      if (dup) continue;
-      CU(cudaMemcpyAsync(pk->w_stage.as<Fr>() + lo[k], reinterpret_cast<const Fr*>(w) + lo[k], (hi[k] - lo[k]) * sizeof(Fr),
-                         cudaMemcpyHostToDevice, st));
-    }
-  }
+  // sharded: stage only what this rank reads, its witness index ranges, and px only if it holds PowersTauDelta points
+  if ((rc = stage_witness(pk, w, pk->world == 1, st))) return rc;
+  const bool need_px = pk_needs_px(pk);
   // px is only needed by the division on side stream 3: copy it there so the transfer overlaps the sort of w
   // (same-stream order makes the division see it; the previous proof's use of pk->px finished before its combine)
   // (measurement mode runs the division on `st`, so the copy goes there too)
@@ -470,16 +499,9 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
                        cudaMemcpyHostToDevice, g_serial ? st : pk->side()[2]));
   }
   Fq* o = pk->out_std.as<Fq>();
-  int rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st, g_d_err);
+  rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st, g_d_err);
   if (rc) return rc;
-  uint64_t* host_out = pk->h_out;
-  CU(cudaMemcpyAsync(host_out, o, 48 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  rc = check_err_flag<Fr>("groth16_prove", st, lk, reinterpret_cast<int*>(host_out + 48));  // synchronises (the wait runs with the library mutex released)
-  if (rc) return rc;
-  memcpy(pi_a, host_out, 12 * 8);
-  memcpy(pi_c, host_out + 12, 12 * 8);
-  memcpy(pi_b, host_out + 24, 24 * 8);
-  return B200_OK;
+  return finish_host_proof(pk, o, "groth16_prove", st, lk, pi_a, pi_b, pi_c);
 }
 
 // Pinocchio result slots (XYZZ, 256 B each): 0 PiA, 1 PiAp, 2 PiBp, 3 PiC, 4 PiCp, 5 PiH, 6 PiKp, 7 PiB (G2).

@@ -410,12 +410,16 @@ inline cudaError_t interpolate_ap(PolyCtx& pc, const QapDomain& dom, QapWork& wk
 // transform of 1/i! each), form h there pointwise — Z(1 + Y) = Y! / (Y - n)! — and interpolate h ONCE over the points
 // n+1 .. 2n-1 (subproduct tree with offset n).  Same field elements as DivisorPolynomial(CombinePolynomials(..)), ~40 % fewer
 // multiplications than going through px.
-struct QapHDomain {
+// The scratch of one quotient computation; a proof in flight needs its own (one per prove context).
+struct QapHWork {
+  QapWork work;                 // e^-x cache etc. of the final interpolation
+  DevBuf V, hv, coef;           // 3 x M shift products; n-1 values of h; N' coefficients (allocated on first use)
+};
+// Read-only once built; its own QapHWork serves callers that compute one quotient at a time.
+struct QapHDomain : QapHWork {
   size_t n = 0, M = 0;          // constraints; cyclic size of the shift products (2 * pow2 >= n)
   QapDomain tree;               // points n+1 .. n+N', factorials up to 2n
   DevBuf G;                     // transform of (1/i!)_{i < 2n-1}, size M, pre-scaled by 1/M
-  QapWork work;                 // e^-x cache etc. of the final interpolation
-  DevBuf V, hv, coef;           // 3 x M shift products; n-1 values of h; N' coefficients
 };
 inline cudaError_t qap_hdomain_build(PolyCtx& pc, QapHDomain& hd, size_t n, cudaStream_t st) {
   hd.n = n;
@@ -426,9 +430,6 @@ inline cudaError_t qap_hdomain_build(PolyCtx& pc, QapHDomain& hd, size_t n, cuda
   while (Np < (n > 1 ? n - 1 : 1)) Np <<= 1;
   PCU(qap_domain_build(pc, hd.tree, Np, st, n, 2 * n, true));
   PCU(hd.G.alloc(hd.M * sizeof(Fr)));
-  PCU(hd.V.alloc(3 * hd.M * sizeof(Fr)));
-  PCU(hd.hv.alloc(n * sizeof(Fr)));
-  PCU(hd.coef.alloc(Np * sizeof(Fr)));
   const int lm = ceil_log2(hd.M);
   NttPlan* pl;
   PCU(pc.plan(lm, &pl, st));
@@ -439,18 +440,23 @@ inline cudaError_t qap_hdomain_build(PolyCtx& pc, QapHDomain& hd, size_t n, cuda
   return cudaGetLastError();
 }
 // d: Newton coefficients of a | b | c over {1..n} (3 blocks of `dstride`, from newton_coeffs on the QAP domain);
-// h_out: n - 1 coefficients of h (Montgomery) in hd.coef.
-inline cudaError_t qap_h_from_newton(PolyCtx& pc, QapHDomain& hd, const Fr* d, size_t dstride, cudaStream_t st) {
+// h_out: n - 1 coefficients of h (Montgomery) in ws->coef (ws = null: the domain's own scratch).
+inline cudaError_t qap_h_from_newton(PolyCtx& pc, QapHDomain& hd, const Fr* d, size_t dstride, cudaStream_t st,
+                                     QapHWork* ws = nullptr) {
+  QapHWork& w = ws ? *ws : hd;
   const size_t n = hd.n, M = hd.M;
   const int lm = ceil_log2(M);
-  Fr* V = hd.V.as<Fr>();
+  PCU(w.V.ensure(3 * M * sizeof(Fr)));
+  PCU(w.hv.ensure(n * sizeof(Fr)));
+  PCU(w.coef.ensure(hd.tree.N * sizeof(Fr)));
+  Fr* V = w.V.as<Fr>();
   for (int q = 0; q < 3; q++) B200_LAUNCH(k_take, nblk(M, 256), 256, st, d + q * dstride, (uint32_t)n, (uint32_t)M, V + q * M);
   PCU(ntt_batched(pc, V, lm, 3 * M, 0, st));
   B200_LAUNCH(k_dc_pointwise, nblk(3 * M, 256), 256, st, V, hd.G.as<Fr>(), (uint32_t)M, (uint32_t)(3 * M));
   PCU(ntt_batched(pc, V, lm, 3 * M, 1, st));
   if (n >= 2) {
-    B200_LAUNCH(k_h_values, nblk(n - 1, 256), 256, st, V, (uint32_t)M, hd.tree.fact.as<Fr>(), (uint32_t)n, hd.hv.as<Fr>());
-    PCU(interpolate_ap(pc, hd.tree, hd.work, hd.hv.as<Fr>(), n - 1, n - 1, 1, hd.coef.as<Fr>(), st));
+    B200_LAUNCH(k_h_values, nblk(n - 1, 256), 256, st, V, (uint32_t)M, hd.tree.fact.as<Fr>(), (uint32_t)n, w.hv.as<Fr>());
+    PCU(interpolate_ap(pc, hd.tree, w.work, w.hv.as<Fr>(), n - 1, n - 1, 1, w.coef.as<Fr>(), st));
   }
   pc.note(8);
   return cudaGetLastError();
@@ -462,13 +468,21 @@ struct SparseMat {
   DevBuf cptr, crow, cval;      // CSC = CSR of the transpose (m rows): the trusted setup's A^T l(tau)
   size_t nnz = 0;
 };
+// Witness -> px / h scratch of one proof in flight on an R1CS: one per prove context, so proofs on keys of the two
+// contexts may share the R1CS and overlap.
+struct R1csWork {
+  DevBuf w_mont, vals, coef;        // witness (m), A w | B w | C w (3 x n), coefficients (3 x N), all Montgomery
+  DevBuf px_mont;                   // 2n - 1
+  DevBuf h_std;                     // h = px / Z, n - 1 coefficients, standard form (h-direct branch)
+  QapWork work;
+  QapHWork hw;
+};
 struct R1cs {
   size_t n = 0, m = 0;
   SparseMat M[3];
-  DevBuf w_mont, vals, coef, lag;   // witness (m), A w | B w | C w (3 x n), coefficients (3 x N), Lagrange basis at tau (n)
-  DevBuf px_mont;                   // 2n - 1
-  QapWork work;
+  DevBuf lag;                       // Lagrange basis at tau (n): the trusted setup
   std::unique_ptr<QapHDomain> hd;   // witness -> h directly (b200_groth16_prove_witness), built on first use
+  std::unique_ptr<R1csWork> ws[2];  // per prove context, allocated on first use
 };
 
 }  // namespace b200

@@ -85,77 +85,90 @@ int r1cs_load(size_t n, size_t m, const uint32_t* const rowptr[3], const uint32_
     int rc = sparse_upload(r->M[k], n, m, rowptr[k], col[k], val[k], names[k]);
     if (rc) return rc;
   }
-  size_t N = pow2_at_least(n);
-  CU(r->w_mont.alloc(m * sizeof(Fr)));
-  CU(r->vals.alloc(3 * n * sizeof(Fr)));
-  CU(r->coef.alloc(3 * N * sizeof(Fr)));
-  CU(r->px_mont.alloc((2 * n) * sizeof(Fr)));
   uint64_t h = g_next_r1cs++;
   g_r1cs[h] = std::move(r);
   *out = h;
   return B200_OK;
 }
 
-// d_w: m witness values in device memory, standard form.  Leaves ax | bx | cx (N-strided, Montgomery) in r->coef and
-// px (2n-1, Montgomery) in r->px_mont; optional standard-form copies to device buffers.
-int qap_px_enqueue(R1cs* r, const Fr* d_w_std, Fr* d_abc_std /* 3 x n or null */, Fr* d_px_std /* 2n-1 or null */,
-                   cudaStream_t st) {
+// The scratch of prove context `ctx` on this R1CS, allocated on first use (which may synchronise the device).
+int r1cs_work(R1cs* r, int ctx, R1csWork** out) {
+  auto& ws = r->ws[ctx];
+  if (!ws) {
+    const size_t n = r->n, m = r->m, N = pow2_at_least(n);
+    auto w = std::make_unique<R1csWork>();
+    CU(w->w_mont.alloc(m * sizeof(Fr)));
+    CU(w->vals.alloc(3 * n * sizeof(Fr)));
+    CU(w->coef.alloc(3 * N * sizeof(Fr)));
+    CU(w->px_mont.alloc((2 * n) * sizeof(Fr)));
+    CU(w->h_std.alloc(n * sizeof(Fr)));
+    ws = std::move(w);
+  }
+  *out = ws.get();
+  return B200_OK;
+}
+
+// d_w: m witness values in device memory, standard form (an entry >= r is read as 0 and sets bit 1 of *err).  Leaves
+// ax | bx | cx (N-strided, Montgomery) in ws.coef and px (2n-1, Montgomery) in ws.px_mont; optional standard-form copies
+// to device buffers.  The interpolation domain is shared by every context: built (and waited for) on the first call.
+int qap_px_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, Fr* d_abc_std /* 3 x n or null */,
+                   Fr* d_px_std /* 2n-1 or null */, int* err, cudaStream_t st) {
   const size_t n = r->n, m = r->m, N = pow2_at_least(n);
   QapDomain* dom;
   int rc = get_domain(N, &dom);
   if (rc) return rc;
-  PolyCtx& pc = *g_poly;
-  Fr* w = r->w_mont.as<Fr>();
-  k_poly_load<<<nblk(m, 256), 256, 0, st>>>(d_w_std, (uint32_t)m, (uint32_t)m, 0, 0, w, (uint32_t)m, g_d_err);
-  Fr* vals = r->vals.as<Fr>();
+  Fr* w = ws.w_mont.as<Fr>();
+  k_poly_load<<<nblk(m, 256), 256, 0, st>>>(d_w_std, (uint32_t)m, (uint32_t)m, 0, 0, w, (uint32_t)m, err);
+  Fr* vals = ws.vals.as<Fr>();
   for (int k = 0; k < 3; k++)
     k_spmv_csr<<<nblk(n, 128), 128, 0, st>>>(r->M[k].rowptr.as<uint32_t>(), r->M[k].col.as<uint32_t>(), r->M[k].val.as<Fr>(), w,
                                               (uint32_t)n, vals + k * n);
   g_launches += 4;
-  Fr* coef = r->coef.as<Fr>();
-  CU(interpolate_ap(pc, *dom, r->work, vals, n, n, 3, coef, st));
+  Fr* coef = ws.coef.as<Fr>();
+  CU(interpolate_ap(pc, *dom, ws.work, vals, n, n, 3, coef, st));
   if (d_abc_std)
     for (int k = 0; k < 3; k++)
       k_poly_store<<<nblk(n, 256), 256, 0, st>>>(coef + k * N, (uint32_t)n, 0, 1, d_abc_std + k * n);
   // px = ax * bx - cx: one size-2N cyclic product (2n - 1 <= 2N)
   const size_t N2 = 2 * N;
   const int l2 = dom->logN + 1;
-  Fr* U = r->work.U.as<Fr>();   // >= 3 * 2N elements (interpolate_ap sized it)
+  Fr* U = ws.work.U.as<Fr>();   // >= 3 * 2N elements (interpolate_ap sized it)
   k_take<<<nblk(N2, 256), 256, 0, st>>>(coef, (uint32_t)n, (uint32_t)N2, U);
   k_take<<<nblk(N2, 256), 256, 0, st>>>(coef + N, (uint32_t)n, (uint32_t)N2, U + N2);
   CU(ntt_batched(pc, U, l2, 2 * N2, 0, st));
   CU(pc.pointwise(U, U + N2, l2, true, st));
   CU(ntt_batched(pc, U, l2, N2, 1, st));
-  k_px_finish<<<nblk(2 * n - 1, 256), 256, 0, st>>>(U, coef + 2 * N, (uint32_t)n, r->px_mont.as<Fr>(), d_px_std);
+  k_px_finish<<<nblk(2 * n - 1, 256), 256, 0, st>>>(U, coef + 2 * N, (uint32_t)n, ws.px_mont.as<Fr>(), d_px_std);
   g_launches += 4;
   CU(cudaGetLastError());
   return B200_OK;
 }
 
-// d_w: m witness values (device, standard form) -> the n - 1 coefficients of h = (ax*bx - cx) / Z in d_h_std (standard form),
-// without forming px (qap_sparse.cuh: QapHDomain).  Requires n >= 2.
-int qap_h_enqueue(R1cs* r, const Fr* d_w_std, Fr* d_h_std, cudaStream_t st) {
+// d_w: m witness values (device, standard form; an entry >= r is read as 0 and sets bit 1 of *err) -> the n - 1
+// coefficients of h = (ax*bx - cx) / Z in ws.h_std (standard form), without forming px (qap_sparse.cuh: QapHDomain).
+// Requires n >= 2.  The domains are shared by every context: built on g_stream and waited for on the first call.
+int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
   const size_t n = r->n, m = r->m, N = pow2_at_least(n);
   if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
   QapDomain* dom;
   int rc = get_domain(N, &dom);
   if (rc) return rc;
-  PolyCtx& pc = *g_poly;
   if (!r->hd) {
-    r->hd = std::make_unique<QapHDomain>();
-    CU(qap_hdomain_build(pc, *r->hd, n, st));
+    auto hd = std::make_unique<QapHDomain>();
+    CU(qap_hdomain_build(*g_poly, *hd, n, g_stream));   // synchronises g_stream
+    r->hd = std::move(hd);
   }
-  Fr* w = r->w_mont.as<Fr>();
-  k_poly_load<<<nblk(m, 256), 256, 0, st>>>(d_w_std, (uint32_t)m, (uint32_t)m, 0, 0, w, (uint32_t)m, g_d_err);
-  Fr* vals = r->vals.as<Fr>();
+  Fr* w = ws.w_mont.as<Fr>();
+  k_poly_load<<<nblk(m, 256), 256, 0, st>>>(d_w_std, (uint32_t)m, (uint32_t)m, 0, 0, w, (uint32_t)m, err);
+  Fr* vals = ws.vals.as<Fr>();
   for (int k = 0; k < 3; k++)
     k_spmv_csr<<<nblk(n, 128), 128, 0, st>>>(r->M[k].rowptr.as<uint32_t>(), r->M[k].col.as<uint32_t>(), r->M[k].val.as<Fr>(), w,
                                               (uint32_t)n, vals + k * n);
   g_launches += 4;
-  Fr* coef = r->coef.as<Fr>();   // here: the Newton coefficients of a | b | c (N-strided)
-  CU(newton_coeffs(pc, *dom, r->work, vals, n, n, 3, coef, st));
-  CU(qap_h_from_newton(pc, *r->hd, coef, N, st));
-  k_poly_store<<<nblk(n - 1, 256), 256, 0, st>>>(r->hd->coef.as<Fr>(), (uint32_t)(n - 1), 0, 1, d_h_std);
+  Fr* coef = ws.coef.as<Fr>();   // here: the Newton coefficients of a | b | c (N-strided)
+  CU(newton_coeffs(pc, *dom, ws.work, vals, n, n, 3, coef, st));
+  CU(qap_h_from_newton(pc, *r->hd, coef, N, st, &ws.hw));
+  k_poly_store<<<nblk(n - 1, 256), 256, 0, st>>>(ws.hw.coef.as<Fr>(), (uint32_t)(n - 1), 0, 1, ws.h_std.as<Fr>());
   g_launches += 1;
   CU(cudaGetLastError());
   return B200_OK;
@@ -167,12 +180,15 @@ int qap_px_host(b200_r1cs_t h, const uint64_t* w, size_t nw, uint64_t* ax, uint6
   if (!w || nw != r->m) return fail(B200_EINVAL, "qap_px: witness length %zu != m %zu", nw, r->m);
   const size_t n = r->n;
   cudaStream_t st = g_stream;
+  R1csWork* ws;
+  int rc = r1cs_work(r, 0, &ws);
+  if (rc) return rc;
   DevBuf dw, dabc, dpx;
   CU(dw.alloc(nw * sizeof(Fr)));
   CU(dabc.alloc(3 * n * sizeof(Fr)));
   CU(dpx.alloc((2 * n - 1) * sizeof(Fr)));
   CU(cudaMemcpyAsync(dw.p, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
-  int rc = qap_px_enqueue(r, dw.as<Fr>(), dabc.as<Fr>(), dpx.as<Fr>(), st);
+  rc = qap_px_enqueue(r, *ws, *g_poly, dw.as<Fr>(), dabc.as<Fr>(), dpx.as<Fr>(), g_d_err, st);
   if (rc) return rc;
   uint64_t* outs[3] = {ax, bx, cx};
   for (int k = 0; k < 3; k++)

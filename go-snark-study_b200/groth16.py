@@ -64,6 +64,17 @@ class DeviceProvingKey:
                                        ptr(rr), ptr(ss), ptr(pa), ptr(pb), ptr(pc)))
         return {"PiA": _unflatten_g1(pa)[0], "PiB": _unflatten_g2(pb)[0], "PiC": _unflatten_g1(pc)[0]}
 
+    def prove_witness_limbs(self, r1cs, w_limbs, r, s):
+        """The proof from the witness alone (b200_groth16_prove_witness): px, or the quotient directly, is computed on the
+        device from ``r1cs`` (an r1csqap.SparseR1CS of the same circuit)."""
+        pa = np.zeros(12, dtype=np.uint64)
+        pb = np.zeros(24, dtype=np.uint64)
+        pc = np.zeros(12, dtype=np.uint64)
+        rr, ss = ints_to_limbs([r]), ints_to_limbs([s])
+        check(lib().b200_groth16_prove_witness(self.handle, r1cs.handle, ptr(w_limbs), w_limbs.shape[0], ptr(rr), ptr(ss),
+                                               ptr(pa), ptr(pb), ptr(pc)))
+        return {"PiA": _unflatten_g1(pa)[0], "PiB": _unflatten_g2(pb)[0], "PiC": _unflatten_g1(pc)[0]}
+
     def free(self):
         if self.handle:
             check(lib().b200_pk_free(self.handle))

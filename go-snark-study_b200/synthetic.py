@@ -231,12 +231,14 @@ class CircuitGroth16(CircuitQAP, SyntheticGroth16):
         self.ic = mint_points(1, ints_to_limbs(self.k_ic))
         self.px = self.px_of(self.w)
 
-    def expected_dlogs(self):
-        w = self.circuit.witness
+    def expected_dlogs(self, witness=None, r=None, s=None):
+        """Discrete logs of PiA, PiB, PiC for ``witness`` (ints, a satisfying witness of this R1CS, e.g. of
+        SyntheticCircuit(n, seed=...)) and blinding r, s — this instance's own unless given."""
+        w = self.circuit.witness if witness is None else witness
         dot = lambda ks: sum(a * b for a, b in zip(ks, w)) % R
         t, ka, kb, kg, kd = (self.toxic[k] for k in ("T", "Kalpha", "Kbeta", "Kgamma", "Kdelta"))
         A, B, C = dot(self.at_s), dot(self.bt_s), dot(self.ct_s)
-        r, s = self.r, self.s
+        r, s = (self.r if r is None else r), (self.s if s is None else s)
         a = (A + ka + r * kd) % R
         b = (B + kb + s * kd) % R
         l1 = self.npublic + 1

@@ -310,9 +310,27 @@ int b200_qap_eval_at(b200_r1cs_t h, const uint64_t tau[4], size_t nz, uint64_t* 
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs);
 /* groth16.GenerateProofs fed from the witness: px is computed on the device from the resident R1CS (b200_qap_px) and
  * never leaves HBM; otherwise identical to b200_groth16_prove (groth16/groth16.go:225-278 after the caller's
- * CombinePolynomials step, cli/main.go:339-349).                                                                     */
+ * CombinePolynomials step, cli/main.go:339-349).  nw must equal the key's m and the R1CS's m.  Like b200_groth16_prove
+ * it runs on the key's prove context (B200_CFG_PK_CONTEXT) and waits with the library mutex released, so two host
+ * threads proving on keys of contexts 0 and 1 overlap, also when both keys share one R1CS handle.  A sharded key needs
+ * a matching communicator (b200_comm_init; SPMD, the proof is returned on every rank); without one the call returns
+ * B200_EINVAL — use b200_groth16_prove_witness_device + b200_groth16_finalize_device instead.                         */
 int b200_groth16_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, const uint64_t r[4],
                                const uint64_t s[4], uint64_t pi_a[12], uint64_t pi_b[24], uint64_t pi_c[12]);
+/* groth16.GenerateProofs fed from a DEVICE-resident witness (m standard-form scalars): b200_groth16_prove_witness with
+ * the result left in device memory on `stream`, as in b200_groth16_prove_device (48 u64 PiA | PiC | PiB; on a sharded
+ * key without a communicator, the 1 KB partial record for b200_groth16_finalize_device).
+ *   - No host synchronisation, except on the FIRST call for a given (R1CS, prove context) pair: that call builds the
+ *     R1CS's interpolation domains (shared by both contexts) and the context's workspaces, and may synchronise.
+ *   - Proofs on keys of the two prove contexts may be in flight together on two streams, also on one R1CS handle (each
+ *     context has its own workspace on the R1CS).  Two proofs on the SAME context must be ordered by the caller.
+ *   - A witness entry >= r is read as 0, and neither this call nor any later one reports it (nor a proof on another
+ *     key), as in b200_groth16_prove_device.  r and s are host values and are checked (B200_ERANGE).
+ *   - A bad handle, a null pointer, or nw different from the key's m or the R1CS's m returns B200_EINVAL.
+ *   - On a sharded key only a rank that holds PowersTauDelta indices (b200_groth16_shard_info needs_px) runs the QAP
+ *     front end, and reads the whole witness; every other rank reads only its witness ranges.                       */
+int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw,
+                                      const uint64_t r[4], const uint64_t s[4], void* d_out, void* stream);
 
 /* ---- element-wise group operations, reference formulas (X,Y,Z-exact) ------------------- */
 /* bn128.G1.Add / Double / Neg / Affine (bn128/g1.go:32-170) and the G2 twins (bn128/g2.go:32-200), n independent
