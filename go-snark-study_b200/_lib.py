@@ -89,6 +89,8 @@ _SIGNATURES = {
     "b200_qap_px": [_h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_qap_eval_at": [_h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_interpolate": [_vp, _sz, _vp],
+    "b200_groth16_setup": [_h, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "b200_pinocchio_setup": [_h, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "b200_groth16_prove_witness": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp, _vp],
     "b200_groth16_prove_witness_device": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_profile": [_int],

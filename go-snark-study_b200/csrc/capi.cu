@@ -20,6 +20,7 @@
 #include "poly_host.cuh"
 #include "qap.cuh"
 #include "qap_sparse.cuh"
+#include "fixed_base.cuh"
 #include "comm.cuh"
 #include "shard_partition.h"
 #include "glv.cuh"
@@ -281,14 +282,7 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   CU(staging.alloc(n * 3 * sizeof(F)));
   CU(state.alloc(n * sizeof(XYZZ<F>)));
   CU(cudaMemcpyAsync(staging.p, pts, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_stream));
-  Affine<F>* table = b->table.as<Affine<F>>();
-  k_load_bases<F><<<nblocks(n, 128), 128, 0, g_stream>>>(staging.as<F>(), n, table, g_d_err);
-  k_affine_to_xyzz<F><<<nblocks(n, 128), 128, 0, g_stream>>>(table, state.as<XYZZ<F>>(), n);
-  for (uint32_t w = 1; w < sh.nwin; w++) {
-    k_window_step<F><<<nblocks(n, 128), 128, 0, g_stream>>>(state.as<XYZZ<F>>(), n, c);
-    constexpr int K = 8;
-    k_batch_to_affine<F, K><<<nblocks((n + K - 1) / K, 128), 128, 0, g_stream>>>(state.as<XYZZ<F>>(), table + (size_t)w * n, n);
-  }
+  window_table_enqueue<F>(staging.as<F>(), n, sh.nwin, c, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_d_err, g_stream);
   CU(cudaGetLastError());
   int rc = check_err_flag<F>("bases_load");
   if (rc) return rc;
@@ -1033,6 +1027,8 @@ int group_op_host(int op, const uint64_t* p, const uint64_t* q, size_t n, uint64
   return check_err_flag<F>("group op");
 }
 
+#include "setup_host.cuh"
+
 }  // namespace
 
 // On an error return, work already queued on the library's streams is drained first: no entry point leaves kernels in
@@ -1258,6 +1254,17 @@ int b200_qap_eval_at(b200_r1cs_t h, const uint64_t tau[4], size_t nz, uint64_t* 
   B200_API_BODY(qap_eval_at_host(h, tau, nz, at, bt, ct, zt))
 }
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs) { B200_API_BODY(interpolate_host(values, n, coeffs)) }
+int b200_groth16_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[20], uint64_t* at, uint64_t* b1, uint64_t* b2,
+                       uint64_t* bacdelta, uint64_t* ptd, uint64_t* z, uint64_t alpha1[12], uint64_t beta1[12],
+                       uint64_t delta1[12], uint64_t beta2[24], uint64_t gamma2[24], uint64_t delta2[24], uint64_t* ic) {
+  B200_API_BODY(groth16_setup_host(r1cs, npublic, toxic, at, b1, b2, bacdelta, ptd, z, alpha1, beta1, delta1, beta2, gamma2,
+                                   delta2, ic))
+}
+int b200_pinocchio_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[32], uint64_t* a, uint64_t* ap, uint64_t* b2,
+                         uint64_t* bp, uint64_t* c, uint64_t* cp, uint64_t* kp, uint64_t* g1t, uint64_t* z, uint64_t vk_g1[24],
+                         uint64_t vk_g2[120]) {
+  B200_API_BODY(pinocchio_setup_host(r1cs, npublic, toxic, a, ap, b2, bp, c, cp, kp, g1t, z, vk_g1, vk_g2))
+}
 int b200_groth16_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, const uint64_t r[4],
                                const uint64_t s[4], uint64_t pi_a[12], uint64_t pi_b[24], uint64_t pi_c[12]) {
   std::unique_lock<std::mutex> lk(g_mu);

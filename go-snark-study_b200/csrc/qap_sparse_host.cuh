@@ -250,24 +250,20 @@ int zero_poly_device(size_t n, DevBuf& d_out, cudaStream_t st) {
 // groth16/groth16.go:164-205, snark.go:171-189) without the dense polynomials: A^T l(tau) with l = Lagrange basis of
 // {1..n} at tau; and zt = prod_{i=1..nz}(tau - i).
 __global__ void k_spmv_t(const uint32_t* __restrict__ cptr, const uint32_t* __restrict__ crow, const Fr* __restrict__ cval,
-                         const Fr* __restrict__ l, uint32_t m, Fr* __restrict__ out_std) {
+                         const Fr* __restrict__ l, uint32_t m, Fr* __restrict__ out) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
   Fr acc = Fr::zero();
   for (uint32_t k = cptr[i], e = cptr[i + 1]; k < e; k++) acc = acc + cval[k] * l[crow[k]];
-  out_std[i] = acc.from_mont();
+  out[i] = acc;
 }
-int qap_eval_at_host(b200_r1cs_t h, const uint64_t* tau, size_t nz, uint64_t* at, uint64_t* bt, uint64_t* ct, uint64_t* zt_out) {
-  R1cs* r = find_r1cs(h);
-  if (!r) return fail(B200_EINVAL, "qap_eval_at: bad R1CS handle");
-  if (!tau || !at || !bt || !ct) return fail(B200_EINVAL, "qap_eval_at: null pointer");
-  Fr t_std = fr_load_std(tau);
-  if (t_std.geq_modulus()) return fail(B200_ERANGE, "qap_eval_at: tau >= r");
+// Enqueues at | bt | ct (Montgomery, m each) into d_out on `st`; *zt = prod_{i=1..nz}(tau - i) (Montgomery).  t: tau in
+// Montgomery form.  tau in 1..n sets bit 4 of g_d_err.
+int qap_eval_at_enqueue(R1cs* r, Fr t, size_t nz, Fr* d_out, Fr* zt, cudaStream_t st) {
   const size_t n = r->n, m = r->m, N = pow2_at_least(n);
   QapDomain* dom;
   int rc = get_domain(N, &dom);
   if (rc) return rc;
-  Fr t = t_std.to_mont();
   Fr zn = Fr::one(), znz = Fr::one();   // prod_{i=1..n}(tau - i) and prod_{i=1..nz}(tau - i), on the host (O(n))
   size_t top = n > nz ? n : nz;
   Fr acc = Fr::one();
@@ -276,17 +272,32 @@ int qap_eval_at_host(b200_r1cs_t h, const uint64_t* tau, size_t nz, uint64_t* at
     if (i == n) zn = acc;
     if (i == nz) znz = acc;
   }
-  cudaStream_t st = g_stream;
   CU(r->lag.ensure(n * sizeof(Fr)));
   k_lagrange_at<<<nblk(n, 128), 128, 0, st>>>(dom->invfact.as<Fr>(), (uint32_t)n, t, zn, r->lag.as<Fr>(), g_d_err);
-  DevBuf o;
-  CU(o.alloc(3 * m * sizeof(Fr)));
-  uint64_t* outs[3] = {at, bt, ct};
-  for (int k = 0; k < 3; k++) {
+  for (int k = 0; k < 3; k++)
     k_spmv_t<<<nblk(m, 128), 128, 0, st>>>(r->M[k].cptr.as<uint32_t>(), r->M[k].crow.as<uint32_t>(), r->M[k].cval.as<Fr>(),
-                                            r->lag.as<Fr>(), (uint32_t)m, o.as<Fr>() + k * m);
-    CU(cudaMemcpyAsync(outs[k], o.as<Fr>() + k * m, m * sizeof(Fr), cudaMemcpyDeviceToHost, st));
-  }
+                                            r->lag.as<Fr>(), (uint32_t)m, d_out + k * m);
+  CU(cudaGetLastError());
+  *zt = znz;
+  return B200_OK;
+}
+int qap_eval_at_host(b200_r1cs_t h, const uint64_t* tau, size_t nz, uint64_t* at, uint64_t* bt, uint64_t* ct, uint64_t* zt_out) {
+  R1cs* r = find_r1cs(h);
+  if (!r) return fail(B200_EINVAL, "qap_eval_at: bad R1CS handle");
+  if (!tau || !at || !bt || !ct) return fail(B200_EINVAL, "qap_eval_at: null pointer");
+  Fr t_std = fr_load_std(tau);
+  if (t_std.geq_modulus()) return fail(B200_ERANGE, "qap_eval_at: tau >= r");
+  const size_t m = r->m;
+  cudaStream_t st = g_stream;
+  DevBuf o, os;
+  CU(o.alloc(3 * m * sizeof(Fr)));
+  CU(os.alloc(3 * m * sizeof(Fr)));
+  Fr znz;
+  int rc = qap_eval_at_enqueue(r, t_std.to_mont(), nz, o.as<Fr>(), &znz, st);
+  if (rc) return rc;
+  k_poly_store<<<nblk(3 * m, 256), 256, 0, st>>>(o.as<Fr>(), (uint32_t)(3 * m), 0, 1, os.as<Fr>());
+  uint64_t* outs[3] = {at, bt, ct};
+  for (int k = 0; k < 3; k++) CU(cudaMemcpyAsync(outs[k], os.as<Fr>() + k * m, m * sizeof(Fr), cudaMemcpyDeviceToHost, st));
   if (zt_out) {
     Fr z = znz.from_mont();
     memcpy(zt_out, &z, sizeof(Fr));

@@ -55,6 +55,13 @@ class DeviceProvingKey:
         self.handle = h.value
         self.m = m
 
+    @classmethod
+    def from_handle(cls, handle, m):
+        """Wrap a key already loaded with b200_groth16_pk_load(_shard)."""
+        self = cls.__new__(cls)
+        self.handle, self.m = handle, m
+        return self
+
     def prove_limbs(self, w_limbs, px_limbs, r, s):
         pa = np.zeros(12, dtype=np.uint64)
         pb = np.zeros(24, dtype=np.uint64)
@@ -199,6 +206,71 @@ def GenerateTrustedSetup(witnessLength, circuit, alphas, betas, gammas, toxic=No
           "G2": {"Beta": beta2, "Gamma": gamma2, "Delta": delta2, "BACGamma": p2[3:]}}
     vk = {"IC": IC, "G1": {"Alpha": alpha1}, "G2": {"Beta": beta2, "Gamma": gamma2, "Delta": delta2}}
     return {"Toxic": {"T": t, "Kalpha": ka, "Kbeta": kb, "Kgamma": kg, "Kdelta": kd}, "Pk": pk, "Vk": vk}
+
+
+def draw_toxic(names, n):
+    """Toxic values drawn like the reference (Fq.Rand), T redrawn while it is one of the interpolation points 1..n."""
+    tox = {k: rand_fr() for k in names}
+    while 1 <= tox["T"] <= n:
+        tox["T"] = rand_fr()
+    return tox
+
+
+def toxic_limbs(tox, names):
+    return ints_to_limbs([int(tox[k]) for k in names])
+
+
+class SparseSetup:
+    """Groth16 key and Vk of GenerateTrustedSetupSparse as limb arrays (standard-form affine (x, y, 1) points, infinity
+    all zero): at, b1, bacdelta (m G1), b2 (m G2), ptd (m-1 G1), z (m-1 coefficients), alpha1, beta1, delta1 (G1),
+    beta2, gamma2, delta2 (G2), ic (npublic+1 G1).  A 2^20-constraint key is ~0.6 GB here; as tuples of Python ints it
+    would take gigabytes, so ``pk_dict`` is for small circuits only."""
+    TOXIC = ("T", "Kalpha", "Kbeta", "Kgamma", "Kdelta")
+
+    def __init__(self, r1cs, n_public, toxic=None):
+        m = self.m = r1cs.m
+        self.n, self.npublic = r1cs.n, n_public
+        tox = draw_toxic(self.TOXIC, r1cs.n) if toxic is None else dict(toxic)
+        self.Toxic = {k: int(tox[k]) for k in self.TOXIC}
+        g1 = lambda k: np.zeros((k, 12), dtype=np.uint64)
+        g2 = lambda k: np.zeros((k, 24), dtype=np.uint64)
+        self.at, self.b1, self.bacdelta, self.b2, self.ptd = g1(m), g1(m), g1(m), g2(m), g1(m - 1)
+        self.z = np.zeros((m - 1, 4), dtype=np.uint64)
+        self.alpha1, self.beta1, self.delta1 = g1(1), g1(1), g1(1)
+        self.beta2, self.gamma2, self.delta2 = g2(1), g2(1), g2(1)
+        self.ic = g1(n_public + 1)
+        check(lib().b200_groth16_setup(r1cs.handle, n_public, ptr(toxic_limbs(self.Toxic, self.TOXIC)), ptr(self.at),
+                                       ptr(self.b1), ptr(self.b2), ptr(self.bacdelta), ptr(self.ptd), ptr(self.z),
+                                       ptr(self.alpha1), ptr(self.beta1), ptr(self.delta1), ptr(self.beta2),
+                                       ptr(self.gamma2), ptr(self.delta2), ptr(self.ic)))
+        self.Vk = {"IC": _unflatten_g1(self.ic), "G1": {"Alpha": _unflatten_g1(self.alpha1)[0]},
+                   "G2": {"Beta": _unflatten_g2(self.beta2)[0], "Gamma": _unflatten_g2(self.gamma2)[0],
+                          "Delta": _unflatten_g2(self.delta2)[0]}}
+
+    def load_pk(self, window_bits=0, rank=0, world=1):
+        """The key on the device (b200_groth16_pk_load_shard): a DeviceProvingKey with prove_limbs / prove_witness_limbs."""
+        h = _lib._h(0)
+        check(lib().b200_groth16_pk_load_shard(
+            ptr(self.at), ptr(self.b1), ptr(self.b2), ptr(self.bacdelta), self.m, ptr(self.ptd), self.m - 1, ptr(self.z),
+            self.m - 1, ptr(self.alpha1), ptr(self.beta1), ptr(self.delta1), ptr(self.beta2), ptr(self.delta2),
+            self.npublic, window_bits, rank, world, h))
+        return DeviceProvingKey.from_handle(h.value, self.m)
+
+    def pk_dict(self):
+        """The key in the shape GenerateTrustedSetup returns (Python ints; small circuits only)."""
+        from ._lib import limbs_to_ints
+        return {"BACDelta": _unflatten_g1(self.bacdelta), "Z": limbs_to_ints(self.z), "PowersTauDelta": _unflatten_g1(self.ptd),
+                "G1": {"Alpha": _unflatten_g1(self.alpha1)[0], "Beta": _unflatten_g1(self.beta1)[0],
+                       "Delta": _unflatten_g1(self.delta1)[0], "At": _unflatten_g1(self.at), "BACGamma": _unflatten_g1(self.b1)},
+                "G2": {"Beta": self.Vk["G2"]["Beta"], "Gamma": self.Vk["G2"]["Gamma"], "Delta": self.Vk["G2"]["Delta"],
+                       "BACGamma": _unflatten_g2(self.b2)}}
+
+
+def GenerateTrustedSetupSparse(r1cs, nPublic, toxic=None):
+    """groth16.GenerateTrustedSetup (groth16/groth16.go:94-222) for an r1csqap.SparseR1CS of any size, on the GPU
+    (b200_groth16_setup): the same group elements as GenerateTrustedSetup for the same toxic values, as affine points.
+    ``toxic`` = dict T, Kalpha, Kbeta, Kgamma, Kdelta; drawn like the reference when omitted (T never in 1..n)."""
+    return SparseSetup(r1cs, nPublic, toxic)
 
 
 def VerifyProof(vk, proof, publicSignals, debug=False):

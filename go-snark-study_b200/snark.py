@@ -27,6 +27,13 @@ class DeviceProvingKey:
                                            len(pk["Z"]), n_public, window_bits, h))
         self.handle = h.value
 
+    @classmethod
+    def from_handle(cls, handle):
+        """Wrap a key already loaded with b200_pinocchio_pk_load(_shard)."""
+        self = cls.__new__(cls)
+        self.handle = handle
+        return self
+
     def prove_limbs(self, w_limbs, px_limbs):
         g1 = np.zeros(84, dtype=np.uint64)
         pb = np.zeros(24, dtype=np.uint64)
@@ -120,6 +127,55 @@ def GenerateTrustedSetup(witnessLength, circuit, alphas, betas, gammas, toxic=No
     toxic_out = {"T": t, "Ka": ka, "Kb": kb, "Kc": kc, "Kbeta": kbeta, "Kgamma": kgamma, "RhoA": rho_a, "RhoB": rho_b,
                  "RhoC": rho_c}
     return {"Toxic": toxic_out, "Pk": pk, "Vk": vk}
+
+
+class SparseSetup:
+    """Pinocchio key and Vk of GenerateTrustedSetupSparse as limb arrays (standard-form affine (x, y, 1) points, infinity
+    all zero): a, ap, bp, c, cp, kp (m G1), b2 (m G2), g1t (m-1 G1), z (m-1 coefficients), vk_g1 = Vkb | G1Kbg,
+    vk_g2 = Vka | Vkc | G2Kbg | G2Kg | Vkz.  ``pk_dict`` is for small circuits only."""
+    TOXIC = ("T", "Ka", "Kb", "Kc", "Kbeta", "Kgamma", "RhoA", "RhoB")
+
+    def __init__(self, r1cs, n_public, toxic=None):
+        from .groth16 import draw_toxic, toxic_limbs
+        m = self.m = r1cs.m
+        self.n, self.npublic = r1cs.n, n_public
+        tox = draw_toxic(self.TOXIC, r1cs.n) if toxic is None else dict(toxic)
+        self.Toxic = {k: int(tox[k]) for k in self.TOXIC}
+        self.Toxic["RhoC"] = self.Toxic["RhoA"] * self.Toxic["RhoB"] % R
+        g1 = lambda k: np.zeros((k, 12), dtype=np.uint64)
+        self.a, self.ap, self.bp, self.c, self.cp, self.kp = (g1(m) for _ in range(6))
+        self.b2 = np.zeros((m, 24), dtype=np.uint64)
+        self.g1t = g1(m - 1)
+        self.z = np.zeros((m - 1, 4), dtype=np.uint64)
+        self.vk_g1, self.vk_g2 = g1(2), np.zeros((5, 24), dtype=np.uint64)
+        check(lib().b200_pinocchio_setup(r1cs.handle, n_public, ptr(toxic_limbs(self.Toxic, self.TOXIC)), ptr(self.a),
+                                         ptr(self.ap), ptr(self.b2), ptr(self.bp), ptr(self.c), ptr(self.cp), ptr(self.kp),
+                                         ptr(self.g1t), ptr(self.z), ptr(self.vk_g1), ptr(self.vk_g2)))
+        self.Vk = dict(zip(("Vkb", "G1Kbg"), _unflatten_g1(self.vk_g1)))
+        self.Vk.update(zip(("Vka", "Vkc", "G2Kbg", "G2Kg", "Vkz"), _unflatten_g2(self.vk_g2)))
+        self.Vk["IC"] = _unflatten_g1(self.a[:n_public + 1])
+
+    def load_pk(self, window_bits=0, rank=0, world=1):
+        """The key on the device (b200_pinocchio_pk_load_shard): a DeviceProvingKey with prove_limbs."""
+        h = _lib._h(0)
+        check(lib().b200_pinocchio_pk_load_shard(
+            ptr(self.a), ptr(self.ap), ptr(self.b2), ptr(self.bp), ptr(self.c), ptr(self.cp), ptr(self.kp), self.m,
+            ptr(self.g1t), self.m - 1, ptr(self.z), self.m - 1, self.npublic, window_bits, rank, world, h))
+        return DeviceProvingKey.from_handle(h.value)
+
+    def pk_dict(self):
+        """The key in the shape GenerateTrustedSetup returns (Python ints; small circuits only)."""
+        from ._lib import limbs_to_ints
+        pk = {k: _unflatten_g1(getattr(self, k.lower())) for k in ("A", "Ap", "Bp", "C", "Cp", "Kp")}
+        pk.update({"B": _unflatten_g2(self.b2), "G1T": _unflatten_g1(self.g1t), "Z": limbs_to_ints(self.z)})
+        return pk
+
+
+def GenerateTrustedSetupSparse(r1cs, nPublic, toxic=None):
+    """snark.GenerateTrustedSetup (snark.go:98-251) for an r1csqap.SparseR1CS of any size, on the GPU
+    (b200_pinocchio_setup): the same group elements as GenerateTrustedSetup for the same toxic values, as affine points.
+    ``toxic`` = dict T, Ka, Kb, Kc, Kbeta, Kgamma, RhoA, RhoB; drawn like the reference when omitted (T never in 1..n)."""
+    return SparseSetup(r1cs, nPublic, toxic)
 
 
 def VerifyProof(vk, proof, publicSignals, debug=False):

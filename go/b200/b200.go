@@ -411,3 +411,97 @@ func LoadGroth16Shard(at, b1 [][3]*big.Int, b2 [][3][2]*big.Int, bacDelta, ptd [
 		C.int(rank), C.int(world), &k.h)
 	return &k, check(rc)
 }
+
+// ---- trusted setup from the sparse R1CS (b200_groth16_setup, b200_pinocchio_setup) --------------------------------------
+// groth16.GenerateTrustedSetup / snark.GenerateTrustedSetup at any size: the dense alphas / betas / gammas they take are
+// m x n matrices and cannot exist beyond a few thousand constraints.  Points are affine (x, y, 1) with infinity all zero:
+// the same group elements as the reference's for the same toxic values, not its Jacobian representatives.
+
+func g1s(w []uint64) [][3]*big.Int {
+	out := make([][3]*big.Int, len(w)/12)
+	for i := range out {
+		out[i] = G1FromLimbs(w[12*i : 12*i+12])
+	}
+	return out
+}
+func g2s(w []uint64) [][3][2]*big.Int {
+	out := make([][3][2]*big.Int, len(w)/24)
+	for i := range out {
+		out[i] = G2FromLimbs(w[24*i : 24*i+24])
+	}
+	return out
+}
+func frs(w []uint64) []*big.Int {
+	out := make([]*big.Int, len(w)/4)
+	for i := range out {
+		out[i] = fromLimbs(w[4*i : 4*i+4])
+	}
+	return out
+}
+
+// Groth16Setup holds groth16.Pk and Vk in the shapes LoadGroth16 and the verifier take.
+type Groth16Setup struct {
+	At, B1, BACDelta, PowersTauDelta, IC [][3]*big.Int
+	B2                                   [][3][2]*big.Int
+	Z                                    []*big.Int
+	Alpha1, Beta1, Delta1                [3]*big.Int
+	Beta2, Gamma2, Delta2                [3][2]*big.Int
+}
+
+// Groth16Setup is groth16.GenerateTrustedSetup (groth16/groth16.go:94-222) on this R1CS.  toxic = T, Kalpha, Kbeta,
+// Kgamma, Kdelta, each < r.
+func (r *R1CS) Groth16Setup(nPublic int, toxic [5]*big.Int) (*Groth16Setup, error) {
+	var tox []uint64
+	for _, t := range toxic {
+		tox = limbs(tox, t)
+	}
+	m := r.M
+	at, b1, cd, b2 := make([]uint64, 12*m), make([]uint64, 12*m), make([]uint64, 12*m), make([]uint64, 24*m)
+	ptd, z, ic := make([]uint64, 12*(m-1)), make([]uint64, 4*(m-1)), make([]uint64, 12*(nPublic+1))
+	a1, be1, d1 := make([]uint64, 12), make([]uint64, 12), make([]uint64, 12)
+	be2, g2, d2 := make([]uint64, 24), make([]uint64, 24), make([]uint64, 24)
+	rc := C.b200_groth16_setup(r.h, C.size_t(nPublic), u64(tox), u64(at), u64(b1), u64(b2), u64(cd), u64(ptd), u64(z),
+		u64(a1), u64(be1), u64(d1), u64(be2), u64(g2), u64(d2), u64(ic))
+	if err := check(rc); err != nil {
+		return nil, err
+	}
+	return &Groth16Setup{At: g1s(at), B1: g1s(b1), BACDelta: g1s(cd), PowersTauDelta: g1s(ptd), IC: g1s(ic), B2: g2s(b2),
+		Z: frs(z), Alpha1: G1FromLimbs(a1), Beta1: G1FromLimbs(be1), Delta1: G1FromLimbs(d1), Beta2: G2FromLimbs(be2),
+		Gamma2: G2FromLimbs(g2), Delta2: G2FromLimbs(d2)}, nil
+}
+
+// PinocchioSetup holds snark.Pk and Vk (IC = A[0..nPublic]).
+type PinocchioSetup struct {
+	A, Ap, Bp, C, Cp, Kp, G1T, IC [][3]*big.Int
+	B                             [][3][2]*big.Int
+	Z                             []*big.Int
+	Vkb, G1Kbg                    [3]*big.Int
+	Vka, Vkc, G2Kbg, G2Kg, Vkz    [3][2]*big.Int
+}
+
+// PinocchioSetup is snark.GenerateTrustedSetup (snark.go:98-251) on this R1CS.  toxic = T, Ka, Kb, Kc, Kbeta, Kgamma,
+// RhoA, RhoB, each < r.
+func (r *R1CS) PinocchioSetup(nPublic int, toxic [8]*big.Int) (*PinocchioSetup, error) {
+	var tox []uint64
+	for _, t := range toxic {
+		tox = limbs(tox, t)
+	}
+	m := r.M
+	g1 := make([][]uint64, 6)
+	for k := range g1 {
+		g1[k] = make([]uint64, 12*m)
+	}
+	b2, g1t, z := make([]uint64, 24*m), make([]uint64, 12*(m-1)), make([]uint64, 4*(m-1))
+	vk1, vk2 := make([]uint64, 24), make([]uint64, 120)
+	rc := C.b200_pinocchio_setup(r.h, C.size_t(nPublic), u64(tox), u64(g1[0]), u64(g1[1]), u64(b2), u64(g1[2]), u64(g1[3]),
+		u64(g1[4]), u64(g1[5]), u64(g1t), u64(z), u64(vk1), u64(vk2))
+	if err := check(rc); err != nil {
+		return nil, err
+	}
+	s := &PinocchioSetup{A: g1s(g1[0]), Ap: g1s(g1[1]), Bp: g1s(g1[2]), C: g1s(g1[3]), Cp: g1s(g1[4]), Kp: g1s(g1[5]),
+		G1T: g1s(g1t), B: g2s(b2), Z: frs(z), Vkb: G1FromLimbs(vk1[:12]), G1Kbg: G1FromLimbs(vk1[12:]),
+		Vka: G2FromLimbs(vk2[:24]), Vkc: G2FromLimbs(vk2[24:48]), G2Kbg: G2FromLimbs(vk2[48:72]),
+		G2Kg: G2FromLimbs(vk2[72:96]), Vkz: G2FromLimbs(vk2[96:])}
+	s.IC = s.A[:nPublic+1]
+	return s, nil
+}

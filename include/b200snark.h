@@ -305,6 +305,32 @@ int b200_qap_px(b200_r1cs_t h, const uint64_t* w, size_t nw, uint64_t* ax, uint6
  * zt = prod_{i=1..nz} (tau - i) (groth16.go:122-136 with nz = len(alphas) - 2).  tau must not be one of 1..n.          */
 int b200_qap_eval_at(b200_r1cs_t h, const uint64_t tau[4], size_t nz, uint64_t* at, uint64_t* bt, uint64_t* ct,
                      uint64_t zt[4]);
+/* ---- trusted setup for a sparse R1CS of any size ----
+ * groth16.GenerateTrustedSetup (groth16/groth16.go:94-222) and snark.GenerateTrustedSetup (snark.go:98-251) from the
+ * resident R1CS (m = its signals, n = its constraints): at / bt / ct = A^T l(T) etc. as in b200_qap_eval_at,
+ * Z = prod_{i=1..m-2}(x - i) as in b200_zero_poly, every CRS scalar derived on the device, and every point minted by a
+ * fixed-base windowed kernel.  The outputs have the shapes b200_groth16_pk_load(_shard) / b200_pinocchio_pk_load(_shard)
+ * take.  All pointers are host pointers; the call is synchronous and runs on the library stream.
+ *   - Points are affine (x, y, 1) in standard form, infinity all zero.  They are the same group elements as the
+ *     reference's for the same toxic values, not its Jacobian representatives (use the dense setup through
+ *     b200_g1/g2_mul_batch_bcast for X,Y,Z-exact points).
+ *   - A bad handle, a null pointer, m < 3, or npublic >= m returns B200_EINVAL.
+ *   - A toxic value >= r returns B200_ERANGE.
+ *   - T in {1..n} returns B200_EINVAL (as b200_qap_eval_at).
+ * The reference's k == a + b + c self-check (snark.go:194-199) holds by construction and is not repeated.            */
+/* toxic = T, Kalpha, Kbeta, Kgamma, Kdelta (4 limbs each); Kgamma or Kdelta = 0 returns B200_EINVAL.
+ * Outputs: at, b1, bacdelta: m G1 points (BACDelta[0..npublic] infinity); b2: m G2 points; ptd: m-1 G1 points;
+ * z: m-1 coefficients; ic: npublic+1 G1 points.                                                                     */
+int b200_groth16_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[20], uint64_t* at, uint64_t* b1,
+                       uint64_t* b2, uint64_t* bacdelta, uint64_t* ptd, uint64_t* z, uint64_t alpha1[12],
+                       uint64_t beta1[12], uint64_t delta1[12], uint64_t beta2[24], uint64_t gamma2[24],
+                       uint64_t delta2[24], uint64_t* ic);
+/* toxic = T, Ka, Kb, Kc, Kbeta, Kgamma, RhoA, RhoB (RhoC = RhoA * RhoB).
+ * Outputs: a, ap, bp, c, cp, kp: m G1 points; b2: m G2 points; g1t: m-1 G1 points (T^0 .. T^(m-2)); z: m-1
+ * coefficients; vk_g1 = Vkb | G1Kbg; vk_g2 = Vka | Vkc | G2Kbg | G2Kg | Vkz.  The Vk's IC is a[0..npublic].           */
+int b200_pinocchio_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[32], uint64_t* a, uint64_t* ap,
+                         uint64_t* b2, uint64_t* bp, uint64_t* c, uint64_t* cp, uint64_t* kp, uint64_t* g1t, uint64_t* z,
+                         uint64_t vk_g1[24], uint64_t vk_g2[120]);
 /* PolynomialField.LagrangeInterpolation over x = 1..n (r1csqap/r1csqap.go:150-158) at any n <= 2^26: n values ->
  * n coefficients.                                                                                                    */
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs);
