@@ -37,19 +37,40 @@ std::mutex g_mu;
 std::string g_err;
 bool g_init = false;
 int g_device = -1;
-cudaStream_t g_stream = nullptr;
-cudaStream_t g_side[4] = {nullptr, nullptr, nullptr, nullptr};  // side streams: independent MSMs of one proof overlap
-// Second prove context (B200_CFG_PK_CONTEXT): a proving key loaded under context 1 runs on its own side streams and
-// polynomial workspace, so a proof on it can be in flight beside a proof on a context-0 key (two proofs pipelined on two
-// caller streams: the latency-bound sort / tail / product chains of one overlap the accumulation of the other).
-cudaStream_t g_side1[4] = {nullptr, nullptr, nullptr, nullptr};
-cudaStream_t g_stream1 = nullptr;   // context 1's main stream (host-pointer entry points)
+// Prove context (B200_CFG_PK_CONTEXT): what a proof on a key loaded under it runs on.  A proof on a context-1 key can be in
+// flight beside a proof on a context-0 key (two proofs pipelined on two caller streams: the latency-bound sort / tail /
+// product chains of one overlap the accumulation of the other).  Every other library call runs on context 0's main stream
+// and polynomial workspace.
+struct ProveCtx {
+  cudaStream_t main = nullptr;   // host-pointer proofs on this context's keys
+  cudaStream_t side[3] = {nullptr, nullptr, nullptr};   // side streams: independent MSMs of one proof overlap
+  std::unique_ptr<PolyCtx> poly;
+  // NCCL communicator of the all-gathers (b200_comm_init).  Context 1 gathers on its own (ncclCommSplit of context 0's):
+  // NCCL matches collectives by issue order per communicator, and two host threads proving on the two contexts reach
+  // their all-gathers in an order that differs from rank to rank.  Without ncclCommSplit it is context 0's.
+  ncclComm_t comm = nullptr;
+};
+ProveCtx g_ctx[2];
 int g_pk_ctx = 0;
 int g_pairing_kernel = 0;   // B200_CFG_PAIRING_KERNEL: 0 auto, 1 one thread per pairing, 2 one warp per pairing
-int* g_d_err = nullptr;  // device error flags (bit0: coordinate >= q, bit1: scalar >= r, bit2: zero leading coeff)
-std::unique_ptr<PolyCtx> g_poly, g_poly1;
+// device error flags of the calls that hold the library mutex until they have waited (bit0: coordinate >= q, bit1: scalar
+// >= r, bit2: zero leading coeff)
+int* g_d_err = nullptr;
 
-Comm g_comm;  // NCCL communicator of this process (b200_comm_init); world 1 = none
+Comm g_comm;  // NCCL library, rank and world of this process (b200_comm_init); world 1 = none
+bool comm_active() { return g_ctx[0].comm != nullptr; }
+
+// Waits for the device, then destroys the communicators of both prove contexts (a shared one once).
+void comm_destroy_locked() {
+  if (!comm_active()) return;
+  cudaSetDevice(g_device);
+  cudaDeviceSynchronize();
+  if (g_ctx[1].comm != g_ctx[0].comm) g_comm.api.CommDestroy(g_ctx[1].comm);
+  g_comm.api.CommDestroy(g_ctx[0].comm);
+  for (auto& c : g_ctx) c.comm = nullptr;
+  g_comm.world = 1;
+  g_comm.rank = 0;
+}
 
 // b200_config: bucket-accumulation kernel of base sets / proving keys created afterwards
 // (0 auto: batched affine where the bucket population and the shard size amortise its rounds, else XYZZ; 1, 2 force)
@@ -116,16 +137,14 @@ int init_locked(int device) {
   }
   if (device >= count) return fail(B200_EINVAL, "device %d out of range (%d devices)", device, count);
   CU(cudaSetDevice(device));
-  CU(cudaStreamCreateWithFlags(&g_stream, cudaStreamNonBlocking));
-  for (auto& sd : g_side) CU(cudaStreamCreateWithFlags(&sd, cudaStreamNonBlocking));  // (stream priorities: no measurable effect)
+  for (auto& c : g_ctx) {
+    CU(cudaStreamCreateWithFlags(&c.main, cudaStreamNonBlocking));
+    for (auto& sd : c.side) CU(cudaStreamCreateWithFlags(&sd, cudaStreamNonBlocking));  // (stream priorities: no measurable effect)
+    c.poly = std::make_unique<PolyCtx>();
+    c.poly->launch_counter = &g_launches;
+  }
   CU(cudaMalloc(&g_d_err, sizeof(int)));
   CU(cudaMemset(g_d_err, 0, sizeof(int)));
-  for (auto& sd : g_side1) CU(cudaStreamCreateWithFlags(&sd, cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(&g_stream1, cudaStreamNonBlocking));
-  g_poly = std::make_unique<PolyCtx>();
-  g_poly->launch_counter = &g_launches;
-  g_poly1 = std::make_unique<PolyCtx>();
-  g_poly1->launch_counter = &g_launches;
   g_device = device;
   g_init = true;
   return B200_OK;
@@ -194,23 +213,24 @@ int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
 std::map<uint64_t, std::unique_ptr<Bases>> g_bases;
 uint64_t g_next_handle = 1;
 
-// Reads the device error flags behind everything queued on `st` and waits for the stream.  With `lk` (the library mutex,
-// held by the caller) the wait itself runs UNLOCKED, so a second host thread can enqueue a proof on the other prove
-// context meanwhile (two host-pointer proofs in flight, B200_CFG_PK_CONTEXT).
-template <class F>
-int check_err_flag(const char* what, cudaStream_t st = nullptr, std::unique_lock<std::mutex>* lk = nullptr, int* pinned = nullptr) {
-  if (!st) st = g_stream;
+// Reads the device error word `d_err` behind everything queued on `st` and waits for the stream.  With `lk` (the library
+// mutex, held by the caller) the wait itself runs UNLOCKED, so a second host thread can enqueue a proof on the other prove
+// context meanwhile (two host-pointer proofs in flight, B200_CFG_PK_CONTEXT).  A set word is cleared on `st`, behind the
+// read, so the next call that uses the word on that stream starts from zero.
+int check_err_flag(const char* what, int* d_err, cudaStream_t st = nullptr, std::unique_lock<std::mutex>* lk = nullptr,
+                   int* pinned = nullptr) {
+  if (!st) st = g_ctx[0].main;
   int h_local = 0;
   int* hp = pinned ? pinned : &h_local;   // `pinned`: a page-locked word, so the copy does not block the host under the mutex
   *hp = 0;
-  CU(cudaMemcpyAsync(hp, g_d_err, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(hp, d_err, sizeof(int), cudaMemcpyDeviceToHost, st));
   if (lk) lk->unlock();
   cudaError_t se = cudaStreamSynchronize(st);
   if (lk) lk->lock();
   CU(se);
   const int h = *hp;
   if (h) {
-    CU(cudaMemset(g_d_err, 0, sizeof(int)));
+    CU(cudaMemsetAsync(d_err, 0, sizeof(int), st));
     if (h & 16) return fail(B200_EINVAL, "%s: tau is one of the interpolation points 1..n", what);
     if (h & 8) return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (G2 point at infinity; the reference panics, bn128.go:238-241)", what);
     if (h & 4) return fail(B200_EDIVZERO, "%s: divisor has a zero leading coefficient", what);
@@ -281,10 +301,10 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   DevBuf staging, state;
   CU(staging.alloc(n * 3 * sizeof(F)));
   CU(state.alloc(n * sizeof(XYZZ<F>)));
-  CU(cudaMemcpyAsync(staging.p, pts, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_stream));
-  window_table_enqueue<F>(staging.as<F>(), n, sh.nwin, c, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_d_err, g_stream);
+  CU(cudaMemcpyAsync(staging.p, pts, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
+  window_table_enqueue<F>(staging.as<F>(), n, sh.nwin, c, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_d_err, g_ctx[0].main);
   CU(cudaGetLastError());
-  int rc = check_err_flag<F>("bases_load");
+  int rc = check_err_flag("bases_load", g_d_err);
   if (rc) return rc;
   out_b = std::move(b);
   return B200_OK;
@@ -508,12 +528,12 @@ int msm_host(b200_bases_t h, int group, const uint64_t* scalars, size_t n, uint6
   Bases* b = find_bases(h, group);
   if (!b) return fail(B200_EINVAL, "msm: bad handle");
   if ((!scalars && n) || !out) return fail(B200_EINVAL, "msm: null pointer");
-  if (n) CU(cudaMemcpyAsync(b->scalars.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  int rc = msm_enqueue<F>(b, b->scalars.as<Fr>(), n, 0, b->result.as<XYZZ<F>>(), g_d_err, g_stream);
+  if (n) CU(cudaMemcpyAsync(b->scalars.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  int rc = msm_enqueue<F>(b, b->scalars.as<Fr>(), n, 0, b->result.as<XYZZ<F>>(), g_d_err, g_ctx[0].main);
   if (rc) return rc;
-  k_finalize<F><<<1, 32, 0, g_stream>>>(b->result.as<XYZZ<F>>(), b->out_std.as<F>());
-  CU(cudaMemcpyAsync(out, b->out_std.p, 3 * sizeof(F), cudaMemcpyDeviceToHost, g_stream));
-  rc = check_err_flag<F>("msm");  // synchronises the stream
+  k_finalize<F><<<1, 32, 0, g_ctx[0].main>>>(b->result.as<XYZZ<F>>(), b->out_std.as<F>());
+  CU(cudaMemcpyAsync(out, b->out_std.p, 3 * sizeof(F), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  rc = check_err_flag("msm", g_d_err);  // synchronises the stream
   return rc;
 }
 
@@ -539,12 +559,12 @@ int mul_batch(const uint64_t* pts, int bcast, const uint64_t* scalars, size_t n,
   CU(dp.alloc(np * 3 * sizeof(F)));
   CU(ds.alloc(n * sizeof(Fr)));
   CU(dout.alloc(n * 3 * sizeof(F)));
-  CU(cudaMemcpyAsync(dp.p, pts, np * 3 * sizeof(F), cudaMemcpyHostToDevice, g_stream));
-  CU(cudaMemcpyAsync(ds.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  k_mul_batch_ref<F><<<nblocks(n, 128), 128, 0, g_stream>>>(dp.as<F>(), bcast, ds.as<Fr>(), n, dout.as<F>(), g_d_err);
+  CU(cudaMemcpyAsync(dp.p, pts, np * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
+  CU(cudaMemcpyAsync(ds.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  k_mul_batch_ref<F><<<nblocks(n, 128), 128, 0, g_ctx[0].main>>>(dp.as<F>(), bcast, ds.as<Fr>(), n, dout.as<F>(), g_d_err);
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, dout.p, n * 3 * sizeof(F), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<F>("mul_batch");
+  CU(cudaMemcpyAsync(out, dout.p, n * 3 * sizeof(F), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("mul_batch", g_d_err);
 }
 
 int poly_mul_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, uint64_t* out) {
@@ -554,21 +574,21 @@ int poly_mul_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, ui
   CU(da.alloc(na * sizeof(Fr)));
   CU(db.alloc(nb * sizeof(Fr)));
   CU(dout.alloc((na + nb - 1) * sizeof(Fr)));
-  CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  CU(cudaMemcpyAsync(db.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  CU(poly_mul_device(*g_poly, da.as<Fr>(), na, 0, db.as<Fr>(), nb, 0, dout.as<Fr>(), g_d_err, g_stream));
-  CU(cudaMemcpyAsync(out, dout.p, (na + nb - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fr>("poly_mul");
+  CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  CU(cudaMemcpyAsync(db.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  CU(poly_mul_device(*g_ctx[0].poly, da.as<Fr>(), na, 0, db.as<Fr>(), nb, 0, dout.as<Fr>(), g_d_err, g_ctx[0].main));
+  CU(cudaMemcpyAsync(out, dout.p, (na + nb - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("poly_mul", g_d_err);
 }
 
 int divisor_init(Divisor& dv, const uint64_t* b, size_t nb) {
   DevBuf tmp;
   CU(tmp.alloc(nb * sizeof(Fr)));
   CU(dv.b_mont.alloc(nb * sizeof(Fr)));
-  CU(cudaMemcpyAsync(tmp.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  k_poly_load<<<nblk(nb, 256), 256, 0, g_stream>>>(tmp.as<Fr>(), (uint32_t)nb, (uint32_t)nb, 0, 0, dv.b_mont.as<Fr>(),
+  CU(cudaMemcpyAsync(tmp.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  k_poly_load<<<nblk(nb, 256), 256, 0, g_ctx[0].main>>>(tmp.as<Fr>(), (uint32_t)nb, (uint32_t)nb, 0, 0, dv.b_mont.as<Fr>(),
                                                     (uint32_t)nb, g_d_err);
-  CU(cudaStreamSynchronize(g_stream));
+  CU(cudaStreamSynchronize(g_ctx[0].main));
   dv.nb = nb;
   return B200_OK;
 }
@@ -588,11 +608,11 @@ int poly_div_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, ui
   CU(da.alloc(na * sizeof(Fr)));
   CU(dq.alloc(nq * sizeof(Fr)));
   if (rem && nb > 1) CU(dr.alloc((nb - 1) * sizeof(Fr)));
-  CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  CU(poly_div_device(*g_poly, dv, da.as<Fr>(), na, 0, dq.as<Fr>(), dr.as<Fr>(), g_d_err, g_stream));
-  CU(cudaMemcpyAsync(q, dq.p, nq * sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  if (rem && nb > 1) CU(cudaMemcpyAsync(rem, dr.p, (nb - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fr>("poly_div");
+  CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  CU(poly_div_device(*g_ctx[0].poly, dv, da.as<Fr>(), na, 0, dq.as<Fr>(), dr.as<Fr>(), g_d_err, g_ctx[0].main));
+  CU(cudaMemcpyAsync(q, dq.p, nq * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  if (rem && nb > 1) CU(cudaMemcpyAsync(rem, dr.p, (nb - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("poly_div", g_d_err);
 }
 
 #include "prove_host.cuh"
@@ -615,7 +635,7 @@ int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint6
   if (rc) return rc;
   // the quotient is only consumed on side stream 3 (groth16_enqueue): compute it THERE, so the QAP front end (NTT passes,
   // HBM-bound) overlaps the A / B1 / B2 bucket phases (multiply-bound) on the other streams
-  cudaStream_t sq = g_serial ? st : pk->side()[2];
+  cudaStream_t sq = g_serial ? st : pk->pctx().side[2];
   if (sq != st) {
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
@@ -623,10 +643,10 @@ int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint6
   // h = (ax*bx - cx) / Z straight from the witness (no px): the shape the reference supports has Z = prod_{i<=n}(x - i)
   // (m = n + 2, SURVEY H5) — checked; anything else goes through px and the division.
   if (r1->n >= 2 && pk->Z.nb == r1->n + 1) {
-    if ((rc = qap_h_enqueue(r1, *ws, pk->poly(), d_w, err, sq))) return rc;
+    if ((rc = qap_h_enqueue(r1, *ws, *pk->pctx().poly, d_w, err, sq))) return rc;
     return groth16_enqueue(pk, d_w, pk->m, nullptr, npx, r, s, d_out, st, err, 0, ws->h_std.as<Fr>());
   }
-  if ((rc = qap_px_enqueue(r1, *ws, pk->poly(), d_w, nullptr, nullptr, err, sq))) return rc;
+  if ((rc = qap_px_enqueue(r1, *ws, *pk->pctx().poly, d_w, nullptr, nullptr, err, sq))) return rc;
   return groth16_enqueue(pk, d_w, pk->m, ws->px_mont.as<Fr>(), npx, r, s, d_out, st, err, /*px_mont=*/1);
 }
 
@@ -639,12 +659,12 @@ int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t
   if (nw != pk->m || nw != r1->m) return fail(B200_EINVAL, "groth16_prove_witness: witness length %zu, NVars %zu, R1CS columns %zu", nw, pk->m, r1->m);
   int rc = check_sharded_host_call(pk, "groth16_prove_witness", "b200_groth16_prove_witness_device");
   if (rc) return rc;
-  cudaStream_t st = pk->main();
+  cudaStream_t st = pk->pctx().main;
   // the QAP front end reads the whole witness; a rank that runs none reads only its own index ranges
   if ((rc = stage_witness(pk, w, pk_needs_px(pk), st))) return rc;
   Fq* o = pk->out_std.as<Fq>();
-  if ((rc = groth16_witness_enqueue(pk, r1, pk->w_stage.as<Fr>(), r, s, o, st, g_d_err))) return rc;
-  return finish_host_proof(pk, o, "groth16_prove_witness", st, lk, pi_a, pi_b, pi_c);
+  if ((rc = groth16_witness_enqueue(pk, r1, pk->w_stage.as<Fr>(), r, s, o, st, pk->d_err_sync.as<int>()))) return rc;
+  return finish_host_proof(pk, o, "groth16_prove_witness", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
 }
 
 // ---- dense QAP API (small n) -------------------------------------------------
@@ -652,7 +672,7 @@ int r1cs_to_qap_host(const uint64_t* a, const uint64_t* b, const uint64_t* c, si
                      uint64_t* betas, uint64_t* gammas, uint64_t* z) {
   if (!a || !b || !c || !alphas || !betas || !gammas || !z) return fail(B200_EINVAL, "r1cs_to_qap: null pointer");
   if (n == 0 || m < 2 || n > 8191 || m > 8193) return fail(B200_EINVAL, "r1cs_to_qap: dense API supports 1 <= n <= 8191");
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   DevBuf zn, L, M, out, zz;
   size_t nz = m - 2;  // Z = prod_{i=1}^{m-2} (x - i)   (r1csqap.go:177-186)
   size_t zmax = (n > nz ? n : nz) + 1;
@@ -676,14 +696,14 @@ int r1cs_to_qap_host(const uint64_t* a, const uint64_t* b, const uint64_t* c, si
   k_poly_store<<<nblk(nz + 1, 256), 256, 0, st>>>(zn.as<Fr>(), (uint32_t)(nz + 1), 0, 1, zz.as<Fr>());
   CU(cudaMemcpyAsync(z, zz.p, (nz + 1) * sizeof(Fr), cudaMemcpyDeviceToHost, st));
   CU(cudaGetLastError());
-  return check_err_flag<Fr>("r1cs_to_qap");
+  return check_err_flag("r1cs_to_qap", g_d_err);
 }
 
 int combine_polynomials_host(const uint64_t* r, size_t m, const uint64_t* ap, const uint64_t* bp, const uint64_t* cp,
                              size_t n, uint64_t* ax, uint64_t* bx, uint64_t* cx, uint64_t* px) {
   if (!r || !ap || !bp || !cp || !ax || !bx || !cx || !px || m == 0 || n == 0)
     return fail(B200_EINVAL, "combine_polynomials: bad arguments");
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   DevBuf dr, dP, mont[3], stdv[3], prod;
   CU(dr.alloc(m * sizeof(Fr)));
   CU(dP.alloc(m * n * sizeof(Fr)));
@@ -701,12 +721,12 @@ int combine_polynomials_host(const uint64_t* r, size_t m, const uint64_t* ap, co
     CU(cudaStreamSynchronize(st));
   }
   // px = ax*bx - cx   (r1csqap.go:208)
-  CU(poly_mul_device(*g_poly, mont[0].as<Fr>(), n, 1, mont[1].as<Fr>(), n, 1, prod.as<Fr>(), g_d_err, st));
+  CU(poly_mul_device(*g_ctx[0].poly, mont[0].as<Fr>(), n, 1, mont[1].as<Fr>(), n, 1, prod.as<Fr>(), g_d_err, st));
   k_poly_addsub<<<nblk(2 * n - 1, 256), 256, 0, st>>>(prod.as<Fr>(), (uint32_t)(2 * n - 1), stdv[2].as<Fr>(), (uint32_t)n, 1,
                                                       prod.as<Fr>(), g_d_err);
   CU(cudaMemcpyAsync(px, prod.p, (2 * n - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, st));
   CU(cudaGetLastError());
-  return check_err_flag<Fr>("combine_polynomials");
+  return check_err_flag("combine_polynomials", g_d_err);
 }
 
 int poly_addsub_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, int sub, uint64_t* out) {
@@ -717,11 +737,11 @@ int poly_addsub_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb,
   CU(da.alloc((na ? na : 1) * sizeof(Fr)));
   CU(db.alloc((nb ? nb : 1) * sizeof(Fr)));
   CU(dout.alloc(n * sizeof(Fr)));
-  if (na) CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  if (nb) CU(cudaMemcpyAsync(db.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  k_poly_addsub<<<nblk(n, 256), 256, 0, g_stream>>>(da.as<Fr>(), (uint32_t)na, db.as<Fr>(), (uint32_t)nb, sub, dout.as<Fr>(), g_d_err);
-  CU(cudaMemcpyAsync(out, dout.p, n * sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fr>("poly_add/sub");
+  if (na) CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  if (nb) CU(cudaMemcpyAsync(db.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  k_poly_addsub<<<nblk(n, 256), 256, 0, g_ctx[0].main>>>(da.as<Fr>(), (uint32_t)na, db.as<Fr>(), (uint32_t)nb, sub, dout.as<Fr>(), g_d_err);
+  CU(cudaMemcpyAsync(out, dout.p, n * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("poly_add/sub", g_d_err);
 }
 
 int poly_eval_host(const uint64_t* v, size_t n, const uint64_t* x, uint64_t* out) {
@@ -729,12 +749,12 @@ int poly_eval_host(const uint64_t* v, size_t n, const uint64_t* x, uint64_t* out
   DevBuf dv, dout;
   CU(dv.alloc((n ? n : 1) * sizeof(Fr)));
   CU(dout.alloc(sizeof(Fr)));
-  if (n) CU(cudaMemcpyAsync(dv.p, v, n * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
+  if (n) CU(cudaMemcpyAsync(dv.p, v, n * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
   Fr xs = fr_load_std(x);
   if (xs.geq_modulus()) return fail(B200_ERANGE, "poly_eval: x >= r");
-  k_poly_eval<<<1, 256, 0, g_stream>>>(dv.as<Fr>(), (uint32_t)n, xs, dout.as<Fr>(), g_d_err);
-  CU(cudaMemcpyAsync(out, dout.p, sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fr>("poly_eval");
+  k_poly_eval<<<1, 256, 0, g_ctx[0].main>>>(dv.as<Fr>(), (uint32_t)n, xs, dout.as<Fr>(), g_d_err);
+  CU(cudaMemcpyAsync(out, dout.p, sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("poly_eval", g_d_err);
 }
 
 int poly_eval_batch_host(const uint64_t* polys, size_t m, size_t n, const uint64_t* x, uint64_t* out) {
@@ -744,11 +764,11 @@ int poly_eval_batch_host(const uint64_t* polys, size_t m, size_t n, const uint64
   DevBuf dp, dout;
   CU(dp.alloc(m * n * sizeof(Fr)));
   CU(dout.alloc(m * sizeof(Fr)));
-  CU(cudaMemcpyAsync(dp.p, polys, m * n * sizeof(Fr), cudaMemcpyHostToDevice, g_stream));
-  k_poly_eval_batch<<<(unsigned)m, 64, 0, g_stream>>>(dp.as<Fr>(), (uint32_t)n, xs, dout.as<Fr>(), g_d_err);
+  CU(cudaMemcpyAsync(dp.p, polys, m * n * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  k_poly_eval_batch<<<(unsigned)m, 64, 0, g_ctx[0].main>>>(dp.as<Fr>(), (uint32_t)n, xs, dout.as<Fr>(), g_d_err);
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, dout.p, m * sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fr>("poly_eval_batch");
+  CU(cudaMemcpyAsync(out, dout.p, m * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("poly_eval_batch", g_d_err);
 }
 
 int zero_poly_host(size_t n, uint64_t* out) {   // coefficients of prod_{i=1..n} (x - i), n + 1 of them
@@ -757,15 +777,15 @@ int zero_poly_host(size_t n, uint64_t* out) {   // coefficients of prod_{i=1..n}
   CU(zz.alloc((n + 1) * sizeof(Fr)));
   if (n <= 2048) {   // one-block schoolbook; above: Newton basis element n through the subproduct tree (qap_sparse.cuh)
     CU(zn.alloc((n + 1) * sizeof(Fr)));
-    k_zero_poly<<<1, 1024, 0, g_stream>>>(zn.as<Fr>(), (uint32_t)n);
+    k_zero_poly<<<1, 1024, 0, g_ctx[0].main>>>(zn.as<Fr>(), (uint32_t)n);
   } else {
-    int rc = zero_poly_device(n, zn, g_stream);
+    int rc = zero_poly_device(n, zn, g_ctx[0].main);
     if (rc) return rc;
   }
-  k_poly_store<<<nblk(n + 1, 256), 256, 0, g_stream>>>(zn.as<Fr>(), (uint32_t)(n + 1), 0, 1, zz.as<Fr>());
+  k_poly_store<<<nblk(n + 1, 256), 256, 0, g_ctx[0].main>>>(zn.as<Fr>(), (uint32_t)(n + 1), 0, 1, zz.as<Fr>());
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, zz.p, (n + 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fr>("zero_poly");
+  CU(cudaMemcpyAsync(out, zz.p, (n + 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("zero_poly", g_d_err);
 }
 
 #ifndef B200_NO_PAIRING
@@ -928,16 +948,16 @@ int pairing_batch_host(const uint64_t* g1, const uint64_t* g2, size_t n, uint64_
   CU(d1.alloc(n * 3 * sizeof(Fq)));
   CU(d2.alloc(n * 3 * sizeof(Fq2)));
   CU(dout.alloc(n * 6 * sizeof(Fq2)));
-  CU(cudaMemcpyAsync(d1.p, g1, n * 3 * sizeof(Fq), cudaMemcpyHostToDevice, g_stream));
-  CU(cudaMemcpyAsync(d2.p, g2, n * 3 * sizeof(Fq2), cudaMemcpyHostToDevice, g_stream));
+  CU(cudaMemcpyAsync(d1.p, g1, n * 3 * sizeof(Fq), cudaMemcpyHostToDevice, g_ctx[0].main));
+  CU(cudaMemcpyAsync(d2.p, g2, n * 3 * sizeof(Fq2), cudaMemcpyHostToDevice, g_ctx[0].main));
   // auto: a warp per pairing has the much shorter latency and wins for small calls; above that the thread-per-pairing
   // kernel keeps more pairings resident and has the higher throughput
   const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
-  if (thread_kernel) k_pairing_batch<kFastFinalExp><<<nblk(n, 32), 32, 0, g_stream>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
-  else k_pairing_batch_warp<<<nblk(n, kPairWarps), 32 * kPairWarps, 0, g_stream>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
+  if (thread_kernel) k_pairing_batch<kFastFinalExp><<<nblk(n, 32), 32, 0, g_ctx[0].main>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
+  else k_pairing_batch_warp<<<nblk(n, kPairWarps), 32 * kPairWarps, 0, g_ctx[0].main>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, dout.p, n * 6 * sizeof(Fq2), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fq>("pairing_batch");
+  CU(cudaMemcpyAsync(out, dout.p, n * 6 * sizeof(Fq2), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("pairing_batch", g_d_err);
 }
 
 int fq12_mul_batch_host(const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) {
@@ -948,12 +968,12 @@ int fq12_mul_batch_host(const uint64_t* a, const uint64_t* b, size_t n, uint64_t
   CU(da.alloc(bytes));
   CU(db.alloc(bytes));
   CU(dout.alloc(bytes));
-  CU(cudaMemcpyAsync(da.p, a, bytes, cudaMemcpyHostToDevice, g_stream));
-  CU(cudaMemcpyAsync(db.p, b, bytes, cudaMemcpyHostToDevice, g_stream));
-  k_fq12_mul_batch<<<nblk(n, 32), 32, 0, g_stream>>>(da.as<Fq2>(), db.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
+  CU(cudaMemcpyAsync(da.p, a, bytes, cudaMemcpyHostToDevice, g_ctx[0].main));
+  CU(cudaMemcpyAsync(db.p, b, bytes, cudaMemcpyHostToDevice, g_ctx[0].main));
+  k_fq12_mul_batch<<<nblk(n, 32), 32, 0, g_ctx[0].main>>>(da.as<Fq2>(), db.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, dout.p, bytes, cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<Fq>("fq12_mul_batch");
+  CU(cudaMemcpyAsync(out, dout.p, bytes, cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("fq12_mul_batch", g_d_err);
 }
 
 int groth16_verify_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2,
@@ -976,7 +996,7 @@ int groth16_verify_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1,
   CU(d1.alloc(4 * 3 * sizeof(Fq)));
   CU(d2.alloc(4 * 3 * sizeof(Fq2)));
   CU(dok.alloc(sizeof(int)));
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   CU(cudaMemcpyAsync(dic.p, ic, n_ic * 3 * sizeof(Fq), cudaMemcpyHostToDevice, st));
   if (npub) CU(cudaMemcpyAsync(dsig.p, gs.data(), npub * sizeof(GlvScalar), cudaMemcpyHostToDevice, st));
   Fq* p1 = d1.as<Fq>();
@@ -993,7 +1013,7 @@ int groth16_verify_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1,
   k_groth16_verify<<<1, 128, 0, st>>>(p1, p2, dok.as<int>(), g_d_err);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(ok, dok.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  return check_err_flag<Fq>("groth16_verify");
+  return check_err_flag("groth16_verify", g_d_err);
 }
 
 #else  // experiment builds without the verifier side (ptxas 12.9 crashes on the pairing kernels under -DB200_KARATSUBA)
@@ -1013,18 +1033,18 @@ int group_op_host(int op, const uint64_t* p, const uint64_t* q, size_t n, uint64
   size_t out_fe = op == 3 ? 2 : 3;
   CU(dp.alloc(n * 3 * sizeof(F)));
   CU(dout.alloc(n * out_fe * sizeof(F)));
-  CU(cudaMemcpyAsync(dp.p, p, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_stream));
+  CU(cudaMemcpyAsync(dp.p, p, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
   if (op == 0) {
     CU(dq.alloc(n * 3 * sizeof(F)));
-    CU(cudaMemcpyAsync(dq.p, q, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_stream));
+    CU(cudaMemcpyAsync(dq.p, q, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
   }
   if (op == 3)
-    k_group_affine<F><<<nblk(n, 128), 128, 0, g_stream>>>(dp.as<F>(), n, dout.as<F>(), g_d_err);
+    k_group_affine<F><<<nblk(n, 128), 128, 0, g_ctx[0].main>>>(dp.as<F>(), n, dout.as<F>(), g_d_err);
   else
-    k_group_op<F><<<nblk(n, 128), 128, 0, g_stream>>>(op, dp.as<F>(), dq.as<F>(), n, dout.as<F>(), g_d_err);
+    k_group_op<F><<<nblk(n, 128), 128, 0, g_ctx[0].main>>>(op, dp.as<F>(), dq.as<F>(), n, dout.as<F>(), g_d_err);
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, dout.p, n * out_fe * sizeof(F), cudaMemcpyDeviceToHost, g_stream));
-  return check_err_flag<F>("group op");
+  CU(cudaMemcpyAsync(out, dout.p, n * out_fe * sizeof(F), cudaMemcpyDeviceToHost, g_ctx[0].main));
+  return check_err_flag("group op", g_d_err);
 }
 
 #include "setup_host.cuh"
@@ -1066,7 +1086,7 @@ int b200_groth16_finalize_device(b200_pk_t pk, const void* d_parts, int nparts, 
   ProvingKey* p = find_pk(pk, 1);
   if (!p || !d_parts || nparts < 1 || !r || !s || !d_out) return fail(B200_EINVAL, "groth16_finalize_device: bad arguments");
   return drain_on_error(groth16_finalize_enqueue(p, (const uint8_t*)d_parts, nparts, r, s, (Fq*)d_out,
-                                  stream ? (cudaStream_t)stream : g_stream));
+                                  stream ? (cudaStream_t)stream : g_ctx[0].main));
 }
 int b200_groth16_prove(b200_pk_t pk, const uint64_t* w, size_t nw, const uint64_t* px, size_t npx,
                        const uint64_t r[4], const uint64_t s[4], uint64_t pi_a[12], uint64_t pi_b[24],
@@ -1095,9 +1115,7 @@ int b200_pinocchio_prove_record_device(b200_pk_t pk, const uint64_t* w, size_t n
   std::lock_guard<std::mutex> lk(g_mu);
   NEED_INIT();
   if (!d_record) return fail(B200_EINVAL, "pinocchio_prove_record_device: null record pointer");
-  int rc = pinocchio_prove(pk, w, nw, px, npx, nullptr, nullptr, (uint8_t*)d_record);
-  if (rc) return rc;
-  return check_err_flag<Fr>("pinocchio_prove_record");
+  return pinocchio_prove(pk, w, nw, px, npx, nullptr, nullptr, (uint8_t*)d_record);
 }
 int b200_pinocchio_finalize_records(const void* d_records, int world, uint64_t* out_g1, uint64_t pi_b[24]) {
   std::lock_guard<std::mutex> lk(g_mu);
@@ -1117,7 +1135,7 @@ int b200_groth16_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const vo
   ProvingKey* p = find_pk(pk, 1);
   if (!p || !d_w || !d_px || !r || !s || !d_out) return fail(B200_EINVAL, "groth16_prove_device: bad arguments");
   return drain_on_error(groth16_enqueue(p, (const Fr*)d_w, nw, (const Fr*)d_px, npx, r, s, (Fq*)d_out,
-                         stream ? (cudaStream_t)stream : g_stream, p->d_err.as<int>()));
+                         stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
 }
 int b200_comm_unique_id(uint8_t out[128]) {
   std::lock_guard<std::mutex> lk(g_mu);
@@ -1133,37 +1151,26 @@ int b200_comm_init(const uint8_t id[128], int rank, int world) {
   std::lock_guard<std::mutex> lk(g_mu);
   NEED_INIT();
   if (!id || world < 1 || rank < 0 || rank >= world) return fail(B200_EINVAL, "comm_init: bad arguments");
-  if (g_comm.active()) return fail(B200_EINVAL, "comm_init: communicator already initialised (rank %d/%d)", g_comm.rank, g_comm.world);
+  if (comm_active()) return fail(B200_EINVAL, "comm_init: communicator already initialised (rank %d/%d)", g_comm.rank, g_comm.world);
   if (const char* e = g_comm.api.load()) return fail(B200_ECOMM, "comm_init: %s", e);
   ncclUniqueId uid;
   memcpy(&uid, id, 128);
-  ncclResult_t rc = g_comm.api.CommInitRank(&g_comm.comm, world, uid, rank);
-  if (rc != ncclSuccess) {
-    g_comm.comm = nullptr;
-    return fail(B200_ECOMM, "ncclCommInitRank: %s", g_comm.api.GetErrorString(rc));
-  }
+  ncclComm_t comm = nullptr;
+  ncclResult_t rc = g_comm.api.CommInitRank(&comm, world, uid, rank);
+  if (rc != ncclSuccess) return fail(B200_ECOMM, "ncclCommInitRank: %s", g_comm.api.GetErrorString(rc));
   g_comm.rank = rank;
   g_comm.world = world;
   // context 1's communicator (collective: every rank is inside b200_comm_init); older NCCL without ncclCommSplit: both
-  // contexts share `comm` and only ONE host thread may prove on sharded keys
-  g_comm.comm1 = nullptr;
-  if (g_comm.api.CommSplit && world > 1) {
-    rc = g_comm.api.CommSplit(g_comm.comm, 0, rank, &g_comm.comm1, nullptr);
-    if (rc != ncclSuccess) g_comm.comm1 = nullptr;
-  }
+  // contexts share context 0's and only ONE host thread may prove on sharded keys
+  g_ctx[0].comm = g_ctx[1].comm = comm;
+  ncclComm_t split = nullptr;
+  if (g_comm.api.CommSplit && world > 1 && g_comm.api.CommSplit(comm, 0, rank, &split, nullptr) == ncclSuccess)
+    g_ctx[1].comm = split;
   return B200_OK;
 }
 int b200_comm_destroy(void) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!g_comm.active()) return B200_OK;
-  cudaSetDevice(g_device);
-  cudaDeviceSynchronize();
-  if (g_comm.comm1) g_comm.api.CommDestroy(g_comm.comm1);
-  g_comm.comm1 = nullptr;
-  g_comm.api.CommDestroy(g_comm.comm);
-  g_comm.comm = nullptr;
-  g_comm.world = 1;
-  g_comm.rank = 0;
+  comm_destroy_locked();
   return B200_OK;
 }
 int b200_groth16_shard_info(b200_pk_t pk, uint64_t out[12]) {
@@ -1213,7 +1220,7 @@ int b200_pk_free(b200_pk_t pk) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_init) return fail(B200_EINVAL, "not initialised");
   cudaSetDevice(g_device);
-  cudaStreamSynchronize(g_stream);
+  cudaStreamSynchronize(g_ctx[0].main);
   return g_pks.erase(pk) ? B200_OK : fail(B200_EINVAL, "pk_free: bad handle");
 }
 
@@ -1281,7 +1288,7 @@ int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void
   if (nw != p->m || nw != r1->m)
     return fail(B200_EINVAL, "groth16_prove_witness_device: witness length %zu, NVars %zu, R1CS columns %zu", nw, p->m, r1->m);
   return drain_on_error(groth16_witness_enqueue(p, r1, (const Fr*)d_w, r, s, (Fq*)d_out,
-                                                stream ? (cudaStream_t)stream : g_stream, p->d_err.as<int>()));
+                                                stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
 }
 int b200_fq12_mul_batch(const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) { B200_API_BODY(fq12_mul_batch_host(a, b, n, out)) }
 int b200_pairing_batch(const uint64_t* g1_jac, const uint64_t* g2_jac, size_t n, uint64_t* out) { B200_API_BODY(pairing_batch_host(g1_jac, g2_jac, n, out)) }
@@ -1349,28 +1356,18 @@ int b200_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_init) return B200_OK;
   cudaSetDevice(g_device);
-  if (g_comm.active()) {
-    cudaDeviceSynchronize();
-    if (g_comm.comm1) g_comm.api.CommDestroy(g_comm.comm1);
-    g_comm.comm1 = nullptr;
-    g_comm.api.CommDestroy(g_comm.comm);
-    g_comm.comm = nullptr;
-    g_comm.world = 1;
-  }
+  comm_destroy_locked();
   g_bases.clear();
   g_pks.clear();
   g_r1cs.clear();
   g_domains.clear();
-  g_poly.reset();
-  g_poly1.reset();
   if (g_d_err) cudaFree(g_d_err);
-  if (g_stream) cudaStreamDestroy(g_stream);
-  for (auto& sd : g_side) { if (sd) cudaStreamDestroy(sd); sd = nullptr; }
-  for (auto& sd : g_side1) { if (sd) cudaStreamDestroy(sd); sd = nullptr; }
-  if (g_stream1) cudaStreamDestroy(g_stream1);
-  g_stream1 = nullptr;
   g_d_err = nullptr;
-  g_stream = nullptr;
+  for (auto& c : g_ctx) {
+    if (c.main) cudaStreamDestroy(c.main);
+    for (auto sd : c.side) if (sd) cudaStreamDestroy(sd);
+    c = ProveCtx{};   // also frees the polynomial workspace
+  }
   g_init = false;
   return B200_OK;
 }
@@ -1389,7 +1386,7 @@ int b200_bases_free(b200_bases_t h) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!g_init) return fail(B200_EINVAL, "not initialised");
   cudaSetDevice(g_device);
-  cudaStreamSynchronize(g_stream);
+  cudaStreamSynchronize(g_ctx[0].main);
   return g_bases.erase(h) ? B200_OK : fail(B200_EINVAL, "bases_free: bad handle");
 }
 int b200_bases_info(b200_bases_t h, size_t* n, int* group, int* window_bits, int* n_windows) {
@@ -1426,7 +1423,7 @@ int b200_msm_device(b200_bases_t h, const void* d_scalars, size_t n, int mont, v
   NEED_INIT();
   Bases* b = find_bases(h, 0);
   if (!b || !d_out || (!d_scalars && n)) return fail(B200_EINVAL, "msm_device: bad arguments");
-  cudaStream_t st = stream ? (cudaStream_t)stream : g_stream;
+  cudaStream_t st = stream ? (cudaStream_t)stream : g_ctx[0].main;
   int* err = b->d_err.as<int>();
   if (b->group == 1) return msm_enqueue<Fq>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq>*)d_out, err, st);
   return msm_enqueue<Fq2>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq2>*)d_out, err, st);
@@ -1435,12 +1432,12 @@ int b200_msm_device(b200_bases_t h, const void* d_scalars, size_t n, int mont, v
 int b200_g1_sum_partials(const void* d, size_t count, uint64_t out[12], void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   NEED_INIT();
-  return sum_partials<Fq>(d, count, out, stream ? (cudaStream_t)stream : g_stream);
+  return sum_partials<Fq>(d, count, out, stream ? (cudaStream_t)stream : g_ctx[0].main);
 }
 int b200_g2_sum_partials(const void* d, size_t count, uint64_t out[24], void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   NEED_INIT();
-  return sum_partials<Fq2>(d, count, out, stream ? (cudaStream_t)stream : g_stream);
+  return sum_partials<Fq2>(d, count, out, stream ? (cudaStream_t)stream : g_ctx[0].main);
 }
 
 int b200_g1_mul_batch(const uint64_t* p, const uint64_t* s, size_t n, uint64_t* out) {

@@ -43,16 +43,10 @@ struct NcclApi {
   }
 };
 
+// The communicators themselves belong to the prove contexts (capi.cu: ProveCtx).
 struct Comm {
   NcclApi api;
-  ncclComm_t comm = nullptr;
-  // Prove context 1 (B200_CFG_PK_CONTEXT) gathers on its own communicator (ncclCommSplit of `comm`): NCCL matches
-  // collectives by issue order per communicator, and two host threads proving on the two contexts reach their
-  // all-gathers in an order that differs from rank to rank.
-  ncclComm_t comm1 = nullptr;
   int rank = 0, world = 1;
-  bool active() const { return comm != nullptr; }
-  ncclComm_t of(int ctx) const { return ctx && comm1 ? comm1 : comm; }
 };
 
 static_assert(sizeof(ncclUniqueId) == 128, "b200_comm_unique_id hands out 128 bytes");

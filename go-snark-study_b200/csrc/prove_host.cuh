@@ -32,10 +32,8 @@ struct ProvingKey {
   // whole MSMs where it can and index ranges where it must: fewer sorts / reduction tails per rank than
   // slicing every MSM `world` ways.  set k: 0 A, 1 B1, 2 B2, 3 C||PTD.
   int rank = 0, world = 1;
-  int ctx = 0;  // prove context (B200_CFG_PK_CONTEXT at load): side streams + polynomial workspace this key's proofs run on
-  cudaStream_t* side() const { return ctx ? g_side1 : g_side; }
-  cudaStream_t main() const { return ctx ? g_stream1 : g_stream; }
-  PolyCtx& poly() const { return ctx ? *g_poly1 : *g_poly; }
+  int ctx = 0;  // prove context (B200_CFG_PK_CONTEXT at load): streams, polynomial workspace and communicator of its proofs
+  ProveCtx& pctx() const { return g_ctx[ctx]; }
   size_t lo[4] = {0, 0, 0, 0}, hi[4] = {0, 0, 0, 0};  // index range inside set k
   bool tail[4] = {false, false, false, false};        // this rank also holds set k's blinding points
   size_t n_c_full = 0;                                // length of the C part of the C||PTD set (m - npublic - 1)
@@ -44,9 +42,9 @@ struct ProvingKey {
   DevBuf h_full;              // full quotient (sharded mode)
   DevBuf gather;              // all-gathered partial records (world x 1 KB), when a communicator is active
   cudaEvent_t ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  // pinned landing area of the host-pointer entry points: 48 words of proof + the error flags.  Pinned, so the D2H copies
-  // are truly asynchronous and the call can wait for them with the library mutex released (a pageable destination
-  // makes cudaMemcpyAsync block until the proof is done — under the mutex).
+  // pinned landing area of the host-pointer entry points: up to kHostProofWords words of proof + the error flags.  Pinned,
+  // so the D2H copies are truly asynchronous and the call can wait for them with the library mutex released (a pageable
+  // destination makes cudaMemcpyAsync block until the proof is done — under the mutex).
   uint64_t* h_out = nullptr;
   ~ProvingKey() {
     for (auto e : ev) if (e) cudaEventDestroy(e);
@@ -62,7 +60,14 @@ struct ProvingKey {
   // error word of b200_groth16_prove_device on this key: written by the kernels, never read (see b200snark.h), so an
   // out-of-range input of one device-resident proof is reported by no later call and never by a proof on another key
   DevBuf d_err;
+  // error word of the host-pointer proofs on this key: written by the proof's kernels and read back by the same call on
+  // the key's main stream.  Its own word, because those calls wait with the library mutex released: a word shared with
+  // a proof on another key would report one proof's error to the other.
+  DevBuf d_err_sync;
 };
+
+// Largest proof a host-pointer entry point copies out: Pinocchio's 7 G1 + 1 G2 Jacobian points.
+constexpr size_t kHostProofWords = 7 * 12 + 24;
 
 std::map<uint64_t, std::unique_ptr<ProvingKey>> g_pks;
 uint64_t g_next_pk = 1;
@@ -150,11 +155,13 @@ int pk_common_init(ProvingKey& pk, const uint64_t* z, size_t nz, size_t m) {
   CU(pk.res.alloc(8 * 256));
   CU(pk.out_std.alloc(64 * sizeof(Fq)));
   CU(pk.rs.alloc(8 * sizeof(Fr)));
-  CU(pk.d_err.alloc(sizeof(int)));
-  CU(cudaMemset(pk.d_err.p, 0, sizeof(int)));
+  for (DevBuf* e : {&pk.d_err, &pk.d_err_sync}) {
+    CU(e->alloc(sizeof(int)));
+    CU(cudaMemset(e->p, 0, sizeof(int)));
+  }
   for (auto& e : pk.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  CU(cudaHostAlloc(reinterpret_cast<void**>(&pk.h_out), 64 * sizeof(uint64_t), cudaHostAllocDefault));
-  return check_err_flag<Fr>("pk_load(Z)");
+  CU(cudaHostAlloc(reinterpret_cast<void**>(&pk.h_out), (kHostProofWords + 1) * sizeof(uint64_t), cudaHostAllocDefault));
+  return check_err_flag("pk_load(Z)", g_d_err);
 }
 
 int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, const uint64_t* bacdelta, size_t m,
@@ -299,7 +306,7 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
   Fr neg_rs = (fr_r.to_mont() * fr_s.to_mont()).neg().from_mont();  // -(r*s) mod r  (groth16.go:274)
   Fr one = Fr::zero();
   one.l[0] = 1;
-  cudaStream_t s1 = pk->side()[0], s2 = pk->side()[1], s3 = pk->side()[2];
+  cudaStream_t s1 = pk->pctx().side[0], s2 = pk->pctx().side[1], s3 = pk->pctx().side[2];
   if (g_serial) s1 = s2 = s3 = st;  // measurement mode (b200_profile bit 1): no overlap, exclusive kernel timings
   cudaEvent_t e_in = pk->ev[0], e_w = pk->ev[1], e_a = pk->ev[2], e_b1 = pk->ev[3], e_b2 = pk->ev[4],
               e_ch = pk->ev[5], e_prod = pk->ev[6];
@@ -342,7 +349,7 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
       Fr* h_dst = direct ? sCH + n_c : pk->h_full.as<Fr>();
       if (!direct && !pk->h_full.p) CU(pk->h_full.alloc((pk->m + pk->n_h_bases + 4) * sizeof(Fr)));
       if (d_h_std) CU(cudaMemcpyAsync(h_dst, d_h_std, nq * sizeof(Fr), cudaMemcpyDeviceToDevice, s3));
-      else CU(poly_div_device(pk->poly(), pk->Z, d_px, npx, px_mont, h_dst, nullptr, err, s3));
+      else CU(poly_div_device(*pk->pctx().poly, pk->Z, d_px, npx, px_mont, h_dst, nullptr, err, s3));
       size_t have = nq > p_lo ? (nq < p_hi ? nq - p_lo : n_p) : 0;   // valid h coefficients inside [p_lo, p_hi)
       if (!direct && have)
         CU(cudaMemcpyAsync(sCH + n_c, pk->h_full.as<Fr>() + p_lo, have * sizeof(Fr), cudaMemcpyDeviceToDevice, s3));
@@ -397,10 +404,10 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
     k_groth16_combine<<<1, 96, 0, st>>>(res, prod, d_out, d_out + 3, reinterpret_cast<Fq2*>(d_out + 6));
   } else {  // fold the products into this rank's C part; the 1 KB partial record goes to the all-gather
     k_groth16_fold_products<<<1, 32, 0, st>>>(res, prod);
-    if (g_comm.active() && g_comm.world == pk->world) {
+    if (comm_active() && g_comm.world == pk->world) {
       if (g_comm.rank != pk->rank) return fail(B200_EINVAL, "groth16_prove: key shard %d on communicator rank %d", pk->rank, g_comm.rank);
       CU(pk->gather.ensure(kPartialBytes * (size_t)pk->world));
-      ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPartialBytes, ncclUint8, g_comm.of(pk->ctx), st);
+      ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPartialBytes, ncclUint8, pk->pctx().comm, st);
       if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
       k_groth16_finalize<<<1, 96, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, d_out, d_out + 3, reinterpret_cast<Fq2*>(d_out + 6));
       g_launches += 2;
@@ -428,7 +435,7 @@ bool pk_needs_px(const ProvingKey* pk) { return pk->hi[3] > pk->n_c_full; }
 
 // Host-pointer entry points: refuse a sharded key unless the proof can be finished inside the call.
 int check_sharded_host_call(const ProvingKey* pk, const char* what, const char* device_entry) {
-  if (pk->world != 1 && !(g_comm.active() && g_comm.world == pk->world))
+  if (pk->world != 1 && !(comm_active() && g_comm.world == pk->world))
     return fail(B200_EINVAL, "%s: sharded key (rank %d/%d) without a matching communicator: call b200_comm_init, "
                              "or use %s + b200_groth16_finalize_device around your own all-gather",
                 what, pk->rank, pk->world, device_entry);
@@ -459,17 +466,21 @@ int stage_witness(ProvingKey* pk, const uint64_t* w, bool all, cudaStream_t st) 
   return B200_OK;
 }
 
-// Copy the 48-word proof out to the key's pinned landing area and wait for it (with `lk`: the wait runs with the library
-// mutex released), then split it into the caller's PiA, PiB, PiC.
+// Copy the proof out to the key's pinned landing area, read the key's d_err_sync behind it and wait (with `lk`: the wait
+// runs with the library mutex released), then split the proof into the caller's arrays: `outs` lists each array and its
+// word count, in the order of the device layout.
 int finish_host_proof(ProvingKey* pk, const Fq* d_proof, const char* what, cudaStream_t st, std::unique_lock<std::mutex>* lk,
-                      uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c) {
+                      std::initializer_list<std::pair<uint64_t*, size_t>> outs) {
+  size_t words = 0;
+  for (const auto& o : outs) words += o.second;
   uint64_t* host_out = pk->h_out;
-  CU(cudaMemcpyAsync(host_out, d_proof, 48 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  int rc = check_err_flag<Fr>(what, st, lk, reinterpret_cast<int*>(host_out + 48));
+  CU(cudaMemcpyAsync(host_out, d_proof, words * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  int rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(host_out + kHostProofWords));
   if (rc) return rc;
-  memcpy(pi_a, host_out, 12 * 8);
-  memcpy(pi_c, host_out + 12, 12 * 8);
-  memcpy(pi_b, host_out + 24, 24 * 8);
+  for (const auto& o : outs) {
+    memcpy(o.first, host_out, o.second * sizeof(uint64_t));
+    host_out += o.second;
+  }
   return B200_OK;
 }
 
@@ -482,7 +493,7 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
   int rc = check_sharded_host_call(pk, "groth16_prove", "b200_groth16_prove_device");
   if (rc) return rc;
   if (npx < pk->Z.nb) return fail(B200_EINVAL, "groth16_prove: len(px) < len(Z)");
-  cudaStream_t st = pk->main();   // context 1 keys: their own main stream (a second host thread's proof in flight)
+  cudaStream_t st = pk->pctx().main;   // context 1 keys: their own main stream (a second host thread's proof in flight)
   CU(pk->px.ensure(npx * sizeof(Fr)));
   // sharded: stage only what this rank reads, its witness index ranges, and px only if it holds PowersTauDelta points
   if ((rc = stage_witness(pk, w, pk->world == 1, st))) return rc;
@@ -496,12 +507,12 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
   if (need_px) {
     const size_t px_off = pk->Z.nb - 1;
     CU(cudaMemcpyAsync(pk->px.as<Fr>() + px_off, reinterpret_cast<const Fr*>(px) + px_off, (npx - px_off) * sizeof(Fr),
-                       cudaMemcpyHostToDevice, g_serial ? st : pk->side()[2]));
+                       cudaMemcpyHostToDevice, g_serial ? st : pk->pctx().side[2]));
   }
   Fq* o = pk->out_std.as<Fq>();
-  rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st, g_d_err);
+  rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st, pk->d_err_sync.as<int>());
   if (rc) return rc;
-  return finish_host_proof(pk, o, "groth16_prove", st, lk, pi_a, pi_b, pi_c);
+  return finish_host_proof(pk, o, "groth16_prove", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
 }
 
 // Pinocchio result slots (XYZZ, 256 B each): 0 PiA, 1 PiAp, 2 PiBp, 3 PiC, 4 PiCp, 5 PiH, 6 PiKp, 7 PiB (G2).
@@ -579,8 +590,8 @@ int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2,
   return B200_OK;
 }
 
-// d_rec_out != nullptr: leave this rank's 2 KB record of XYZZ results there (device) and return without synchronising —
-// the form the one-GPU tests use to emulate N ranks.
+// On the key's prove context; waits with the library mutex held.  d_rec_out != nullptr: leave this rank's 2 KB record of
+// XYZZ results there (device) — the form the one-GPU tests use to emulate N ranks.
 int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px, size_t npx, uint64_t* out_g1,
                     uint64_t* pi_b, uint8_t* d_rec_out = nullptr) {
   ProvingKey* pk = find_pk(h, 2);
@@ -593,10 +604,12 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
   if (nq > pk->n_h_bases) return fail(B200_EINVAL, "pinocchio_prove: len(hx)=%zu exceeds len(G1T)=%zu", nq, pk->n_h_bases);
   const bool sharded = pk->world > 1;
   const bool gather = sharded && !d_rec_out;
-  if (gather && !(g_comm.active() && g_comm.world == pk->world && g_comm.rank == pk->rank))
+  if (gather && !(comm_active() && g_comm.world == pk->world && g_comm.rank == pk->rank))
     return fail(B200_EINVAL, "pinocchio_prove: sharded key (rank %d/%d) without a matching communicator (b200_comm_init)",
                 pk->rank, pk->world);
-  cudaStream_t st = g_stream, side[3] = {pk->side()[0], pk->side()[1], pk->side()[2]};
+  cudaStream_t st = pk->pctx().main;
+  const cudaStream_t* side = pk->pctx().side;
+  int* err = pk->d_err_sync.as<int>();
   cudaEvent_t e_in = pk->ev[0], e_sorted[2] = {pk->ev[1], pk->ev[2]}, e_done[3] = {pk->ev[3], pk->ev[4], pk->ev[5]};
   Fr* dw = pk->s1.as<Fr>();
   Fr* dh = pk->s3.as<Fr>();
@@ -618,8 +631,8 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
     cudaStream_t s3 = side[2];
     used[2] = true;
     EV_WAIT(s3, e_in);
-    CU(poly_div_device(pk->poly(), pk->Z, pk->px.as<Fr>(), npx, 0, dh, nullptr, g_d_err, s3));
-    if ((rc = msm_enqueue<Fq>(pk->g[7].get(), dh, nq, 0, slot_g1(7), g_d_err, s3))) return rc;
+    CU(poly_div_device(*pk->pctx().poly, pk->Z, pk->px.as<Fr>(), npx, 0, dh, nullptr, err, s3));
+    if ((rc = msm_enqueue<Fq>(pk->g[7].get(), dh, nq, 0, slot_g1(7), err, s3))) return rc;
   }
   // two scalar vectors: w[l+1..m) feeds PiA, PiAp (snark.go:265-268); w feeds PiB, PiBp, PiC, PiCp, PiKp (:270-278).
   // Per vector ONE digit sort (held by the first owned set of the group), the bucket phases fan out over the streams.
@@ -631,7 +644,7 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
     if (holder[gi] < 0) continue;
     const Fr* sc = gi == 0 ? dw + l1 : dw;
     const size_t cnt = gi == 0 ? m - l1 : m;
-    if ((rc = msm_sort(pk->g[holder[gi]]->sort, pk->g[holder[gi]]->sh, sc, cnt, 0, g_d_err, st))) return rc;
+    if ((rc = msm_sort(pk->g[holder[gi]]->sort, pk->g[holder[gi]]->sh, sc, cnt, 0, err, st))) return rc;
     EV_REC(e_sorted[gi], st);
   }
   for (int gi = 1; gi >= 0; gi--) {   // the larger group first
@@ -661,25 +674,19 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
   if (d_rec_out) {
     CU(cudaMemcpyAsync(d_rec_out, res, kPinRecordBytes, cudaMemcpyDeviceToDevice, st));
     CU(cudaGetLastError());
-    return B200_OK;
+    return check_err_flag("pinocchio_prove_record", err, st);
   }
   Fq* o = pk->out_std.as<Fq>();
   if (gather) {
     CU(pk->gather.ensure(kPinRecordBytes * (size_t)pk->world));
-    ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPinRecordBytes, ncclUint8, g_comm.of(pk->ctx), st);
+    ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPinRecordBytes, ncclUint8, pk->pctx().comm, st);
     if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
     k_pinocchio_gather_finalize<<<1, 64, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, o, reinterpret_cast<Fq2*>(o + 21));
   } else {
     k_pinocchio_finalize<<<1, 64, 0, st>>>(res, o, reinterpret_cast<Fq2*>(o + 21));
   }
   CU(cudaGetLastError());
-  uint64_t host_out[(21 + 6) * 4];
-  CU(cudaMemcpyAsync(host_out, o, sizeof host_out, cudaMemcpyDeviceToHost, st));
-  rc = check_err_flag<Fr>("pinocchio_prove");
-  if (rc) return rc;
-  memcpy(out_g1, host_out, 84 * 8);
-  memcpy(pi_b, host_out + 84, 24 * 8);
-  return B200_OK;
+  return finish_host_proof(pk, o, "pinocchio_prove", st, nullptr, {{out_g1, 84}, {pi_b, 24}});
 }
 
 // one-GPU emulation of the collective: sum `world` gathered records (device) -> the proof (host)
@@ -687,11 +694,11 @@ int pinocchio_finalize_records(const uint8_t* d_recs, int world, uint64_t* out_g
   if (!d_recs || world < 1 || !out_g1 || !pi_b) return fail(B200_EINVAL, "pinocchio_finalize: bad arguments");
   DevBuf o;
   CU(o.alloc(64 * sizeof(Fq)));
-  k_pinocchio_gather_finalize<<<1, 64, 0, g_stream>>>(d_recs, world, o.as<Fq>(), reinterpret_cast<Fq2*>(o.as<Fq>() + 21));
+  k_pinocchio_gather_finalize<<<1, 64, 0, g_ctx[0].main>>>(d_recs, world, o.as<Fq>(), reinterpret_cast<Fq2*>(o.as<Fq>() + 21));
   CU(cudaGetLastError());
   uint64_t host_out[(21 + 6) * 4];
-  CU(cudaMemcpyAsync(host_out, o.p, sizeof host_out, cudaMemcpyDeviceToHost, g_stream));
-  int rc = check_err_flag<Fr>("pinocchio_finalize");
+  CU(cudaMemcpyAsync(host_out, o.p, sizeof host_out, cudaMemcpyDeviceToHost, g_ctx[0].main));
+  int rc = check_err_flag("pinocchio_finalize", g_d_err);
   if (rc) return rc;
   memcpy(out_g1, host_out, 84 * 8);
   memcpy(pi_b, host_out + 84, 24 * 8);

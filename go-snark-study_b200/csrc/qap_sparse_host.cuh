@@ -10,7 +10,7 @@ int get_domain(size_t N, QapDomain** out) {
   auto it = g_domains.find(N);
   if (it == g_domains.end()) {
     auto d = std::make_unique<QapDomain>();
-    CU(qap_domain_build(*g_poly, *d, N, g_stream));
+    CU(qap_domain_build(*g_ctx[0].poly, *d, N, g_ctx[0].main));
     it = g_domains.emplace(N, std::move(d)).first;
   }
   *out = it->second.get();
@@ -146,7 +146,7 @@ int qap_px_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, Fr* d_
 
 // d_w: m witness values (device, standard form; an entry >= r is read as 0 and sets bit 1 of *err) -> the n - 1
 // coefficients of h = (ax*bx - cx) / Z in ws.h_std (standard form), without forming px (qap_sparse.cuh: QapHDomain).
-// Requires n >= 2.  The domains are shared by every context: built on g_stream and waited for on the first call.
+// Requires n >= 2.  The domains are shared by every context: built on g_ctx[0].main and waited for on the first call.
 int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
   const size_t n = r->n, m = r->m, N = pow2_at_least(n);
   if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
@@ -155,7 +155,7 @@ int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* er
   if (rc) return rc;
   if (!r->hd) {
     auto hd = std::make_unique<QapHDomain>();
-    CU(qap_hdomain_build(*g_poly, *hd, n, g_stream));   // synchronises g_stream
+    CU(qap_hdomain_build(*g_ctx[0].poly, *hd, n, g_ctx[0].main));   // synchronises g_ctx[0].main
     r->hd = std::move(hd);
   }
   Fr* w = ws.w_mont.as<Fr>();
@@ -179,7 +179,7 @@ int qap_px_host(b200_r1cs_t h, const uint64_t* w, size_t nw, uint64_t* ax, uint6
   if (!r) return fail(B200_EINVAL, "qap_px: bad R1CS handle");
   if (!w || nw != r->m) return fail(B200_EINVAL, "qap_px: witness length %zu != m %zu", nw, r->m);
   const size_t n = r->n;
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   R1csWork* ws;
   int rc = r1cs_work(r, 0, &ws);
   if (rc) return rc;
@@ -188,13 +188,13 @@ int qap_px_host(b200_r1cs_t h, const uint64_t* w, size_t nw, uint64_t* ax, uint6
   CU(dabc.alloc(3 * n * sizeof(Fr)));
   CU(dpx.alloc((2 * n - 1) * sizeof(Fr)));
   CU(cudaMemcpyAsync(dw.p, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
-  rc = qap_px_enqueue(r, *ws, *g_poly, dw.as<Fr>(), dabc.as<Fr>(), dpx.as<Fr>(), g_d_err, st);
+  rc = qap_px_enqueue(r, *ws, *g_ctx[0].poly, dw.as<Fr>(), dabc.as<Fr>(), dpx.as<Fr>(), g_d_err, st);
   if (rc) return rc;
   uint64_t* outs[3] = {ax, bx, cx};
   for (int k = 0; k < 3; k++)
     if (outs[k]) CU(cudaMemcpyAsync(outs[k], dabc.as<Fr>() + k * n, n * sizeof(Fr), cudaMemcpyDeviceToHost, st));
   if (px) CU(cudaMemcpyAsync(px, dpx.p, (2 * n - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, st));
-  return check_err_flag<Fr>("qap_px");
+  return check_err_flag("qap_px", g_d_err);
 }
 
 // LagrangeInterpolation over x = 1..n (r1csqap.go:150-158) at any n: values -> n coefficients
@@ -204,7 +204,7 @@ int interpolate_host(const uint64_t* values, size_t n, uint64_t* coeffs) {
   QapDomain* dom;
   int rc = get_domain(N, &dom);
   if (rc) return rc;
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   DevBuf dv, dm, dc, ds;
   QapWork wk;
   CU(dv.alloc(n * sizeof(Fr)));
@@ -213,10 +213,10 @@ int interpolate_host(const uint64_t* values, size_t n, uint64_t* coeffs) {
   CU(ds.alloc(n * sizeof(Fr)));
   CU(cudaMemcpyAsync(dv.p, values, n * sizeof(Fr), cudaMemcpyHostToDevice, st));
   k_poly_load<<<nblk(n, 256), 256, 0, st>>>(dv.as<Fr>(), (uint32_t)n, (uint32_t)n, 0, 0, dm.as<Fr>(), (uint32_t)n, g_d_err);
-  CU(interpolate_ap(*g_poly, *dom, wk, dm.as<Fr>(), n, n, 1, dc.as<Fr>(), st));
+  CU(interpolate_ap(*g_ctx[0].poly, *dom, wk, dm.as<Fr>(), n, n, 1, dc.as<Fr>(), st));
   k_poly_store<<<nblk(n, 256), 256, 0, st>>>(dc.as<Fr>(), (uint32_t)n, 0, 1, ds.as<Fr>());
   CU(cudaMemcpyAsync(coeffs, ds.p, n * sizeof(Fr), cudaMemcpyDeviceToHost, st));
-  return check_err_flag<Fr>("interpolate");
+  return check_err_flag("interpolate", g_d_err);
 }
 
 // prod_{i=1..n}(x - i) at any n: the Newton basis element of index n, converted by the same divide and conquer
@@ -240,7 +240,7 @@ int zero_poly_device(size_t n, DevBuf& d_out, cudaStream_t st) {
   CU(cudaMemsetAsync(P.p, 0, N * sizeof(Fr), st));
   Fr one = Fr::one();
   CU(cudaMemcpyAsync(P.as<Fr>() + n, &one, sizeof(Fr), cudaMemcpyHostToDevice, st));
-  CU(newton_to_monomial(*g_poly, *dom, P.as<Fr>(), X.as<Fr>(), 1, st));
+  CU(newton_to_monomial(*g_ctx[0].poly, *dom, P.as<Fr>(), X.as<Fr>(), 1, st));
   CU(cudaMemcpyAsync(o, P.p, (n + 1) * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
   CU(cudaStreamSynchronize(st));
   return B200_OK;
@@ -288,7 +288,7 @@ int qap_eval_at_host(b200_r1cs_t h, const uint64_t* tau, size_t nz, uint64_t* at
   Fr t_std = fr_load_std(tau);
   if (t_std.geq_modulus()) return fail(B200_ERANGE, "qap_eval_at: tau >= r");
   const size_t m = r->m;
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   DevBuf o, os;
   CU(o.alloc(3 * m * sizeof(Fr)));
   CU(os.alloc(3 * m * sizeof(Fr)));
@@ -302,7 +302,7 @@ int qap_eval_at_host(b200_r1cs_t h, const uint64_t* tau, size_t nz, uint64_t* at
     Fr z = znz.from_mont();
     memcpy(zt_out, &z, sizeof(Fr));
   }
-  rc = check_err_flag<Fr>("qap_eval_at");
+  rc = check_err_flag("qap_eval_at", g_d_err);
   if (rc == B200_OK) return rc;
   return rc;
 }

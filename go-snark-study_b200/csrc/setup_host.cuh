@@ -99,7 +99,7 @@ int groth16_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uin
   if ((rc = setup_check_tau(r, toxic, what))) return rc;
   const size_t m = r->m, l1 = npublic + 1;
   if ((rc = zero_poly_host(m - 2, z))) return rc;                  // Z = prod_{i=1..m-2}(x - i), groth16.go:122-132
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   const size_t n1 = 4 * m - 1 + l1 + 3, n2 = m + 3;
   DevBuf ev, s1, s2, p1, p2;
   CU(ev.alloc(3 * m * sizeof(Fr)));
@@ -132,7 +132,7 @@ int groth16_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uin
     if ((rc = copy_points(vk2[k], g2, m + k, 1, st))) return rc;
   }
   if ((rc = copy_points(b2, g2, 0, m, st))) return rc;
-  return check_err_flag<Fr>(what);
+  return check_err_flag(what, g_d_err);
 }
 
 int pinocchio_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uint64_t* a, uint64_t* ap, uint64_t* b2,
@@ -148,7 +148,7 @@ int pinocchio_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, u
   if ((rc = setup_check_tau(r, toxic, what))) return rc;
   const size_t m = r->m;
   if ((rc = zero_poly_host(m - 2, z))) return rc;                  // snark.go:210-221
-  cudaStream_t st = g_stream;
+  cudaStream_t st = g_ctx[0].main;
   const size_t n1 = 7 * m - 1 + 2, n2 = m + 5;
   DevBuf ev, s1, s2, p1, p2;
   CU(ev.alloc(3 * m * sizeof(Fr)));
@@ -177,5 +177,5 @@ int pinocchio_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, u
   if ((rc = copy_points(vk_g1, g1, n1 - 2, 2, st))) return rc;
   if ((rc = copy_points(b2, g2, 0, m, st))) return rc;
   if ((rc = copy_points(vk_g2, g2, m, 5, st))) return rc;
-  return check_err_flag<Fr>(what);
+  return check_err_flag(what, g_d_err);
 }

@@ -58,11 +58,13 @@ int b200_version(void);
  * copies (cp.async.bulk + per-warp mbarrier) in the contiguous rounds, cp.async gathers in round 1.  0 (default) the
  * register-load kernel (the kernel is bound by the multiply pipe, not by the fetch); 1 staged in every round, 2 staged in rounds >= 2 only.  Same results.          */
 #define B200_CFG_TMA_STAGING 2
-/* B200_CFG_PK_CONTEXT: prove context (0 or 1) of proving keys loaded AFTERWARDS.  The two contexts own separate side
- * streams and polynomial workspaces, so a device-resident proof on a context-1 key (b200_groth16_prove_device on the
- * caller's second stream) may be in flight beside one on a context-0 key: a prover that keeps two proofs in flight hides
- * the latency-bound sort / bucket-tail / blinding-product chains of one behind the accumulation of the other (bench.py
- * `proofs_in_flight`; the keys are independent objects, each with its own tables and scratch).                       */
+/* B200_CFG_PK_CONTEXT: prove context (0 or 1) of proving keys loaded AFTERWARDS.  The two contexts own separate main and
+ * side streams, polynomial workspaces and NCCL communicators, so a device-resident proof on a context-1 key
+ * (b200_groth16_prove_device on the caller's second stream) may be in flight beside one on a context-0 key: a prover that
+ * keeps two proofs in flight hides the latency-bound sort / bucket-tail / blinding-product chains of one behind the
+ * accumulation of the other (bench.py `proofs_in_flight`; the keys are independent objects, each with its own tables,
+ * scratch and error words).  Host-pointer proofs run on their key's context and report only their own input errors, also
+ * when two host threads prove at once.  Other calls run on context 0.                                                 */
 #define B200_CFG_PK_CONTEXT 4
 /* B200_CFG_PAIRING_KERNEL: b200_pairing_batch with one THREAD per pairing (1: the step-by-step restatement of
  * bn128.go:179-421, a long chain of dependent multiplications per pairing) or one WARP per pairing (2: F_q^12 in shared
