@@ -1,4 +1,5 @@
 """ctypes binding of libb200snark.so (the C ABI of include/b200snark.h)."""
+import contextlib
 import ctypes
 import os
 
@@ -11,6 +12,7 @@ CFG_TMA_STAGING = 2
 CFG_SHARD_W_AB, CFG_SHARD_W_G2, CFG_SHARD_AFFINE_MIN_G1, CFG_SHARD_AFFINE_MIN_G2 = 10, 11, 12, 13
 CFG_PAIRING_KERNEL = 5  # b200_pairing_batch: 0 default (one warp per pairing), 1 one thread per pairing, 2 one warp
 CFG_PK_CONTEXT = 4    # prove context (0 / 1) of proving keys loaded afterwards: two proofs in flight
+CFG_TABLE_WINDOWS = 14  # stored window rows t of base sets / keys loaded afterwards (0: all; fewer: less memory, slower)
 
 B200_OK = 0
 ERRORS = {-1: "ENODEVICE", -2: "ECUDA", -3: "EINVAL", -4: "ERANGE", -5: "EDIVZERO", -6: "ENOMEM", -7: "ECOMM"}
@@ -40,6 +42,9 @@ _SIGNATURES = {
     "b200_bases_free": [_h],
     "b200_bases_info": [_h, ctypes.POINTER(_sz), ctypes.POINTER(_int), ctypes.POINTER(_int), ctypes.POINTER(_int)],
     "b200_bases_acc_mode": [_h, ctypes.POINTER(_int)],
+    "b200_bases_table_windows": [_h, ctypes.POINTER(_int)],
+    "b200_bases_device_bytes": [_h, ctypes.POINTER(_sz)],
+    "b200_pk_device_bytes": [_h, ctypes.POINTER(_sz)],
     "b200_g1_msm": [_h, _vp, _sz, _vp],
     "b200_g2_msm": [_h, _vp, _sz, _vp],
     "b200_msm_device": [_h, _vp, _sz, _int, _vp, _vp],
@@ -130,6 +135,23 @@ def init(device=None):
 
 
 # ---- big-int <-> limb marshalling (what the cgo shim does with big.Int.Bits()) ----
+@contextlib.contextmanager
+def table_windows(t):
+    """Loads inside the block store t window rows (B200_CFG_TABLE_WINDOWS; 0 = all); the option is 0 again after it."""
+    check(lib().b200_config(CFG_TABLE_WINDOWS, int(t)))
+    try:
+        yield
+    finally:
+        lib().b200_config(CFG_TABLE_WINDOWS, 0)
+
+
+def pk_device_bytes(handle):
+    """Device memory a proving key holds (b200_pk_device_bytes)."""
+    v = _sz(0)
+    check(lib().b200_pk_device_bytes(handle, ctypes.byref(v)))
+    return v.value
+
+
 def ints_to_limbs(vals, words_per_val=4):
     """list[int] -> contiguous uint64 array (len, words_per_val), little endian."""
     nbytes = 8 * words_per_val

@@ -51,8 +51,9 @@ class BaseSet:
     """A CRS array (e.g. Pk.G1.At) uploaded once: normalised to affine Montgomery
     form and window-precomputed on the device (b200_g*_bases_load)."""
 
-    def __init__(self, group, points=None, limbs=None, window_bits=0, acc_mode=0):
-        """acc_mode: 0 auto, 1 batched-affine, 2 XYZZ bucket accumulation (b200_config; same result)."""
+    def __init__(self, group, points=None, limbs=None, window_bits=0, acc_mode=0, table_windows=0):
+        """acc_mode: 0 auto, 1 batched-affine, 2 XYZZ bucket accumulation (b200_config; same result).
+        table_windows: stored window rows t (B200_CFG_TABLE_WINDOWS; 0 = all, same result, t < all: less memory)."""
         assert group in (1, 2)
         self.group = group
         if limbs is None:
@@ -65,10 +66,21 @@ class BaseSet:
         fn = lib().b200_g1_bases_load if group == 1 else lib().b200_g2_bases_load
         check(lib().b200_config(_lib.CFG_ACC_MODE, acc_mode))
         try:
-            check(fn(ptr(limbs), self.n, window_bits, h))
+            with _lib.table_windows(table_windows):
+                check(fn(ptr(limbs), self.n, window_bits, h))
         finally:
             check(lib().b200_config(_lib.CFG_ACC_MODE, _lib.ACC_AUTO))
         self.handle = h.value
+
+    def table_windows(self):
+        t = _lib._int(0)
+        check(lib().b200_bases_table_windows(self.handle, t))
+        return t.value
+
+    def device_bytes(self):
+        v = _lib._sz(0)
+        check(lib().b200_bases_device_bytes(self.handle, v))
+        return v.value
 
     def acc_mode(self):
         m = _lib._int(0)

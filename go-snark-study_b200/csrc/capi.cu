@@ -78,6 +78,7 @@ int g_acc_mode = 0;
 // partition tuning (b200_config keys 10..13; defaults = the measured best for one proof at a time)
 int g_w_ab = 100, g_w_g2 = 280, g_aff_min_g1 = 700000, g_aff_min_g2 = 400000;
 int g_tma_staging = 0;   // B200_CFG_TMA_STAGING: 1 staged backward pass in every round, 2 only in the contiguous rounds (>= 2)
+int g_table_windows = 0;   // B200_CFG_TABLE_WINDOWS: stored window rows t of base sets created afterwards (0: all)
 
 // ---- instrumentation (bench.py): kernel-launch counter and optional CUDA-event
 // timing of the dominant kernel (k_accumulate), per group.
@@ -164,6 +165,12 @@ int pick_window_bits(size_t n) {
   return best;
 }
 
+// Records of launch_bucket_tail's scratch: H rows, K columns and c planes per window group.
+size_t bucket_tail_records(const MsmShape& sh) {
+  const uint32_t bits = sh.c - 1, kl = (bits + 1) / 2, kh = bits - kl;
+  return (size_t)sh.groups * ((1u << kh) + (1u << kl) + bits + 1);
+}
+
 // Output of the digit-recode / counting-sort front end for one scalar vector.  It depends only on the
 // scalars and the window shape, so base sets that consume the SAME scalars (A, B1, B2 of a Groth16
 // proof) share one SortScratch read-only.
@@ -193,18 +200,32 @@ struct Bases {
   DevBuf d_err;
 };
 
+// Device memory held by the buffers (b200_bases_device_bytes / b200_pk_device_bytes).
+size_t dev_bytes(std::initializer_list<const DevBuf*> bufs) {
+  size_t s = 0;
+  for (const DevBuf* d : bufs) s += d->p ? d->bytes : 0;
+  return s;
+}
+size_t bases_device_bytes(const Bases& b) {
+  const SortScratch& ss = b.sort;
+  return dev_bytes({&b.table, &b.scalars, &b.slice_out, &b.buckets, &b.partials, &b.result, &b.out_std, &b.nodeA, &b.nodeB,
+                    &b.aff_pre, &b.aff_others, &b.aff_btot, &b.aff_ids, &b.d_err, &ss.counts, &ss.offsets, &ss.cursor,
+                    &ss.entries, &ss.slice_off, &ss.slice_start, &ss.slice_end});
+}
+
 int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
   ss.sh = sh;
   ss.slice_S = slice_S;
   size_t entries = (size_t)sh.nwin * sh.n;
-  CU(ss.counts.alloc((sh.nbuckets + 2) * sizeof(uint32_t)));
-  CU(ss.offsets.alloc((sh.nbuckets + 3) * sizeof(uint32_t)));
-  CU(ss.cursor.alloc((sh.nbuckets + 2) * sizeof(uint32_t)));
+  const uint32_t B = total_buckets(sh);
+  CU(ss.counts.alloc((B + 2) * sizeof(uint32_t)));
+  CU(ss.offsets.alloc((B + 3) * sizeof(uint32_t)));
+  CU(ss.cursor.alloc((B + 2) * sizeof(uint32_t)));
   CU(ss.entries.alloc(entries * sizeof(uint32_t)));
   // slices: every bucket owns >= 1; a bucket above cap = 2*mean entries is cut => at most B + B/2 + 1
-  ss.max_slices = sh.nbuckets + sh.nbuckets / 2 + 2;
-  if (slice_S) ss.max_slices = sh.nbuckets + (uint32_t)((entries + slice_S - 1) / slice_S) + 2;
-  CU(ss.slice_off.alloc((sh.nbuckets + 3) * sizeof(uint32_t)));
+  ss.max_slices = B + B / 2 + 2;
+  if (slice_S) ss.max_slices = B + (uint32_t)((entries + slice_S - 1) / slice_S) + 2;
+  CU(ss.slice_off.alloc((B + 3) * sizeof(uint32_t)));
   CU(ss.slice_start.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
   CU(ss.slice_end.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
   return B200_OK;
@@ -257,17 +278,21 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   sh.nwin = (255 + c - 1) / c;
   sh.nbuckets = 1u << (c - 1);
   sh.table_stride = (uint32_t)n;
+  // B200_CFG_TABLE_WINDOWS: keep t of the nwin window rows; window w reads row w mod t and feeds bucket group w / t
+  sh.rows = g_table_windows > 0 && (uint32_t)g_table_windows < sh.nwin ? (uint32_t)g_table_windows : sh.nwin;
+  sh.groups = (sh.nwin + sh.rows - 1) / sh.rows;
+  const bool reduced = sh.rows < sh.nwin;
   if ((uint64_t)sh.nwin * n >= (1ull << 31)) return fail(B200_EINVAL, "nwin*n exceeds 2^31 entries");
-  size_t entries = (size_t)sh.nwin * n;
-  CU(b->table.alloc(entries * sizeof(Affine<F>)));
+  CU(b->table.alloc((size_t)sh.rows * n * sizeof(Affine<F>)));
   CU(b->scalars.alloc(n * sizeof(Fr)));
-  CU(b->buckets.alloc((size_t)sh.nbuckets * sizeof(XYZZ<F>)));
+  CU(b->buckets.alloc((size_t)total_buckets(sh) * sizeof(XYZZ<F>)));
   {
     // accumulation mode: batched affine (6.5 multiplies per add, 3 launches per round) where the buckets are populated
-    // enough to amortise the rounds, else XYZZ mixed adds (10 multiplies, one launch); b200_config forces either
-    const bool xyzz_mode = g_acc_mode == 2 || (g_acc_mode == 0 && !prefer_affine);
+    // enough to amortise the rounds, else XYZZ mixed adds (10 multiplies, one launch); b200_config forces either.  Auto
+    // mode keeps a reduced table on XYZZ: the batched-affine node scratch alone is about the size of a full table.
+    const bool xyzz_mode = g_acc_mode == 2 || (g_acc_mode == 0 && (!prefer_affine || reduced));
     uint32_t S = 0;
-    uint64_t mean = ((uint64_t)sh.nwin * n) / sh.nbuckets;
+    uint64_t mean = ((uint64_t)sh.nwin * n) / total_buckets(sh);
     const uint64_t min_mean = g_acc_mode == 1 ? 16 : 96;
     if (!xyzz_mode && mean >= min_mean) {
       S = 8;
@@ -289,9 +314,10 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   }
   CU(b->slice_out.alloc((size_t)(b->affine_S ? 1 : b->sort.max_slices) * sizeof(XYZZ<F>)));
   // short latency chain: 4-bucket segments (8 adds + one small scalar mul per thread), then a two-level tree sum
+  // (c < 7); nseg segments per window group.  c >= 7: the scratch of launch_bucket_tail.
   b->seg = sh.nbuckets >= 256 ? 4 : 1;
   b->nseg = (sh.nbuckets + b->seg - 1) / b->seg;
-  CU(b->partials.alloc(((size_t)b->nseg + 1024) * sizeof(XYZZ<F>)));
+  CU(b->partials.alloc(std::max((size_t)sh.groups * b->nseg + 1024, bucket_tail_records(sh)) * sizeof(XYZZ<F>)));
   CU(b->result.alloc(sizeof(XYZZ<F>)));
   CU(b->out_std.alloc(3 * sizeof(F)));
   CU(b->d_err.alloc(sizeof(int)));
@@ -302,7 +328,7 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   CU(staging.alloc(n * 3 * sizeof(F)));
   CU(state.alloc(n * sizeof(XYZZ<F>)));
   CU(cudaMemcpyAsync(staging.p, pts, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
-  window_table_enqueue<F>(staging.as<F>(), n, sh.nwin, c, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_d_err, g_ctx[0].main);
+  window_table_enqueue<F>(staging.as<F>(), n, sh.rows, c, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_d_err, g_ctx[0].main);
   CU(cudaGetLastError());
   int rc = check_err_flag("bases_load", g_d_err);
   if (rc) return rc;
@@ -370,30 +396,41 @@ void launch_tree_sum(XYZZ<F>* partials, uint32_t n, XYZZ<F>* d_out, cudaStream_t
   g_launches += 2;
 }
 
-// sum_b b * S_b over the bucket array -> one XYZZ record (msm.cuh: rows / columns, bit planes, Horner).  `scratch` holds
-// H + K + (c - 1) + 1 records.  Tiny bucket sets keep the segment kernel.
+// sum_g 2^(c*t*g) sum_b b * S_(g,b) over the bucket array -> one XYZZ record (msm.cuh: rows / columns and bit planes of
+// every window group, one Horner chain over all groups).  `scratch` holds bucket_tail_records(sh) records.  Tiny bucket
+// sets keep the segment kernel.
 template <class F>
-void launch_bucket_tail(const XYZZ<F>* buckets, uint32_t c, XYZZ<F>* scratch, XYZZ<F>* d_out, cudaStream_t st) {
-  const uint32_t bits = c - 1, kl = (bits + 1) / 2, kh = bits - kl, K = 1u << kl, H = 1u << kh;
+void launch_bucket_tail(const XYZZ<F>* buckets, const MsmShape& sh, XYZZ<F>* scratch, XYZZ<F>* d_out, cudaStream_t st) {
+  const uint32_t bits = sh.c - 1, kl = (bits + 1) / 2, kh = bits - kl, K = 1u << kl, H = 1u << kh, G = sh.groups;
   XYZZ<F>* R = scratch;
-  XYZZ<F>* C = scratch + H;
-  XYZZ<F>* planes = C + K;
-  k_tail_rowcol<F><<<nblocks((size_t)(H + K) * 32, 128), 128, 0, st>>>(buckets, kl, H, R, C);
-  k_tail_planes<F><<<nblocks((size_t)(bits + 1) * 32, 128), 128, 0, st>>>(R, C, kl, kh, planes);
-  k_tail_horner<F><<<1, 32, 0, st>>>(planes, bits, d_out);
+  XYZZ<F>* C = scratch + (size_t)G * H;
+  XYZZ<F>* planes = C + (size_t)G * K;
+  k_tail_rowcol<F><<<dim3(nblocks((size_t)(H + K) * 32, 128), G), 128, 0, st>>>(buckets, kl, H, R, C);
+  k_tail_planes<F><<<dim3(nblocks((size_t)(bits + 1) * 32, 128), G), 128, 0, st>>>(R, C, kl, kh, planes);
+  k_tail_horner<F><<<1, 32, 0, st>>>(planes, bits, d_out, G, sh.c * sh.rows);
   g_launches += 3;
+}
+
+// The c < 7 tail: segment sums of every window group, each scaled by 2^(c*t*g), then one tree sum over all of them.
+template <class F>
+void launch_segment_tail(const Bases* b, const XYZZ<F>* buckets, XYZZ<F>* partials, XYZZ<F>* d_out, cudaStream_t st) {
+  const MsmShape& sh = b->sh;
+  k_bucket_reduce<F><<<dim3(nblocks(b->nseg, 128), sh.groups), 128, 0, st>>>(buckets, sh.nbuckets, b->seg, partials, b->nseg,
+                                                                              sh.c * sh.rows);
+  launch_tree_sum<F>(partials, sh.groups * b->nseg, d_out, st);
 }
 
 // Front end: signed-digit recode + counting sort of n scalars into bucket order (3 launches).  A standard-form scalar
 // >= r is read as 0 and sets bit 1 of *err.
 int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, int* err, cudaStream_t st) {
-  if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride)
+  if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride || shape.rows != ss.sh.rows)
     return fail(B200_EINVAL, "msm_sort: shape mismatch");
   MsmShape sh = shape;
   sh.n = (uint32_t)n;
-  uint32_t m = sh.nbuckets + 1;  // counts[0] unused (digit 0), buckets 1..B
+  const uint32_t B = total_buckets(sh);
+  uint32_t m = B + 1;  // counts[0] unused (digit 0), buckets 1..B of all window groups
   // slice cap: twice the mean bucket population (uniform scalars never split), at least 4 per lane
-  uint64_t mean = ((uint64_t)sh.nwin * n + sh.nbuckets - 1) / sh.nbuckets;
+  uint64_t mean = ((uint64_t)sh.nwin * n + B - 1) / B;
   uint32_t cap = (uint32_t)(2 * mean < 4 * kLPB ? 4 * kLPB : 2 * mean);
   int fixed = 0;
   if (ss.slice_S) {
@@ -417,10 +454,11 @@ int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t
 template <class F>
 int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out, cudaStream_t st) {
   const MsmShape& sh = b->sh;
-  if (ss.sh.c != sh.c || ss.sh.table_stride != sh.table_stride || ss.max_slices != b->sort.max_slices ||
+  if (ss.sh.c != sh.c || ss.sh.table_stride != sh.table_stride || ss.sh.rows != sh.rows || ss.max_slices != b->sort.max_slices ||
       ss.slice_S != b->sort.slice_S)
     return fail(B200_EINVAL, "msm_buckets: sort scratch does not match the base set");
-  uint32_t m = sh.nbuckets + 1;
+  const uint32_t B = total_buckets(sh);
+  uint32_t m = B + 1;
   XYZZ<F>* buckets = b->buckets.as<XYZZ<F>>();
   XYZZ<F>* partials = b->partials.as<XYZZ<F>>();
   SliceTables stb = ss.tables();
@@ -438,7 +476,7 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
     while ((1u << R) < S) R++;
     // host-side bound on the live slice count for this call (the exact count lives on the device)
     uint64_t total = (uint64_t)sh.nwin * n_terms;
-    uint64_t nsl_bound = (uint64_t)sh.nbuckets + (total + S - 1) / S + 2;
+    uint64_t nsl_bound = (uint64_t)B + (total + S - 1) / S + 2;
     if (nsl_bound > ss.max_slices) nsl_bound = ss.max_slices;
     AffineRound<F> ar{};
     ar.table = b->table.as<Affine<F>>();
@@ -482,19 +520,18 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
       cudaEventRecord(pr.e1, st);
       g_prof_recs.push_back(pr);
     }
-    k_merge_slices_affine<F><<<nblocks(sh.nbuckets, 128), 128, 0, st>>>(prev, stb, sh.nbuckets, buckets);
+    k_merge_slices_affine<F><<<nblocks(B, 128), 128, 0, st>>>(prev, stb, B, buckets);
     if (sh.c >= 7) {
-      launch_bucket_tail<F>(buckets, sh.c, partials, d_out, st);
+      launch_bucket_tail<F>(buckets, sh, partials, d_out, st);
       g_launches += 1;
     } else {
-      k_bucket_reduce<F><<<nblocks(b->nseg, 128), 128, 0, st>>>(buckets, sh.nbuckets, b->seg, partials, b->nseg);
-      launch_tree_sum<F>(partials, b->nseg, d_out, st);
+      launch_segment_tail<F>(b, buckets, partials, d_out, st);
       g_launches += 2;
     }
     CU(cudaGetLastError());
     return B200_OK;
   }
-  uint64_t mean = ((uint64_t)sh.nwin * n_terms + sh.nbuckets - 1) / sh.nbuckets;
+  uint64_t mean = ((uint64_t)sh.nwin * n_terms + B - 1) / B;
   int lpb = mean >= 384 ? 8 : (mean >= 96 ? 4 : 2);
   launch_accumulate<F>(lpb, b->table.as<Affine<F>>(), ss.entries.as<uint32_t>(), stb, m,
                        b->slice_out.as<XYZZ<F>>(), ss.max_slices, st);
@@ -502,13 +539,12 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
     cudaEventRecord(pr.e1, st);
     g_prof_recs.push_back(pr);
   }
-  k_merge_slices<F><<<nblocks(sh.nbuckets, 128), 128, 0, st>>>(b->slice_out.as<XYZZ<F>>(), stb, sh.nbuckets, buckets);
+  k_merge_slices<F><<<nblocks(B, 128), 128, 0, st>>>(b->slice_out.as<XYZZ<F>>(), stb, B, buckets);
   if (sh.c >= 7) {
-    launch_bucket_tail<F>(buckets, sh.c, partials, d_out, st);
+    launch_bucket_tail<F>(buckets, sh, partials, d_out, st);
     g_launches += 1;
   } else {
-    k_bucket_reduce<F><<<nblocks(b->nseg, 128), 128, 0, st>>>(buckets, sh.nbuckets, b->seg, partials, b->nseg);
-    launch_tree_sum<F>(partials, b->nseg, d_out, st);
+    launch_segment_tail<F>(b, buckets, partials, d_out, st);
     g_launches += 3;
   }
   CU(cudaGetLastError());
@@ -1223,6 +1259,13 @@ int b200_pk_free(b200_pk_t pk) {
   cudaStreamSynchronize(g_ctx[0].main);
   return g_pks.erase(pk) ? B200_OK : fail(B200_EINVAL, "pk_free: bad handle");
 }
+int b200_pk_device_bytes(b200_pk_t h, size_t* bytes) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  auto it = g_pks.find(h);
+  if (it == g_pks.end() || !bytes) return fail(B200_EINVAL, "pk_device_bytes: bad handle");
+  *bytes = pk_device_bytes(*it->second);
+  return B200_OK;
+}
 
 #define B200_API_BODY(expr)              \
   std::lock_guard<std::mutex> lk(g_mu);  \
@@ -1342,6 +1385,10 @@ int b200_config(int key, int value) {
     g_tma_staging = value;
     return B200_OK;
   }
+  if (key == B200_CFG_TABLE_WINDOWS && value >= 0) {
+    g_table_windows = value;
+    return B200_OK;
+  }
   return fail(B200_EINVAL, "b200_config: unknown key %d or bad value %d", key, value);
 }
 
@@ -1397,6 +1444,21 @@ int b200_bases_info(b200_bases_t h, size_t* n, int* group, int* window_bits, int
   if (group) *group = b->group;
   if (window_bits) *window_bits = (int)b->sh.c;
   if (n_windows) *n_windows = (int)b->sh.nwin;
+  return B200_OK;
+}
+
+int b200_bases_table_windows(b200_bases_t h, int* t) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  Bases* b = find_bases(h, 0);
+  if (!b || !t) return fail(B200_EINVAL, "bases_table_windows: bad handle");
+  *t = (int)b->sh.rows;
+  return B200_OK;
+}
+int b200_bases_device_bytes(b200_bases_t h, size_t* bytes) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  Bases* b = find_bases(h, 0);
+  if (!b || !bytes) return fail(B200_EINVAL, "bases_device_bytes: bad handle");
+  *bytes = bases_device_bytes(*b);
   return B200_OK;
 }
 

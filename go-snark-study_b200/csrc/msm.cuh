@@ -3,18 +3,20 @@
 // (groth16/groth16.go:243-250,269-271; snark.go:265-286).
 //
 // Data layout in HBM (DESIGN.md §3):
-//   table   [nwin][n]  Affine<F>, Montgomery form: table[w][i] = 2^(c*w) * P_i
+//   table   [t][n]     Affine<F>, Montgomery form: table[j][i] = 2^(c*j) * P_i
 //                      (64 B per G1 point, 128 B per G2 point, 32 B-aligned so a
 //                      point is 4 / 8 sector-exact 128-bit loads)
 //   scalars [n]        4 x u64 standard form (or Montgomery if produced by the
 //                      NTT pipeline)
-//   entries [nwin*n]   u32: (w*n + i) << 1 | sign, counting-sorted by bucket
-//   buckets [B]        XYZZ<F>, B = 2^(c-1) (signed digits)
+//   entries [nwin*n]   u32: (j*n + i) << 1 | sign, counting-sorted by bucket
+//   buckets [G*B]      XYZZ<F>, B = 2^(c-1) (signed digits) per window group
 //
-// Because every window's multiple is precomputed (the CRS is static; a 2^20-term
-// G1 table is ~1 GB, so 80 GB of HBM holds the tables of several keys), all windows feed ONE bucket set and the
-// final result is a single sum_b b * S_b — no per-window reduction, no Horner
-// doublings on the critical path.
+// With full tables (t = nwin, the default; the CRS is static and a 2^20-term G1
+// table is ~1 GB) all windows feed ONE bucket set and the final result is a single
+// sum_b b * S_b — no per-window reduction, no Horner doublings on the critical path.
+// A reduced table (t < nwin rows) stores only 2^(c*j) * P_i for j < t: window w
+// reads row j = w mod t and feeds the buckets of group g = w / t, and the tail
+// returns sum_g 2^(c*t*g) * sum_b b * S_(g,b) (one Horner chain over all groups).
 //
 // Pipeline per MSM (one stream, no host sync):
 //   k_digits_count   signed-digit recode, histogram of bucket sizes (RED.ADD)
@@ -168,9 +170,14 @@ struct MsmShape {
   uint32_t n;      // terms
   uint32_t c;      // window bits
   uint32_t nwin;   // ceil(255 / c)
-  uint32_t nbuckets;  // 2^(c-1)
+  uint32_t nbuckets;  // 2^(c-1): buckets of one window group
   uint32_t table_stride;  // points per window in the table (>= n)
+  uint32_t rows = nwin;   // table rows t: window w reads row w mod t (nwin = full tables)
+  uint32_t groups = 1;    // ceil(nwin / rows) window groups, buckets g*nbuckets + 1 .. (g+1)*nbuckets
 };
+
+// Buckets over all window groups: the range of the counting sort, the slice tables and the accumulation.
+__host__ __device__ __forceinline__ uint32_t total_buckets(const MsmShape& sh) { return sh.groups * sh.nbuckets; }
 
 // Signed-digit windows of a 254-bit scalar: digit w in (-2^(c-1), 2^(c-1)].
 // Calls f(w, bucket, sign) for every non-zero digit.
@@ -203,12 +210,23 @@ __device__ __forceinline__ void load_scalar(const Fr* scalars, size_t i, int mon
   for (int k = 0; k < 8; k++) s[k] = v.l[k];
 }
 
+// Where the digit |d| of window w goes: table row w mod t, bucket id g*2^(c-1) + |d| of group g = w / t.
+__device__ __forceinline__ uint32_t digit_row(const MsmShape& sh, uint32_t w, uint32_t d, uint32_t& bucket_id) {
+  const uint32_t g = sh.groups > 1 ? w / sh.rows : 0u;
+  bucket_id = g * sh.nbuckets + d;
+  return w - g * sh.rows;
+}
+
 __global__ void k_digits_count(const Fr* __restrict__ scalars, MsmShape sh, int mont, uint32_t* counts, int* err) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= sh.n) return;
   uint32_t s[8];
   load_scalar(scalars, i, mont, s, err);
-  for_each_digit(s, sh, [&](uint32_t, uint32_t bucket, uint32_t) { atomicAdd(&counts[bucket], 1u); });
+  for_each_digit(s, sh, [&](uint32_t w, uint32_t d, uint32_t) {
+    uint32_t bucket;
+    digit_row(sh, w, d, bucket);
+    atomicAdd(&counts[bucket], 1u);
+  });
 }
 
 __global__ void k_digits_scatter(const Fr* __restrict__ scalars, MsmShape sh, int mont, uint32_t* cursor,
@@ -217,9 +235,11 @@ __global__ void k_digits_scatter(const Fr* __restrict__ scalars, MsmShape sh, in
   if (i >= sh.n) return;
   uint32_t s[8];
   load_scalar(scalars, i, mont, s, err);
-  for_each_digit(s, sh, [&](uint32_t w, uint32_t bucket, uint32_t neg) {
+  for_each_digit(s, sh, [&](uint32_t w, uint32_t d, uint32_t neg) {
+    uint32_t bucket;
+    const uint32_t row = digit_row(sh, w, d, bucket);
     uint32_t pos = atomicAdd(&cursor[bucket], 1u);
-    entries[pos] = ((w * sh.table_stride + (uint32_t)i) << 1) | neg;
+    entries[pos] = ((row * sh.table_stride + (uint32_t)i) << 1) | neg;
   });
 }
 
@@ -376,13 +396,17 @@ __device__ __forceinline__ XYZZ<F> xyzz_mul_small(const XYZZ<F>& p, uint32_t m) 
   return m ? r : XYZZ<F>::inf();
 }
 
-// Segment t covers buckets [t*seg+1, (t+1)*seg]: out[t] = sum_b b * S_b over the segment.
+// Segment t covers buckets [t*seg+1, (t+1)*seg]: out[t] = sum_b b * S_b over the segment.  Window group g = blockIdx.y
+// reads its own nbuckets buckets, writes its own nseg records and scales them by 2^(g*gshift) (gshift = c*t).
 template <class F>
 __global__ void __launch_bounds__(128)
 k_bucket_reduce(const XYZZ<F>* __restrict__ buckets, uint32_t nbuckets, uint32_t seg, XYZZ<F>* __restrict__ out,
-                uint32_t nseg) {
+                uint32_t nseg, uint32_t gshift = 0) {
   uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= nseg) return;
+  const uint32_t g = blockIdx.y;
+  buckets += (size_t)g * nbuckets;
+  out += (size_t)g * nseg;
   uint32_t lo = t * seg + 1;
   uint32_t hi = lo + seg - 1 < nbuckets ? lo + seg - 1 : nbuckets;
   XYZZ<F> acc = XYZZ<F>::inf(), sum = XYZZ<F>::inf();
@@ -392,6 +416,7 @@ k_bucket_reduce(const XYZZ<F>* __restrict__ buckets, uint32_t nbuckets, uint32_t
   }
   XYZZ<F> scaled = xyzz_mul_small(acc, lo - 1);
   xyzz_add(sum, scaled);
+  for (uint32_t k = 0; k < g * gshift; k++) sum = xyzz_dbl(sum);
   out[t] = sum;
 }
 
@@ -446,12 +471,17 @@ __device__ __forceinline__ XYZZ<F> warp_sum_xyzz(XYZZ<F> acc) {
   return acc;   // lane 0 holds the sum
 }
 // warps [0, H): R[hi];  warps [H, H+K): C[lo]      (H = B / K rows of K buckets)
+// Window group g = blockIdx.y reads buckets [g*B, (g+1)*B) and writes R[g*H ..], C[g*K ..].
 template <class F>
 __global__ void __launch_bounds__(128) k_tail_rowcol(const XYZZ<F>* __restrict__ buckets, uint32_t kl, uint32_t H,
                                                      XYZZ<F>* __restrict__ R, XYZZ<F>* __restrict__ C) {
   const uint32_t K = 1u << kl;
   uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
   if (w >= H + K) return;
+  const uint32_t g = blockIdx.y;
+  buckets += ((size_t)g * H) << kl;
+  R += (size_t)g * H;
+  C += (size_t)g * K;
   XYZZ<F> acc = XYZZ<F>::inf();
   if (w < H) {
     for (uint32_t lo = lane; lo < K; lo += 32) xyzz_add(acc, buckets[((size_t)w << kl) + lo]);
@@ -463,12 +493,16 @@ __global__ void __launch_bounds__(128) k_tail_rowcol(const XYZZ<F>* __restrict__
   if (lane == 0) (w < H ? R[w] : C[w - H]) = acc;
 }
 // planes[j] for j < kl: sum of C[i] over i with bit j set; planes[kl + j] for j < kh: sum of R[i] over i with bit j set;
-// planes[kl + kh]: sum of all R[i].   One warp per plane.
+// planes[kl + kh]: sum of all R[i].   One warp per plane; window group g = blockIdx.y has its own R, C and kl + kh + 1 planes.
 template <class F>
 __global__ void __launch_bounds__(128) k_tail_planes(const XYZZ<F>* __restrict__ R, const XYZZ<F>* __restrict__ C, uint32_t kl,
                                                      uint32_t kh, XYZZ<F>* __restrict__ planes) {
   uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
   if (w > kl + kh) return;
+  const uint32_t g = blockIdx.y;
+  R += (size_t)g << kh;
+  C += (size_t)g << kl;
+  planes += (size_t)g * (kl + kh + 1);
   const XYZZ<F>* src = w < kl ? C : R;
   const uint32_t n = w < kl ? (1u << kl) : (1u << kh);
   const uint32_t bit = w < kl ? w : w - kl;
@@ -479,22 +513,29 @@ __global__ void __launch_bounds__(128) k_tail_planes(const XYZZ<F>* __restrict__
   acc = warp_sum_xyzz(acc);
   if (lane == 0) planes[w] = acc;
 }
-// out = sum_{j < nplanes} 2^j planes[j] + planes[nplanes].  One warp; lane q < 16 takes `per` consecutive planes (Horner),
-// shifts its partial sum by q * per doublings, and a 4-level shuffle tree adds the 16 partial sums: ~nplanes + 5 dependent
-// group operations instead of 2 * nplanes for a single Horner chain.
+// out = sum_g 2^(g*gshift) (sum_{j < nplanes} 2^j P_g[j] + P_g[nplanes]) over `groups` window groups, P_g = planes +
+// g*(nplanes + 1) and gshift = c*t (one group: the full-table tail).  The bit positions p = g*gshift + j, 0 <= p < npos,
+// form one Horner chain; positions nplanes <= j < gshift of a group hold no plane.  One warp; lane q < 16 takes `per`
+// consecutive positions, shifts its partial sum by q * per doublings, and a 4-level shuffle tree adds the 16 partial sums:
+// ~npos + 5 dependent group operations (npos ~ 255 for a reduced table) instead of 2 * npos for a single Horner chain.
 template <class F>
-__global__ void __launch_bounds__(32) k_tail_horner(const XYZZ<F>* __restrict__ planes, uint32_t nplanes, XYZZ<F>* __restrict__ out) {
+__global__ void __launch_bounds__(32) k_tail_horner(const XYZZ<F>* __restrict__ planes, uint32_t nplanes, XYZZ<F>* __restrict__ out,
+                                                    uint32_t groups = 1, uint32_t gshift = 0) {
   if (blockIdx.x) return;
   const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t per = (nplanes + 15) / 16;
+  const uint32_t npos = (groups - 1) * gshift + nplanes;
+  const uint32_t per = (npos + 15) / 16;
   XYZZ<F> acc = XYZZ<F>::inf();
   if (lane < 16) {
-    const uint32_t lo = lane * per, hi = lo + per < nplanes ? lo + per : nplanes;
-    for (int j = (int)hi - 1; j >= (int)lo; j--) {
+    const uint32_t lo = lane * per, hi = lo + per < npos ? lo + per : npos;
+    for (int p = (int)hi - 1; p >= (int)lo; p--) {
       acc = xyzz_dbl(acc);
-      xyzz_add(acc, planes[j]);
+      const uint32_t g = groups > 1 ? (uint32_t)p / gshift : 0u, j = (uint32_t)p - g * gshift;
+      const XYZZ<F>* pg = planes + (size_t)g * (nplanes + 1);
+      if (j < nplanes) xyzz_add(acc, pg[j]);
+      if (j == 0 && g > 0) xyzz_add(acc, pg[nplanes]);   // plain sum of group g, weight 2^(g*gshift)
     }
-    if (lo < nplanes)
+    if (lo < npos)
       for (uint32_t d = 0; d < lo; d++) acc = xyzz_dbl(acc);
     if (lane == 0) xyzz_add(acc, planes[nplanes]);
   }

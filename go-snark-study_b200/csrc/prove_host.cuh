@@ -66,6 +66,14 @@ struct ProvingKey {
   DevBuf d_err_sync;
 };
 
+size_t pk_device_bytes(const ProvingKey& pk) {
+  size_t s = dev_bytes({&pk.Z.b_mont, &pk.Z.inv_ntt, &pk.s1, &pk.s2, &pk.s3, &pk.s4, &pk.h_full, &pk.gather, &pk.px,
+                        &pk.w_stage, &pk.res, &pk.out_std, &pk.rs, &pk.d_err, &pk.d_err_sync});
+  for (const auto& g : pk.g)
+    if (g) s += bases_device_bytes(*g);
+  return s;
+}
+
 // Largest proof a host-pointer entry point copies out: Pinocchio's 7 G1 + 1 G2 Jacobian points.
 constexpr size_t kHostProofWords = 7 * 12 + 24;
 
@@ -203,12 +211,6 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   // MSMs cover each other's gaps.
   auto set_terms = [&](int k) { return (double)(pk->hi[k] - pk->lo[k]); };
   auto affine_for = [&](int k) { return world == 1 || set_terms(k) >= (double)(k == 2 ? g_aff_min_g2 : g_aff_min_g1); };
-  // sets that consume identical scalar slices share one digit sort
-  for (int k = 1; k < 3; k++)
-    for (int j = 0; j < k; j++)
-      if (pk->sort_src[k] == k && pk->lo[k] == pk->lo[j] && pk->hi[k] == pk->hi[j] && pk->tail[k] == pk->tail[j] && affine_for(k) == affine_for(j) &&
-          (pk->lo[k] < pk->hi[k] || pk->tail[k]))
-        pk->sort_src[k] = pk->sort_src[j];
   static const uint64_t inf1[12] = {0}, inf2[24] = {0};
   auto has = [&](int k) { return pk->lo[k] < pk->hi[k] || pk->tail[k]; };
   if (has(0)) {
@@ -239,6 +241,12 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
     if (pk->tail[3]) cat.add(delta1, 1);
     if ((rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[3], affine_for(3)))) return rc;
   }
+  // sets that consume identical scalar slices into the same table rows share one digit sort
+  for (int k = 1; k < 3; k++)
+    for (int j = 0; j < k; j++)
+      if (pk->sort_src[k] == k && pk->lo[k] == pk->lo[j] && pk->hi[k] == pk->hi[j] && pk->tail[k] == pk->tail[j] && affine_for(k) == affine_for(j) &&
+          (pk->lo[k] < pk->hi[k] || pk->tail[k]) && pk->g[k]->sh.rows == pk->g[j]->sh.rows)
+        pk->sort_src[k] = pk->sort_src[j];
   CU(pk->s3.alloc((m + n_ptd + 4) * sizeof(Fr)));
   CU(pk->s4.alloc((m + 4) * sizeof(Fr)));
   if (world > 1) CU(pk->h_full.alloc((m + n_ptd + 4) * sizeof(Fr)));

@@ -36,7 +36,9 @@ def rand_fr():
 
 
 class DeviceProvingKey:
-    def __init__(self, pk, n_vars, n_public, window_bits=0):
+    """table_windows: stored window rows t per base set (B200_CFG_TABLE_WINDOWS; 0 = all, the fastest; 1 the smallest)."""
+
+    def __init__(self, pk, n_vars, n_public, window_bits=0, table_windows=0):
         m = n_vars
         g1, g2 = pk["G1"], pk["G2"]
         assert len(g1["At"]) >= m and len(g1["BACGamma"]) >= m and len(g2["BACGamma"]) >= m and len(pk["BACDelta"]) >= m
@@ -49,9 +51,10 @@ class DeviceProvingKey:
         a1, be1, d1 = (_flatten_g1([g1[k]]) for k in ("Alpha", "Beta", "Delta"))
         be2, d2 = (_flatten_g2([g2[k]]) for k in ("Beta", "Delta"))
         h = _lib._h(0)
-        check(lib().b200_groth16_pk_load(ptr(at), ptr(b1), ptr(b2), ptr(cd), m, ptr(ptd), len(pk["PowersTauDelta"]),
-                                         ptr(z), len(pk["Z"]), ptr(a1), ptr(be1), ptr(d1), ptr(be2), ptr(d2),
-                                         n_public, window_bits, h))
+        with _lib.table_windows(table_windows):
+            check(lib().b200_groth16_pk_load(ptr(at), ptr(b1), ptr(b2), ptr(cd), m, ptr(ptd), len(pk["PowersTauDelta"]),
+                                             ptr(z), len(pk["Z"]), ptr(a1), ptr(be1), ptr(d1), ptr(be2), ptr(d2),
+                                             n_public, window_bits, h))
         self.handle = h.value
         self.m = m
 
@@ -82,6 +85,9 @@ class DeviceProvingKey:
                                                ptr(pa), ptr(pb), ptr(pc)))
         return {"PiA": _unflatten_g1(pa)[0], "PiB": _unflatten_g2(pb)[0], "PiC": _unflatten_g1(pc)[0]}
 
+    def device_bytes(self):
+        return _lib.pk_device_bytes(self.handle)
+
     def free(self):
         if self.handle:
             check(lib().b200_pk_free(self.handle))
@@ -99,13 +105,14 @@ class KeyCache:
     def __init__(self, factory, capacity=2):
         self.factory, self.capacity, self.entries = factory, capacity, []
 
-    def get(self, circuit, pk, window_bits=0):
-        shape = (_attr(circuit, "NVars"), _attr(circuit, "NPublic"), window_bits)
+    def get(self, circuit, pk, window_bits=0, table_windows=0):
+        shape = (_attr(circuit, "NVars"), _attr(circuit, "NPublic"), window_bits, table_windows)
         for k, (epk, eshape, dpk) in enumerate(self.entries):
             if epk is pk and eshape == shape:
                 self.entries.append(self.entries.pop(k))          # most recently used last
                 return dpk
-        dpk = self.factory(pk, shape[0], shape[1], window_bits)
+        kw = {"table_windows": table_windows} if table_windows else {}
+        dpk = self.factory(pk, shape[0], shape[1], window_bits, **kw)
         self.entries.append((pk, shape, dpk))
         while len(self.entries) > self.capacity:
             self.entries.pop(0)[2].free()
@@ -121,12 +128,12 @@ class KeyCache:
         self.entries = keep
 
 
-_pk_cache = KeyCache(lambda pk, m, npub, c: DeviceProvingKey(pk, m, npub, c))
+_pk_cache = KeyCache(DeviceProvingKey)
 
 
-def LoadProvingKey(circuit, pk, window_bits=0):
+def LoadProvingKey(circuit, pk, window_bits=0, table_windows=0):
     """Explicit handle form: the returned DeviceProvingKey can be passed as ``pk`` to GenerateProofs."""
-    return _pk_cache.get(circuit, pk, window_bits)
+    return _pk_cache.get(circuit, pk, window_bits, table_windows)
 
 
 def Forget(pk=None):
@@ -247,13 +254,15 @@ class SparseSetup:
                    "G2": {"Beta": _unflatten_g2(self.beta2)[0], "Gamma": _unflatten_g2(self.gamma2)[0],
                           "Delta": _unflatten_g2(self.delta2)[0]}}
 
-    def load_pk(self, window_bits=0, rank=0, world=1):
-        """The key on the device (b200_groth16_pk_load_shard): a DeviceProvingKey with prove_limbs / prove_witness_limbs."""
+    def load_pk(self, window_bits=0, rank=0, world=1, table_windows=0):
+        """The key on the device (b200_groth16_pk_load_shard): a DeviceProvingKey with prove_limbs / prove_witness_limbs.
+        table_windows: stored window rows per base set (B200_CFG_TABLE_WINDOWS; 0 = all)."""
         h = _lib._h(0)
-        check(lib().b200_groth16_pk_load_shard(
-            ptr(self.at), ptr(self.b1), ptr(self.b2), ptr(self.bacdelta), self.m, ptr(self.ptd), self.m - 1, ptr(self.z),
-            self.m - 1, ptr(self.alpha1), ptr(self.beta1), ptr(self.delta1), ptr(self.beta2), ptr(self.delta2),
-            self.npublic, window_bits, rank, world, h))
+        with _lib.table_windows(table_windows):
+            check(lib().b200_groth16_pk_load_shard(
+                ptr(self.at), ptr(self.b1), ptr(self.b2), ptr(self.bacdelta), self.m, ptr(self.ptd), self.m - 1,
+                ptr(self.z), self.m - 1, ptr(self.alpha1), ptr(self.beta1), ptr(self.delta1), ptr(self.beta2),
+                ptr(self.delta2), self.npublic, window_bits, rank, world, h))
         return DeviceProvingKey.from_handle(h.value, self.m)
 
     def pk_dict(self):

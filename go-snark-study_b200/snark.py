@@ -15,16 +15,19 @@ _ORDER = ("PiA", "PiAp", "PiBp", "PiC", "PiCp", "PiH", "PiKp")
 
 
 class DeviceProvingKey:
-    def __init__(self, pk, n_vars, n_public, window_bits=0):
+    """table_windows: stored window rows t per base set (B200_CFG_TABLE_WINDOWS; 0 = all, the fastest; 1 the smallest)."""
+
+    def __init__(self, pk, n_vars, n_public, window_bits=0, table_windows=0):
         m = n_vars
         arr = {k: _flatten_g1(pk[k][:m]) for k in ("A", "Ap", "Bp", "C", "Cp", "Kp")}
         b2 = _flatten_g2(pk["B"][:m])
         g1t = _flatten_g1(pk["G1T"])
         z = ints_to_limbs([int(x) % R for x in pk["Z"]])
         h = _lib._h(0)
-        check(lib().b200_pinocchio_pk_load(ptr(arr["A"]), ptr(arr["Ap"]), ptr(b2), ptr(arr["Bp"]), ptr(arr["C"]),
-                                           ptr(arr["Cp"]), ptr(arr["Kp"]), m, ptr(g1t), len(pk["G1T"]), ptr(z),
-                                           len(pk["Z"]), n_public, window_bits, h))
+        with _lib.table_windows(table_windows):
+            check(lib().b200_pinocchio_pk_load(ptr(arr["A"]), ptr(arr["Ap"]), ptr(b2), ptr(arr["Bp"]), ptr(arr["C"]),
+                                               ptr(arr["Cp"]), ptr(arr["Kp"]), m, ptr(g1t), len(pk["G1T"]), ptr(z),
+                                               len(pk["Z"]), n_public, window_bits, h))
         self.handle = h.value
 
     @classmethod
@@ -43,17 +46,20 @@ class DeviceProvingKey:
         proof["PiB"] = _unflatten_g2(pb)[0]
         return proof
 
+    def device_bytes(self):
+        return _lib.pk_device_bytes(self.handle)
+
     def free(self):
         if self.handle:
             check(lib().b200_pk_free(self.handle))
             self.handle = 0
 
 
-_pk_cache = KeyCache(lambda pk, m, npub, c: DeviceProvingKey(pk, m, npub, c))       # see groth16.KeyCache (identity + strong ref)
+_pk_cache = KeyCache(DeviceProvingKey)       # see groth16.KeyCache (identity + strong ref)
 
 
-def LoadProvingKey(circuit, pk, window_bits=0):
-    return _pk_cache.get(circuit, pk, window_bits)
+def LoadProvingKey(circuit, pk, window_bits=0, table_windows=0):
+    return _pk_cache.get(circuit, pk, window_bits, table_windows)
 
 
 def Forget(pk=None):
@@ -155,12 +161,14 @@ class SparseSetup:
         self.Vk.update(zip(("Vka", "Vkc", "G2Kbg", "G2Kg", "Vkz"), _unflatten_g2(self.vk_g2)))
         self.Vk["IC"] = _unflatten_g1(self.a[:n_public + 1])
 
-    def load_pk(self, window_bits=0, rank=0, world=1):
-        """The key on the device (b200_pinocchio_pk_load_shard): a DeviceProvingKey with prove_limbs."""
+    def load_pk(self, window_bits=0, rank=0, world=1, table_windows=0):
+        """The key on the device (b200_pinocchio_pk_load_shard): a DeviceProvingKey with prove_limbs.
+        table_windows: stored window rows per base set (B200_CFG_TABLE_WINDOWS; 0 = all)."""
         h = _lib._h(0)
-        check(lib().b200_pinocchio_pk_load_shard(
-            ptr(self.a), ptr(self.ap), ptr(self.b2), ptr(self.bp), ptr(self.c), ptr(self.cp), ptr(self.kp), self.m,
-            ptr(self.g1t), self.m - 1, ptr(self.z), self.m - 1, self.npublic, window_bits, rank, world, h))
+        with _lib.table_windows(table_windows):
+            check(lib().b200_pinocchio_pk_load_shard(
+                ptr(self.a), ptr(self.ap), ptr(self.b2), ptr(self.bp), ptr(self.c), ptr(self.cp), ptr(self.kp), self.m,
+                ptr(self.g1t), self.m - 1, ptr(self.z), self.m - 1, self.npublic, window_bits, rank, world, h))
         return DeviceProvingKey.from_handle(h.value)
 
     def pk_dict(self):

@@ -147,6 +147,28 @@ func LoadGroth16Pair(at, b1 [][3]*big.Int, b2 [][3][2]*big.Int, bacDelta, ptd []
 	return
 }
 
+// SetTableWindows sets how many precomputed window rows base sets and proving keys loaded afterwards store
+// (B200_CFG_TABLE_WINDOWS): 0 all (the default, fastest), fewer for circuits whose keys do not fit on the GPU otherwise.
+func SetTableWindows(t int) error { return check(C.b200_config(C.B200_CFG_TABLE_WINDOWS, C.int(t))) }
+
+// LoadGroth16Windows is LoadGroth16 with t stored window rows per base set (SetTableWindows); the option is 0 again after.
+func LoadGroth16Windows(at, b1 [][3]*big.Int, b2 [][3][2]*big.Int, bacDelta, ptd [][3]*big.Int, z []*big.Int,
+	alpha1, beta1, delta1 [3]*big.Int, beta2, delta2 [3][2]*big.Int, nVars, nPublic, t int) (key *Groth16Key, err error) {
+	if err = SetTableWindows(t); err != nil {
+		return nil, err
+	}
+	key, err = LoadGroth16(at, b1, b2, bacDelta, ptd, z, alpha1, beta1, delta1, beta2, delta2, nVars, nPublic)
+	SetTableWindows(0)
+	return
+}
+
+// DeviceBytes is the device memory the key holds (b200_pk_device_bytes).
+func (k *Groth16Key) DeviceBytes() (uint64, error) {
+	var b C.size_t
+	err := check(C.b200_pk_device_bytes(k.h, &b))
+	return uint64(b), err
+}
+
 // PolyMul / PolyDiv back r1csqap.PolynomialField.Mul / Div (r1csqap/r1csqap.go:57-84).
 func PolyMul(a, b []*big.Int) ([]*big.Int, error) {
 	fa, fb := FlatFr(a, Coeff), FlatFr(b, Coeff)

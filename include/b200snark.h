@@ -81,6 +81,16 @@ int b200_version(void);
 #define B200_CFG_SHARD_W_G2 11
 #define B200_CFG_SHARD_AFFINE_MIN_G1 12
 #define B200_CFG_SHARD_AFFINE_MIN_G2 13
+/* B200_CFG_TABLE_WINDOWS: t, the number of precomputed window rows 2^(c*j) * P (j < t) that base sets and proving keys
+ * loaded AFTERWARDS store (b200_g1/g2_bases_load, b200_groth16_pk_load(_shard), b200_pinocchio_pk_load(_shard)).
+ * 0 (default) or any t >= the set's nwin = ceil(255/c) keeps every window: one bucket set, no doublings.  With t < nwin
+ * the table holds t*n points instead of nwin*n; the nwin windows fall into ceil(nwin/t) groups with their own buckets,
+ * recombined by doublings in the bucket tail.  Same results, less memory, a slower MSM: the setting for circuits whose
+ * keys do not fit on the GPU with full tables (INTEGRATION.md "Large circuits").  B200_CFG_ACC_MODE 0 (auto) gives a
+ * set with t < nwin the XYZZ kernel, since the batched-affine scratch alone is about the size of a full table; mode 1
+ * still forces batched affine (with its scratch) where the mean population of the G*2^(c-1) buckets allows it.
+ * Negative: B200_EINVAL.  The trusted setup's own fixed-base table is not affected.                                  */
+#define B200_CFG_TABLE_WINDOWS 14
 int b200_config(int key, int value);
 
 /* ---- base-point sets (the CRS arrays of groth16.Pk / snark.Pk) ---------- */
@@ -95,6 +105,11 @@ int b200_bases_free(b200_bases_t h);
 int b200_bases_info(b200_bases_t h, size_t* n, int* group, int* window_bits, int* n_windows);
 /* which bucket-accumulation kernel the set was built for: 1 batched affine, 2 XYZZ (see b200_config) */
 int b200_bases_acc_mode(b200_bases_t h, int* mode);
+/* t: the window rows the set's table stores (B200_CFG_TABLE_WINDOWS at load; nwin for full tables).  b200_bases_info's
+ * n_windows stays ceil(255/c). */
+int b200_bases_table_windows(b200_bases_t h, int* t);
+/* device memory the set holds: window table, sort and bucket scratch, batched-affine scratch, result buffers */
+int b200_bases_device_bytes(b200_bases_t h, size_t* bytes);
 
 /* ---- multi-scalar multiplication ---------------------------------------- */
 /* out = sum_i scalars[i] * P_i over the first n bases of the set.
@@ -227,6 +242,9 @@ int b200_pinocchio_prove_record_device(b200_pk_t pk, const uint64_t* w, size_t n
                                        void* d_record);
 int b200_pinocchio_finalize_records(const void* d_records, int world, uint64_t* out_g1, uint64_t pi_b[24]);
 int b200_pk_free(b200_pk_t pk);
+/* device memory the key holds: its base sets (b200_bases_device_bytes), the divisor Z and its inverse-series cache, the
+ * scalar, quotient, staging and proof buffers (buffers sized on a key's first proof are counted once allocated) */
+int b200_pk_device_bytes(b200_pk_t pk, size_t* bytes);
 
 /* ---- instrumentation (bench.py) -------------------------------------------- */
 /* b200_profile(flags): bit 0 brackets every bucket-accumulation phase (the dominant
