@@ -110,6 +110,18 @@ def build_host_table_windows(force=False):
     return target
 
 
+def build_host_batch_msm(force=False):
+    """g++ build of the batched MSM pipeline (k scalar vectors over one base set, multi-block counter scan, per-vector
+    tails) over csrc/host_stub (CPU test vehicle, tests/test_host_batch_msm.py)."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    target = os.path.join(LIBDIR, "libb200_host_batch_msm.so")
+    if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):
+        return target
+    _run(["g++", "-O2", "-std=c++17", "-pthread", "-x", "c++", "-shared", "-fPIC", "-Wno-psabi", "-I", os.path.join(HOSTTEST, "host_stub"),
+          "-I", HOSTTEST, "-I", CSRC, "-o", target, os.path.join(HOSTTEST, "batch_msm_test.cpp")])
+    return target
+
+
 def build_shard_partition(force=False):
     """g++ build of csrc/shard_partition.h behind a C entry point (CPU test vehicle, tests/test_shard_partition.py)."""
     os.makedirs(LIBDIR, exist_ok=True)

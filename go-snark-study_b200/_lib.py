@@ -48,6 +48,7 @@ _SIGNATURES = {
     "b200_g1_msm": [_h, _vp, _sz, _vp],
     "b200_g2_msm": [_h, _vp, _sz, _vp],
     "b200_msm_device": [_h, _vp, _sz, _int, _vp, _vp],
+    "b200_msm_device_batch": [_h, _vp, _sz, _sz, _sz, _int, _vp, _vp],
     "b200_g1_sum_partials": [_vp, _sz, _vp, _vp],
     "b200_g2_sum_partials": [_vp, _sz, _vp, _vp],
     "b200_g1_mul_batch": [_vp, _vp, _sz, _vp],

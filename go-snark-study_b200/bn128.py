@@ -103,6 +103,17 @@ class BaseSet:
         check(fn(self.handle, ptr(limbs), n, ptr(out)))
         return _unflatten_g1(out)[0] if self.group == 1 else _unflatten_g2(out)[0]
 
+    def msm_device_batch(self, d_scalars, n, k, d_out, stride=None, mont=0, stream=None):
+        """k MSMs over the first n bases in one set of launches (b200_msm_device_batch): record p of ``d_out`` (k XYZZ
+        records of 16 / 32 u64 words, device memory) is sum_i scalar[p*stride + i] * P_i.  ``d_scalars`` / ``d_out`` are
+        device pointers or objects with ``data_ptr()`` (torch tensors); ``stream`` a cudaStream_t or an object with
+        ``cuda_stream``; ``stride`` defaults to n.  No host synchronisation."""
+        def _p(x):
+            return None if x is None else (x.data_ptr() if hasattr(x, "data_ptr") else int(x))
+        st = getattr(stream, "cuda_stream", stream)
+        check(lib().b200_msm_device_batch(self.handle, _p(d_scalars), n, k, n if stride is None else stride, mont,
+                                          _p(d_out), st))
+
     def free(self):
         if self.handle:
             check(lib().b200_bases_free(self.handle))

@@ -165,10 +165,10 @@ int pick_window_bits(size_t n) {
   return best;
 }
 
-// Records of launch_bucket_tail's scratch: H rows, K columns and c planes per window group.
+// Records of launch_bucket_tail's scratch: H rows, K columns and c planes per window group of every scalar vector.
 size_t bucket_tail_records(const MsmShape& sh) {
   const uint32_t bits = sh.c - 1, kl = (bits + 1) / 2, kh = bits - kl;
-  return (size_t)sh.groups * ((1u << kh) + (1u << kl) + bits + 1);
+  return (size_t)sh.vecs * sh.groups * ((1u << kh) + (1u << kl) + bits + 1);
 }
 
 // Output of the digit-recode / counting-sort front end for one scalar vector.  It depends only on the
@@ -182,6 +182,28 @@ struct SortScratch {
   SliceTables tables() const { return SliceTables{slice_off.as<uint32_t>(), slice_start.as<uint32_t>(), slice_end.as<uint32_t>()}; }
 };
 
+// Scratch of the bucket phase: slice sums, buckets, tail records and, for batched-affine accumulation (affine_S > 0),
+// ping-pong node buffers, prefix products and per-thread / per-block products.
+struct BucketScratch {
+  DevBuf slice_out, buckets, partials;
+  DevBuf nodeA, nodeB, aff_pre, aff_others, aff_btot, aff_ids;
+};
+
+// Front-end and bucket scratch of b200_msm_device_batch on one base set, sized for `vecs` scalar vectors of the set's
+// full size.  Allocated on the set's first batch and grown (never shrunk) when a later batch has more vectors.
+struct MsmBatch {
+  uint32_t vecs = 0;
+  SortScratch sort;
+  BucketScratch bk;
+  DevBuf scan_totals;   // per-block totals of the multi-block counter scan
+  cudaEvent_t done = nullptr;   // recorded behind the last batch on the set: a regrowth waits for it, not for the device
+  MsmBatch() = default;
+  MsmBatch(const MsmBatch&) = delete;
+  MsmBatch& operator=(const MsmBatch&) = delete;
+  ~MsmBatch() { if (done) cudaEventDestroy(done); }
+};
+constexpr uint32_t kScanBlocks = 1024;   // upper bound on the blocks of a batch's counter scan
+
 struct Bases {
   int group = 0;  // 1: G1 (Fq), 2: G2 (Fq2)
   size_t n = 0;
@@ -189,12 +211,12 @@ struct Bases {
   DevBuf table;    // [nwin][n] Affine<F>
   // per-base-set scratch of the bucket phase (different base sets may run concurrently)
   DevBuf scalars;  // n * 32 B (host-scalar entry points)
-  DevBuf slice_out, buckets, partials, result, out_std;
+  BucketScratch bk;
+  DevBuf result, out_std;
   SortScratch sort;  // own front-end scratch (stand-alone MSMs)
   uint32_t nseg = 0, seg = 0;
-  // batched-affine accumulation (affine_S > 0): ping-pong node buffers, prefix products, per-thread / per-block products
-  uint32_t affine_S = 0;
-  DevBuf nodeA, nodeB, aff_pre, aff_others, aff_btot, aff_ids;
+  uint32_t affine_S = 0;   // > 0: batched-affine accumulation with slices of affine_S entries
+  std::unique_ptr<MsmBatch> batch;   // b200_msm_device_batch scratch (null until the first batch)
   // error word of b200_msm_device on this set: written by the kernels, never read (the call cannot wait for it, and a
   // later call on any object must not report it; see b200snark.h).  Host-pointer MSMs use g_d_err.
   DevBuf d_err;
@@ -206,17 +228,21 @@ size_t dev_bytes(std::initializer_list<const DevBuf*> bufs) {
   for (const DevBuf* d : bufs) s += d->p ? d->bytes : 0;
   return s;
 }
+size_t scratch_device_bytes(const SortScratch& ss, const BucketScratch& bk) {
+  return dev_bytes({&ss.counts, &ss.offsets, &ss.cursor, &ss.entries, &ss.slice_off, &ss.slice_start, &ss.slice_end,
+                    &bk.slice_out, &bk.buckets, &bk.partials, &bk.nodeA, &bk.nodeB, &bk.aff_pre, &bk.aff_others,
+                    &bk.aff_btot, &bk.aff_ids});
+}
 size_t bases_device_bytes(const Bases& b) {
-  const SortScratch& ss = b.sort;
-  return dev_bytes({&b.table, &b.scalars, &b.slice_out, &b.buckets, &b.partials, &b.result, &b.out_std, &b.nodeA, &b.nodeB,
-                    &b.aff_pre, &b.aff_others, &b.aff_btot, &b.aff_ids, &b.d_err, &ss.counts, &ss.offsets, &ss.cursor,
-                    &ss.entries, &ss.slice_off, &ss.slice_start, &ss.slice_end});
+  size_t s = dev_bytes({&b.table, &b.scalars, &b.result, &b.out_std, &b.d_err}) + scratch_device_bytes(b.sort, b.bk);
+  if (b.batch) s += scratch_device_bytes(b.batch->sort, b.batch->bk) + dev_bytes({&b.batch->scan_totals});
+  return s;
 }
 
 int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
   ss.sh = sh;
   ss.slice_S = slice_S;
-  size_t entries = (size_t)sh.nwin * sh.n;
+  size_t entries = (size_t)sh.vecs * sh.nwin * sh.n;
   const uint32_t B = total_buckets(sh);
   CU(ss.counts.alloc((B + 2) * sizeof(uint32_t)));
   CU(ss.offsets.alloc((B + 3) * sizeof(uint32_t)));
@@ -228,6 +254,26 @@ int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
   CU(ss.slice_off.alloc((B + 3) * sizeof(uint32_t)));
   CU(ss.slice_start.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
   CU(ss.slice_end.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
+  return B200_OK;
+}
+
+// Bucket scratch for the shape `sh` (its vecs included) over the sort scratch `ss`: affine_S > 0 adds the batched-affine
+// buffers for ss.max_slices slices; nseg: segments per window group of the c < 7 tail.
+template <class F>
+int bucket_alloc(BucketScratch& bk, const MsmShape& sh, const SortScratch& ss, uint32_t affine_S, uint32_t nseg) {
+  CU(bk.buckets.alloc((size_t)total_buckets(sh) * sizeof(XYZZ<F>)));
+  if (const uint32_t S = affine_S) {
+    size_t nsl = ss.max_slices;
+    CU(bk.nodeA.alloc(nsl * (S / 2) * sizeof(Affine<F>)));
+    CU(bk.nodeB.alloc(nsl * (S / 4 ? S / 4 : 1) * sizeof(Affine<F>)));
+    CU(bk.aff_pre.alloc(nsl * (S / 2) * sizeof(F)));
+    CU(bk.aff_ids.alloc(nsl * (S / 2) * sizeof(uint2)));
+    size_t nblk_max = (nsl * (S / 2) + kAffBlock * kAffPairs - 1) / (kAffBlock * kAffPairs);
+    CU(bk.aff_others.alloc(nblk_max * kAffBlock * sizeof(F)));
+    CU(bk.aff_btot.alloc(nblk_max * sizeof(F)));
+  }
+  CU(bk.slice_out.alloc((size_t)(affine_S ? 1 : ss.max_slices) * sizeof(XYZZ<F>)));
+  CU(bk.partials.alloc(std::max((size_t)sh.vecs * sh.groups * nseg + 1024, bucket_tail_records(sh)) * sizeof(XYZZ<F>)));
   return B200_OK;
 }
 
@@ -285,7 +331,6 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   if ((uint64_t)sh.nwin * n >= (1ull << 31)) return fail(B200_EINVAL, "nwin*n exceeds 2^31 entries");
   CU(b->table.alloc((size_t)sh.rows * n * sizeof(Affine<F>)));
   CU(b->scalars.alloc(n * sizeof(Fr)));
-  CU(b->buckets.alloc((size_t)total_buckets(sh) * sizeof(XYZZ<F>)));
   {
     // accumulation mode: batched affine (6.5 multiplies per add, 3 launches per round) where the buckets are populated
     // enough to amortise the rounds, else XYZZ mixed adds (10 multiplies, one launch); b200_config forces either.  Auto
@@ -301,23 +346,13 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
     b->affine_S = S;
     int rc_ = sort_alloc(b->sort, sh, S);
     if (rc_) return rc_;
-    if (S) {
-      size_t nsl = b->sort.max_slices;
-      CU(b->nodeA.alloc(nsl * (S / 2) * sizeof(Affine<F>)));
-      CU(b->nodeB.alloc(nsl * (S / 4 ? S / 4 : 1) * sizeof(Affine<F>)));
-      CU(b->aff_pre.alloc(nsl * (S / 2) * sizeof(F)));
-      CU(b->aff_ids.alloc(nsl * (S / 2) * sizeof(uint2)));
-      size_t nblk_max = (nsl * (S / 2) + kAffBlock * kAffPairs - 1) / (kAffBlock * kAffPairs);
-      CU(b->aff_others.alloc(nblk_max * kAffBlock * sizeof(F)));
-      CU(b->aff_btot.alloc(nblk_max * sizeof(F)));
-    }
   }
-  CU(b->slice_out.alloc((size_t)(b->affine_S ? 1 : b->sort.max_slices) * sizeof(XYZZ<F>)));
   // short latency chain: 4-bucket segments (8 adds + one small scalar mul per thread), then a two-level tree sum
   // (c < 7); nseg segments per window group.  c >= 7: the scratch of launch_bucket_tail.
   b->seg = sh.nbuckets >= 256 ? 4 : 1;
   b->nseg = (sh.nbuckets + b->seg - 1) / b->seg;
-  CU(b->partials.alloc(std::max((size_t)sh.groups * b->nseg + 1024, bucket_tail_records(sh)) * sizeof(XYZZ<F>)));
+  int rc_ = bucket_alloc<F>(b->bk, sh, b->sort, b->affine_S, b->nseg);
+  if (rc_) return rc_;
   CU(b->result.alloc(sizeof(XYZZ<F>)));
   CU(b->out_std.alloc(3 * sizeof(F)));
   CU(b->d_err.alloc(sizeof(int)));
@@ -396,41 +431,66 @@ void launch_tree_sum(XYZZ<F>* partials, uint32_t n, XYZZ<F>* d_out, cudaStream_t
   g_launches += 2;
 }
 
-// sum_g 2^(c*t*g) sum_b b * S_(g,b) over the bucket array -> one XYZZ record (msm.cuh: rows / columns and bit planes of
-// every window group, one Horner chain over all groups).  `scratch` holds bucket_tail_records(sh) records.  Tiny bucket
-// sets keep the segment kernel.
+constexpr uint32_t kMaxGridY = 65535;   // gridDim.y limit: rows per launch of the (vector, group) tail kernels
+
+// sum_g 2^(c*t*g) sum_b b * S_(g,b) over the bucket array -> one XYZZ record per scalar vector (msm.cuh: rows / columns
+// and bit planes of every window group, one Horner chain over the groups of each vector).  `scratch` holds
+// bucket_tail_records(sh) records.  Tiny bucket sets keep the segment kernel.
 template <class F>
 void launch_bucket_tail(const XYZZ<F>* buckets, const MsmShape& sh, XYZZ<F>* scratch, XYZZ<F>* d_out, cudaStream_t st) {
   const uint32_t bits = sh.c - 1, kl = (bits + 1) / 2, kh = bits - kl, K = 1u << kl, H = 1u << kh, G = sh.groups;
+  const uint32_t GV = sh.vecs * G;
   XYZZ<F>* R = scratch;
-  XYZZ<F>* C = scratch + (size_t)G * H;
-  XYZZ<F>* planes = C + (size_t)G * K;
-  k_tail_rowcol<F><<<dim3(nblocks((size_t)(H + K) * 32, 128), G), 128, 0, st>>>(buckets, kl, H, R, C);
-  k_tail_planes<F><<<dim3(nblocks((size_t)(bits + 1) * 32, 128), G), 128, 0, st>>>(R, C, kl, kh, planes);
-  k_tail_horner<F><<<1, 32, 0, st>>>(planes, bits, d_out, G, sh.c * sh.rows);
-  g_launches += 3;
+  XYZZ<F>* C = scratch + (size_t)GV * H;
+  XYZZ<F>* planes = C + (size_t)GV * K;
+  for_each_tail_chunk(sh, kMaxGridY, [&](uint32_t y0, uint32_t ny) {
+    k_tail_rowcol<F><<<dim3(nblocks((size_t)(H + K) * 32, 128), ny), 128, 0, st>>>(buckets + (size_t)y0 * H * K, kl, H,
+                                                                                    R + (size_t)y0 * H, C + (size_t)y0 * K);
+    k_tail_planes<F><<<dim3(nblocks((size_t)(bits + 1) * 32, 128), ny), 128, 0, st>>>(
+        R + (size_t)y0 * H, C + (size_t)y0 * K, kl, kh, planes + (size_t)y0 * (bits + 1));
+    g_launches += 2;
+  });
+  k_tail_horner<F><<<sh.vecs, 32, 0, st>>>(planes, bits, d_out, G, sh.c * sh.rows);
+  g_launches += 1;
 }
 
-// The c < 7 tail: segment sums of every window group, each scaled by 2^(c*t*g), then one tree sum over all of them.
+// The c < 7 tail: segment sums of every window group, each scaled by 2^(c*t*g), then one tree sum over all of them (one
+// block per scalar vector in a batch).
 template <class F>
-void launch_segment_tail(const Bases* b, const XYZZ<F>* buckets, XYZZ<F>* partials, XYZZ<F>* d_out, cudaStream_t st) {
-  const MsmShape& sh = b->sh;
-  k_bucket_reduce<F><<<dim3(nblocks(b->nseg, 128), sh.groups), 128, 0, st>>>(buckets, sh.nbuckets, b->seg, partials, b->nseg,
-                                                                              sh.c * sh.rows);
-  launch_tree_sum<F>(partials, sh.groups * b->nseg, d_out, st);
+void launch_segment_tail(const Bases* b, const MsmShape& sh, const XYZZ<F>* buckets, XYZZ<F>* partials, XYZZ<F>* d_out,
+                         cudaStream_t st) {
+  if (sh.vecs == 1) {
+    k_bucket_reduce<F><<<dim3(nblocks(b->nseg, 128), sh.groups), 128, 0, st>>>(buckets, sh.nbuckets, b->seg, partials, b->nseg,
+                                                                                sh.c * sh.rows);
+    launch_tree_sum<F>(partials, sh.groups * b->nseg, d_out, st);
+    return;
+  }
+  for_each_tail_chunk(sh, kMaxGridY, [&](uint32_t y0, uint32_t ny) {
+    k_bucket_reduce<F, true><<<dim3(nblocks(b->nseg, 128), ny), 128, 0, st>>>(
+        buckets + (size_t)y0 * sh.nbuckets, sh.nbuckets, b->seg, partials + (size_t)y0 * b->nseg, b->nseg, sh.c * sh.rows,
+        sh.groups);
+    if (y0) g_launches += 1;   // the caller counts the first k_bucket_reduce
+  });
+  const uint32_t per = sh.groups * b->nseg;
+  k_sum_points<F><<<sh.vecs, 256, 0, st>>>(partials, sh.vecs * per, per, d_out);
+  g_launches += 1;
 }
 
-// Front end: signed-digit recode + counting sort of n scalars into bucket order (3 launches).  A standard-form scalar
-// >= r is read as 0 and sets bit 1 of *err.
-int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, int* err, cudaStream_t st) {
-  if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride || shape.rows != ss.sh.rows)
+// Front end: signed-digit recode + counting sort of n scalars (of each of shape.vecs vectors) into bucket order.  A
+// standard-form scalar >= r is read as 0 and sets bit 1 of *err.  With `scan_totals` (room for kScanBlocks values) a
+// large batch scans its counters with several blocks (one more launch).
+int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, int* err, cudaStream_t st,
+             unsigned long long* scan_totals = nullptr) {
+  if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride || shape.rows != ss.sh.rows ||
+      shape.vecs > ss.sh.vecs)
     return fail(B200_EINVAL, "msm_sort: shape mismatch");
   MsmShape sh = shape;
   sh.n = (uint32_t)n;
   const uint32_t B = total_buckets(sh);
   uint32_t m = B + 1;  // counts[0] unused (digit 0), buckets 1..B of all window groups
-  // slice cap: twice the mean bucket population (uniform scalars never split), at least 4 per lane
-  uint64_t mean = ((uint64_t)sh.nwin * n + B - 1) / B;
+  // slice cap: twice the mean bucket population (uniform scalars never split), at least 4 per lane.  The mean over a
+  // batch's buckets is that of one vector.
+  uint64_t mean = ((uint64_t)sh.vecs * sh.nwin * n + B - 1) / B;
   uint32_t cap = (uint32_t)(2 * mean < 4 * kLPB ? 4 * kLPB : 2 * mean);
   int fixed = 0;
   if (ss.slice_S) {
@@ -438,35 +498,47 @@ int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t
     fixed = 1;
   }
   uint32_t* counts = ss.counts.as<uint32_t>();
+  const size_t nterm = (size_t)sh.vecs * n;
   CU(cudaMemsetAsync(counts, 0, (m + 1) * sizeof(uint32_t), st));
-  if (n) k_digits_count<<<nblocks(n, 256), 256, 0, st>>>(d_scalars, sh, mont, counts, err);
-  k_scan<<<1, 1024, 0, st>>>(counts, m, cap, fixed, ss.offsets.as<uint32_t>(), ss.cursor.as<uint32_t>(), ss.tables());
+  if (n) k_digits_count<<<nblocks(nterm, 256), 256, 0, st>>>(d_scalars, sh, mont, counts, err);
+  // one block walks up to 64 tiles of counters; beyond that, blocks of 64 tiles each (at most kScanBlocks)
+  constexpr uint32_t kScanTile = 1024, kScanChunk = 64 * kScanTile;
+  if (scan_totals && m > kScanChunk) {
+    uint32_t chunk = kScanChunk;
+    while ((m + chunk - 1) / chunk > kScanBlocks) chunk *= 2;
+    const uint32_t nb = (m + chunk - 1) / chunk;
+    k_scan_totals<<<nb, kScanTile, 0, st>>>(counts, m, cap, chunk, scan_totals);
+    k_scan<<<nb, kScanTile, 0, st>>>(counts, m, cap, fixed, ss.offsets.as<uint32_t>(), ss.cursor.as<uint32_t>(), ss.tables(),
+                                     chunk, scan_totals);
+    g_launches += 1;
+  } else {
+    k_scan<<<1, kScanTile, 0, st>>>(counts, m, cap, fixed, ss.offsets.as<uint32_t>(), ss.cursor.as<uint32_t>(), ss.tables());
+  }
   k_fill_slices<<<nblocks(m, 256), 256, 0, st>>>(counts, ss.offsets.as<uint32_t>(), m, cap, fixed, ss.tables());
-  if (n) k_digits_scatter<<<nblocks(n, 256), 256, 0, st>>>(d_scalars, sh, mont, ss.cursor.as<uint32_t>(),
-                                                           ss.entries.as<uint32_t>(), err);
+  if (n) k_digits_scatter<<<nblocks(nterm, 256), 256, 0, st>>>(d_scalars, sh, mont, ss.cursor.as<uint32_t>(),
+                                                               ss.entries.as<uint32_t>(), err);
   g_launches += n ? 4 : 2;
   CU(cudaGetLastError());
   return B200_OK;
 }
 
 // Back end: bucket accumulation over the sorted entries of `ss`, slice merge, weighted bucket
-// reduction and final tree sum -> one XYZZ record in d_out (4 launches).
+// reduction and final tree sum -> one XYZZ record in d_out per scalar vector (vecs of them), in the scratch `bk`.
 template <class F>
-int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out, cudaStream_t st) {
-  const MsmShape& sh = b->sh;
-  if (ss.sh.c != sh.c || ss.sh.table_stride != sh.table_stride || ss.sh.rows != sh.rows || ss.max_slices != b->sort.max_slices ||
-      ss.slice_S != b->sort.slice_S)
-    return fail(B200_EINVAL, "msm_buckets: sort scratch does not match the base set");
+int bucket_phase(Bases* b, const SortScratch& ss, BucketScratch& bk, uint32_t vecs, size_t n_terms, XYZZ<F>* d_out,
+                 cudaStream_t st) {
+  MsmShape sh = b->sh;
+  sh.vecs = vecs;
   const uint32_t B = total_buckets(sh);
   uint32_t m = B + 1;
-  XYZZ<F>* buckets = b->buckets.as<XYZZ<F>>();
-  XYZZ<F>* partials = b->partials.as<XYZZ<F>>();
+  XYZZ<F>* buckets = bk.buckets.as<XYZZ<F>>();
+  XYZZ<F>* partials = bk.partials.as<XYZZ<F>>();
   SliceTables stb = ss.tables();
   // The out-of-line F_q multiply wins here: the fully inlined madd body (~38 KB of SASS) thrashes the
   // instruction caches.
   ProfRec pr{};
   if (g_prof) {
-    pr = ProfRec{prof_event(), prof_event(), b->group, n_terms};
+    pr = ProfRec{prof_event(), prof_event(), b->group, (size_t)vecs * n_terms};
     cudaEventRecord(pr.e0, st);
   }
   if (b->affine_S) {
@@ -475,7 +547,7 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
     uint32_t R = 0;
     while ((1u << R) < S) R++;
     // host-side bound on the live slice count for this call (the exact count lives on the device)
-    uint64_t total = (uint64_t)sh.nwin * n_terms;
+    uint64_t total = (uint64_t)vecs * sh.nwin * n_terms;
     uint64_t nsl_bound = (uint64_t)B + (total + S - 1) / S + 2;
     if (nsl_bound > ss.max_slices) nsl_bound = ss.max_slices;
     AffineRound<F> ar{};
@@ -484,13 +556,13 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
     ar.slice_start = stb.slice_start;
     ar.slice_end = stb.slice_end;
     ar.nslices_ptr = stb.slice_off + m;
-    ar.pre = b->aff_pre.as<F>();
-    ar.others = b->aff_others.as<F>();
-    ar.btot = b->aff_btot.as<F>();
-    ar.pair_ids = g_tma_staging == 1 ? b->aff_ids.as<uint2>() : nullptr;
+    ar.pre = bk.aff_pre.as<F>();
+    ar.others = bk.aff_others.as<F>();
+    ar.btot = bk.aff_btot.as<F>();
+    ar.pair_ids = g_tma_staging == 1 ? bk.aff_ids.as<uint2>() : nullptr;
     // node buffers, x- and y-coordinates in separate halves (bucket_affine.cuh NodeBuf)
     const size_t capA = (size_t)ss.max_slices * (S / 2), capB = (size_t)ss.max_slices * (S / 4 ? S / 4 : 1);
-    NodeBuf<F> bufs[2] = {{b->nodeA.as<F>(), b->nodeA.as<F>() + capA}, {b->nodeB.as<F>(), b->nodeB.as<F>() + capB}};
+    NodeBuf<F> bufs[2] = {{bk.nodeA.as<F>(), bk.nodeA.as<F>() + capA}, {bk.nodeB.as<F>(), bk.nodeB.as<F>() + capB}};
     NodeBuf<F> prev{nullptr, nullptr};
     // all R rounds affine: inside a proof the per-round inversion latency is hidden by the other MSMs' streams
     for (uint32_t r = 1; r <= R; r++) {
@@ -525,30 +597,40 @@ int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out,
       launch_bucket_tail<F>(buckets, sh, partials, d_out, st);
       g_launches += 1;
     } else {
-      launch_segment_tail<F>(b, buckets, partials, d_out, st);
+      launch_segment_tail<F>(b, sh, buckets, partials, d_out, st);
       g_launches += 2;
     }
     CU(cudaGetLastError());
     return B200_OK;
   }
-  uint64_t mean = ((uint64_t)sh.nwin * n_terms + B - 1) / B;
+  uint64_t mean = ((uint64_t)vecs * sh.nwin * n_terms + B - 1) / B;   // that of one vector
   int lpb = mean >= 384 ? 8 : (mean >= 96 ? 4 : 2);
   launch_accumulate<F>(lpb, b->table.as<Affine<F>>(), ss.entries.as<uint32_t>(), stb, m,
-                       b->slice_out.as<XYZZ<F>>(), ss.max_slices, st);
+                       bk.slice_out.as<XYZZ<F>>(), ss.max_slices, st);
   if (g_prof) {
     cudaEventRecord(pr.e1, st);
     g_prof_recs.push_back(pr);
   }
-  k_merge_slices<F><<<nblocks(B, 128), 128, 0, st>>>(b->slice_out.as<XYZZ<F>>(), stb, B, buckets);
+  k_merge_slices<F><<<nblocks(B, 128), 128, 0, st>>>(bk.slice_out.as<XYZZ<F>>(), stb, B, buckets);
   if (sh.c >= 7) {
     launch_bucket_tail<F>(buckets, sh, partials, d_out, st);
     g_launches += 1;
   } else {
-    launch_segment_tail<F>(b, buckets, partials, d_out, st);
+    launch_segment_tail<F>(b, sh, buckets, partials, d_out, st);
     g_launches += 3;
   }
   CU(cudaGetLastError());
   return B200_OK;
+}
+
+// One MSM's back end in the set's own bucket scratch (4 launches + the tail).
+template <class F>
+int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out, cudaStream_t st) {
+  const MsmShape& sh = b->sh;
+  if (ss.sh.c != sh.c || ss.sh.table_stride != sh.table_stride || ss.sh.rows != sh.rows || ss.max_slices != b->sort.max_slices ||
+      ss.slice_S != b->sort.slice_S)
+    return fail(B200_EINVAL, "msm_buckets: sort scratch does not match the base set");
+  return bucket_phase<F>(b, ss, b->bk, 1, n_terms, d_out, st);
 }
 
 template <class F>
@@ -557,6 +639,63 @@ int msm_enqueue(Bases* b, const Fr* d_scalars, size_t n, int mont, XYZZ<F>* d_ou
   int rc = msm_sort(b->sort, b->sh, d_scalars, n, mont, err, st);
   if (rc) return rc;
   return msm_buckets<F>(b, b->sort, n, d_out, st);
+}
+
+// ---- batches: k scalar vectors over one base set -----------------------------------------------------------------
+// Term i of vector p is scalar p*stride + i times base i; vector p's digits go to its own window groups, so one recode,
+// one counting sort, one accumulation and one tail serve all k vectors.  Populations per bucket, and so the slice cap,
+// the lanes per bucket and the accumulation kernel, are those of one vector.
+bool batch_fits(const Bases* b, size_t k, size_t n) {
+  return (uint64_t)k * b->sh.nwin * n < (1ull << 31) && (uint64_t)k * total_buckets(b->sh) + 3 < (1ull << 31);
+}
+
+// The batch scratch of `b` for k vectors of n terms: allocated on the first batch, regrown to the larger of the old and
+// the new capacity in each dimension when a batch exceeds it.  Before the old buffers are freed the host waits for the
+// set's last batch (its `done` event); batches on one set are ordered on one stream (b200snark.h), so nothing else of
+// this set can still read them, and work on other sets and prove contexts is not waited for.
+template <class F>
+int batch_scratch(Bases* b, uint32_t k, uint32_t n) {
+  if (n == 0) n = 1;
+  if (b->batch && b->batch->vecs >= k && b->batch->sort.sh.n >= n) return B200_OK;
+  if (b->batch) {
+    CU(cudaEventSynchronize(b->batch->done));
+    const uint32_t k2 = std::max(k, b->batch->vecs), n2 = std::max(n, b->batch->sort.sh.n);
+    if (batch_fits(b, k2, n2)) k = k2, n = n2;   // else: exactly this batch's size
+  }
+  b->batch.reset();
+  auto mb = std::make_unique<MsmBatch>();
+  MsmShape sh = b->sh;
+  sh.n = n;
+  sh.vecs = k;
+  int rc = sort_alloc(mb->sort, sh, b->affine_S);
+  if (rc) return rc;
+  if ((rc = bucket_alloc<F>(mb->bk, sh, mb->sort, b->affine_S, b->nseg))) return rc;
+  CU(mb->scan_totals.alloc(kScanBlocks * sizeof(unsigned long long)));
+  CU(cudaEventCreateWithFlags(&mb->done, cudaEventDisableTiming));
+  mb->vecs = k;
+  b->batch = std::move(mb);
+  return B200_OK;
+}
+
+template <class F>
+int msm_batch_enqueue(Bases* b, const Fr* d_scalars, size_t n, size_t k, size_t stride, int mont, XYZZ<F>* d_out, int* err,
+                      cudaStream_t st) {
+  if (k == 0) return fail(B200_EINVAL, "msm_device_batch: k = 0");
+  if (n > b->n) return fail(B200_EINVAL, "msm_device_batch: n=%zu exceeds base set size %zu", n, b->n);
+  if (stride > 0xffffffffull) return fail(B200_EINVAL, "msm_device_batch: stride %zu exceeds 2^32 - 1", stride);
+  if (!batch_fits(b, k, n ? n : 1))
+    return fail(B200_EINVAL, "msm_device_batch: k * nwin * n = %zu * %u * %zu sort entries (or the buckets) exceed 2^31", k,
+                b->sh.nwin, n);
+  int rc = batch_scratch<F>(b, (uint32_t)k, (uint32_t)n);
+  if (rc) return rc;
+  MsmBatch& mb = *b->batch;
+  MsmShape sh = b->sh;
+  sh.vecs = (uint32_t)k;
+  sh.vec_stride = (uint32_t)stride;
+  if ((rc = msm_sort(mb.sort, sh, d_scalars, n, mont, err, st, mb.scan_totals.as<unsigned long long>()))) return rc;
+  if ((rc = bucket_phase<F>(b, mb.sort, mb.bk, (uint32_t)k, n, d_out, st))) return rc;
+  CU(cudaEventRecord(mb.done, st));
+  return B200_OK;
 }
 
 template <class F>
@@ -1489,6 +1628,17 @@ int b200_msm_device(b200_bases_t h, const void* d_scalars, size_t n, int mont, v
   int* err = b->d_err.as<int>();
   if (b->group == 1) return msm_enqueue<Fq>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq>*)d_out, err, st);
   return msm_enqueue<Fq2>(b, (const Fr*)d_scalars, n, mont, (XYZZ<Fq2>*)d_out, err, st);
+}
+int b200_msm_device_batch(b200_bases_t h, const void* d_scalars, size_t n, size_t k, size_t stride, int mont, void* d_out,
+                          void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  Bases* b = find_bases(h, 0);
+  if (!b || !d_out || (!d_scalars && n)) return fail(B200_EINVAL, "msm_device_batch: bad arguments");
+  cudaStream_t st = stream ? (cudaStream_t)stream : g_ctx[0].main;
+  int* err = b->d_err.as<int>();
+  if (b->group == 1) return msm_batch_enqueue<Fq>(b, (const Fr*)d_scalars, n, k, stride, mont, (XYZZ<Fq>*)d_out, err, st);
+  return msm_batch_enqueue<Fq2>(b, (const Fr*)d_scalars, n, k, stride, mont, (XYZZ<Fq2>*)d_out, err, st);
 }
 
 int b200_g1_sum_partials(const void* d, size_t count, uint64_t out[12], void* stream) {

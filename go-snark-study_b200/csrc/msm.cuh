@@ -9,7 +9,7 @@
 //   scalars [n]        4 x u64 standard form (or Montgomery if produced by the
 //                      NTT pipeline)
 //   entries [nwin*n]   u32: (j*n + i) << 1 | sign, counting-sorted by bucket
-//   buckets [G*B]      XYZZ<F>, B = 2^(c-1) (signed digits) per window group
+//   buckets [k*G*B]    XYZZ<F>, B = 2^(c-1) (signed digits) per window group of each of k scalar vectors (k = 1 but in a batch)
 //
 // With full tables (t = nwin, the default; the CRS is static and a 2^20-term G1
 // table is ~1 GB) all windows feed ONE bucket set and the final result is a single
@@ -174,10 +174,14 @@ struct MsmShape {
   uint32_t table_stride;  // points per window in the table (>= n)
   uint32_t rows = nwin;   // table rows t: window w reads row w mod t (nwin = full tables)
   uint32_t groups = 1;    // ceil(nwin / rows) window groups, buckets g*nbuckets + 1 .. (g+1)*nbuckets
+  // k scalar vectors over the same bases (b200_msm_device_batch): term i of vector p is scalar p*vec_stride + i times
+  // base i, and vector p owns window groups p*groups .. (p+1)*groups - 1 of the bucket range
+  uint32_t vecs = 1;
+  uint32_t vec_stride = 0;
 };
 
-// Buckets over all window groups: the range of the counting sort, the slice tables and the accumulation.
-__host__ __device__ __forceinline__ uint32_t total_buckets(const MsmShape& sh) { return sh.groups * sh.nbuckets; }
+// Buckets over all window groups of all vectors: the range of the counting sort, the slice tables and the accumulation.
+__host__ __device__ __forceinline__ uint32_t total_buckets(const MsmShape& sh) { return sh.vecs * sh.groups * sh.nbuckets; }
 
 // Signed-digit windows of a 254-bit scalar: digit w in (-2^(c-1), 2^(c-1)].
 // Calls f(w, bucket, sign) for every non-zero digit.
@@ -210,34 +214,53 @@ __device__ __forceinline__ void load_scalar(const Fr* scalars, size_t i, int mon
   for (int k = 0; k < 8; k++) s[k] = v.l[k];
 }
 
-// Where the digit |d| of window w goes: table row w mod t, bucket id g*2^(c-1) + |d| of group g = w / t.
-__device__ __forceinline__ uint32_t digit_row(const MsmShape& sh, uint32_t w, uint32_t d, uint32_t& bucket_id) {
+// Where the digit |d| of window w goes: table row w mod t, bucket id (vg + g)*2^(c-1) + |d| of group g = w / t, with vg
+// the first group of the term's scalar vector.
+__device__ __forceinline__ uint32_t digit_row(const MsmShape& sh, uint32_t w, uint32_t d, uint32_t& bucket_id, uint32_t vg = 0) {
   const uint32_t g = sh.groups > 1 ? w / sh.rows : 0u;
-  bucket_id = g * sh.nbuckets + d;
+  bucket_id = (vg + g) * sh.nbuckets + d;
   return w - g * sh.rows;
 }
 
+// Thread i of the recode kernels takes term i of vector i / n (one vector: term i).  Returns false past the last term;
+// `vg` is the vector's first window group and `si` the scalar's index.
+__device__ __forceinline__ bool batch_term(const MsmShape& sh, size_t& i, size_t& si, uint32_t& vg) {
+  if (sh.vecs == 1) {
+    si = i;
+    vg = 0;
+    return i < sh.n;
+  }
+  const size_t p = i / sh.n;
+  if (p >= sh.vecs) return false;
+  i -= p * sh.n;
+  si = p * sh.vec_stride + i;
+  vg = (uint32_t)p * sh.groups;
+  return true;
+}
+
 __global__ void k_digits_count(const Fr* __restrict__ scalars, MsmShape sh, int mont, uint32_t* counts, int* err) {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= sh.n) return;
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x, si;
+  uint32_t vg;
+  if (!batch_term(sh, i, si, vg)) return;
   uint32_t s[8];
-  load_scalar(scalars, i, mont, s, err);
+  load_scalar(scalars, si, mont, s, err);
   for_each_digit(s, sh, [&](uint32_t w, uint32_t d, uint32_t) {
     uint32_t bucket;
-    digit_row(sh, w, d, bucket);
+    digit_row(sh, w, d, bucket, vg);
     atomicAdd(&counts[bucket], 1u);
   });
 }
 
 __global__ void k_digits_scatter(const Fr* __restrict__ scalars, MsmShape sh, int mont, uint32_t* cursor,
                                  uint32_t* __restrict__ entries, int* err) {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= sh.n) return;
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x, si;
+  uint32_t vg;
+  if (!batch_term(sh, i, si, vg)) return;
   uint32_t s[8];
-  load_scalar(scalars, i, mont, s, err);
+  load_scalar(scalars, si, mont, s, err);
   for_each_digit(s, sh, [&](uint32_t w, uint32_t d, uint32_t neg) {
     uint32_t bucket;
-    const uint32_t row = digit_row(sh, w, d, bucket);
+    const uint32_t row = digit_row(sh, w, d, bucket, vg);
     uint32_t pos = atomicAdd(&cursor[bucket], 1u);
     entries[pos] = ((row * sh.table_stride + (uint32_t)i) << 1) | neg;
   });
@@ -255,21 +278,48 @@ struct SliceTables {
 };
 // fixed != 0: slices hold exactly `cap` entry slots (last one of a bucket partially filled) — the
 // perfect-binary-tree layout of the batched-affine accumulation.
+//
+// The counters of a batch of k scalar vectors (k*G*2^(c-1) of them) are scanned by several blocks: block b takes counters
+// [b*chunk, (b+1)*chunk), k_scan_totals first writes every block's packed (entries, slices) total, and block b starts
+// from the sum of the totals before it.  One block (chunk >= m, no totals) is the single-MSM scan.
+__device__ __forceinline__ unsigned long long scan_item(const uint32_t* counts, uint32_t k, uint32_t hi, uint32_t cap) {
+  uint32_t c = k < hi ? counts[k] : 0u;
+  uint32_t sl = (k == 0 || k >= hi) ? 0u : (c <= cap ? 1u : (c + cap - 1) / cap);
+  return ((unsigned long long)sl << 32) | c;
+}
+__global__ void __launch_bounds__(1024) k_scan_totals(const uint32_t* __restrict__ counts, uint32_t m, uint32_t cap,
+                                                      uint32_t chunk, unsigned long long* __restrict__ totals) {
+  __shared__ unsigned long long tot_s;
+  const uint32_t lo = blockIdx.x * chunk, hi = m - lo < chunk ? m : lo + chunk;
+  if (threadIdx.x == 0) tot_s = 0ull;
+  __syncthreads();
+  unsigned long long v = 0ull;
+  for (uint32_t k = lo + threadIdx.x; k < hi; k += blockDim.x) v += scan_item(counts, k, hi, cap);
+  if (v) atomicAdd(&tot_s, v);
+  __syncthreads();
+  if (threadIdx.x == 0) totals[blockIdx.x] = tot_s;
+}
 __global__ void __launch_bounds__(1024) k_scan(const uint32_t* __restrict__ counts, uint32_t m, uint32_t cap, int fixed,
-                                               uint32_t* offsets, uint32_t* cursor, SliceTables st) {
-  // One block walks the m counters in coalesced tiles of blockDim.x; (entry count, slice count) are packed into one
+                                               uint32_t* offsets, uint32_t* cursor, SliceTables st,
+                                               uint32_t chunk = 0xffffffffu, const unsigned long long* totals = nullptr) {
+  // One block walks its counters in coalesced tiles of blockDim.x; (entry count, slice count) are packed into one
   // 64-bit value so a single warp-shuffle scan + a scan of the warp totals serves both prefix sums.  (The first version
   // gave every thread 64 consecutive counters: uncoalesced and serial.)
   __shared__ unsigned long long wsum[32];
   __shared__ unsigned long long carry_s;
   const uint32_t t = threadIdx.x, T = blockDim.x, lane = t & 31u, warp = t >> 5, nwarps = T >> 5;
+  const uint32_t lo = blockIdx.x * chunk, hi = m - lo < chunk ? m : lo + chunk;
   if (t == 0) carry_s = 0ull;
   __syncthreads();
-  for (uint32_t base = 0; base < m; base += T) {
+  if (totals) {   // the blocks before this one
+    unsigned long long before = 0ull;
+    for (uint32_t j = t; j < blockIdx.x; j += T) before += totals[j];
+    if (before) atomicAdd(&carry_s, before);
+    __syncthreads();
+  }
+  for (uint32_t base = lo; base < hi; base += T) {
     uint32_t k = base + t;
-    uint32_t c = k < m ? counts[k] : 0u;
-    uint32_t sl = (k == 0 || k >= m) ? 0u : (c <= cap ? 1u : (c + cap - 1) / cap);
-    unsigned long long v = ((unsigned long long)sl << 32) | c, incl = v;
+    unsigned long long v = scan_item(counts, k, hi, cap), incl = v;
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
       unsigned long long up = __shfl_up_sync(0xffffffffu, incl, off);
@@ -289,7 +339,7 @@ __global__ void __launch_bounds__(1024) k_scan(const uint32_t* __restrict__ coun
     __syncthreads();
     unsigned long long carry = carry_s;
     unsigned long long excl = carry + wsum[warp] + (incl - v);
-    if (k < m) {
+    if (k < hi) {
       uint32_t run = (uint32_t)excl, srun = (uint32_t)(excl >> 32);
       offsets[k] = run;
       cursor[k] = run;
@@ -299,7 +349,7 @@ __global__ void __launch_bounds__(1024) k_scan(const uint32_t* __restrict__ coun
     if (t == T - 1) carry_s = excl + v;   // inclusive prefix of the tile's last element = new carry
     __syncthreads();
   }
-  if (t == 0) {
+  if (t == 0 && hi == m) {
     unsigned long long tot = carry_s;
     offsets[m] = (uint32_t)tot;
     st.slice_off[m] = (uint32_t)(tot >> 32);
@@ -396,17 +446,18 @@ __device__ __forceinline__ XYZZ<F> xyzz_mul_small(const XYZZ<F>& p, uint32_t m) 
   return m ? r : XYZZ<F>::inf();
 }
 
-// Segment t covers buckets [t*seg+1, (t+1)*seg]: out[t] = sum_b b * S_b over the segment.  Window group g = blockIdx.y
-// reads its own nbuckets buckets, writes its own nseg records and scales them by 2^(g*gshift) (gshift = c*t).
-template <class F>
+// Segment t covers buckets [t*seg+1, (t+1)*seg]: out[t] = sum_b b * S_b over the segment.  Window group y = blockIdx.y
+// reads its own nbuckets buckets, writes its own nseg records and scales them by 2^(g*gshift) (gshift = c*t): g = y for
+// one MSM, g = y mod `groups` in a batch of scalar vectors (BATCH, a separate instantiation: the one-MSM kernel is unchanged).
+template <class F, bool BATCH = false>
 __global__ void __launch_bounds__(128)
 k_bucket_reduce(const XYZZ<F>* __restrict__ buckets, uint32_t nbuckets, uint32_t seg, XYZZ<F>* __restrict__ out,
-                uint32_t nseg, uint32_t gshift = 0) {
+                uint32_t nseg, uint32_t gshift = 0, uint32_t groups = 1) {
   uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= nseg) return;
-  const uint32_t g = blockIdx.y;
-  buckets += (size_t)g * nbuckets;
-  out += (size_t)g * nseg;
+  const uint32_t y = blockIdx.y, g = BATCH ? y % groups : y;
+  buckets += (size_t)y * nbuckets;
+  out += (size_t)y * nseg;
   uint32_t lo = t * seg + 1;
   uint32_t hi = lo + seg - 1 < nbuckets ? lo + seg - 1 : nbuckets;
   XYZZ<F> acc = XYZZ<F>::inf(), sum = XYZZ<F>::inf();
@@ -513,15 +564,26 @@ __global__ void __launch_bounds__(128) k_tail_planes(const XYZZ<F>* __restrict__
   acc = warp_sum_xyzz(acc);
   if (lane == 0) planes[w] = acc;
 }
+// Row chunks of the tail kernels that take (vector, window group) as blockIdx.y: launch(y0, ny) for consecutive chunks of
+// the vecs*groups rows, each at most max_rows rows (65535 on the device: the gridDim.y limit) and a multiple of groups,
+// so that blockIdx.y mod groups inside a chunk is still the window group.
+template <class Fn>
+inline void for_each_tail_chunk(const MsmShape& sh, uint32_t max_rows, Fn&& launch) {
+  const uint32_t rows = sh.vecs * sh.groups, whole = max_rows / sh.groups, chunk = (whole ? whole : 1u) * sh.groups;
+  for (uint32_t y0 = 0; y0 < rows; y0 += chunk) launch(y0, rows - y0 < chunk ? rows - y0 : chunk);
+}
+
 // out = sum_g 2^(g*gshift) (sum_{j < nplanes} 2^j P_g[j] + P_g[nplanes]) over `groups` window groups, P_g = planes +
 // g*(nplanes + 1) and gshift = c*t (one group: the full-table tail).  The bit positions p = g*gshift + j, 0 <= p < npos,
 // form one Horner chain; positions nplanes <= j < gshift of a group hold no plane.  One warp; lane q < 16 takes `per`
 // consecutive positions, shifts its partial sum by q * per doublings, and a 4-level shuffle tree adds the 16 partial sums:
 // ~npos + 5 dependent group operations (npos ~ 255 for a reduced table) instead of 2 * npos for a single Horner chain.
+// Block v runs the chain of scalar vector v of a batch: its groups * (nplanes + 1) planes, record out[v].
 template <class F>
 __global__ void __launch_bounds__(32) k_tail_horner(const XYZZ<F>* __restrict__ planes, uint32_t nplanes, XYZZ<F>* __restrict__ out,
                                                     uint32_t groups = 1, uint32_t gshift = 0) {
-  if (blockIdx.x) return;
+  planes += (size_t)blockIdx.x * groups * (nplanes + 1);
+  out += blockIdx.x;
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t npos = (groups - 1) * gshift + nplanes;
   const uint32_t per = (npos + 15) / 16;

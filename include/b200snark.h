@@ -135,6 +135,29 @@ int b200_g2_msm(b200_bases_t h, const uint64_t* scalars, size_t n, uint64_t out_
  * scalars_mont != 0 any 256-bit value v is accepted and read as v * 2^-256 mod r. */
 int b200_msm_device(b200_bases_t h, const void* d_scalars, size_t n, int scalars_mont,
                     void* d_out_xyzz, void* stream);
+/* k MSMs over the same first n bases in one set of launches: record p (k XYZZ
+ * records, 128 B / 256 B apart in d_out_xyzz) is sum_i d_scalars[p*stride + i] * P_i.
+ * The contract is that of b200_msm_device (device memory, no host synchronisation,
+ * scalars_mont, no range report); k = 1 gives b200_msm_device's record.  Any stride
+ * (0 included) is accepted; the scalar buffer holds (k-1)*stride + n scalars.
+ * One digit recode, counting sort, bucket accumulation and bucket tail serve all k
+ * vectors, so a batch of small MSMs costs about one MSM of k*n terms.  The launches
+ * are those of one MSM, plus one when k*G*2^(c-1) bucket counters exceed 64 Ki
+ * (G = window groups: 1 for full tables; the counter scan then runs on several
+ * blocks) and one or two per further 65535 (vector, group) rows of the tail.
+ * Scratch: the first batch on a set allocates sort, bucket and (batched-affine
+ * sets) node buffers for k vectors of n terms, about k times those of one n-term
+ * MSM; a later batch with more vectors or terms grows them (the host first waits
+ * for the set's previous batch) and they are never shrunk.
+ * b200_bases_device_bytes / b200_pk_device_bytes count them.  Single MSMs keep
+ * their own buffers.
+ * Each base set has ONE scratch for its single MSMs (b200_msm_device,
+ * b200_g*_msm) and one for its batches: calls on the same set must be ordered,
+ * e.g. issued on one stream; sets are independent of each other.
+ * B200_EINVAL: k = 0, n > the set's size, stride >= 2^32, or k*ceil(255/c)*n sort
+ * entries (or k times the set's buckets) reaching 2^31; nothing is allocated then. */
+int b200_msm_device_batch(b200_bases_t h, const void* d_scalars, size_t n, size_t k, size_t stride,
+                          int scalars_mont, void* d_out_xyzz, void* stream);
 /* Sum `count` XYZZ partial records (device memory, e.g. the gathered per-rank
  * partials) and normalise: out_jac = (x, y, 1) in standard form on the host,
  * infinity as all-zero.  1 <= count <= 2^20, else B200_EINVAL.  Synchronises `stream`. */
