@@ -163,6 +163,11 @@ __global__ void k_h_values(const Fr* __restrict__ V, uint32_t M, const Fr* __res
   Fr va = V[Y], vb = V[(size_t)M + Y], vc = V[2 * (size_t)M + Y];
   hv[j] = (va * vb * fact[Y] - vc) * fact[j];
 }
+// c[j] = a[j] * b[j], j < n: the values the quotient path uses in place of (C w)_j (qap_h_from_values)
+__global__ void k_row_products(const Fr* __restrict__ a, const Fr* __restrict__ b, uint32_t n, Fr* __restrict__ c) {
+  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n) c[j] = a[j] * b[j];
+}
 // schoolbook level of the tree: tc2[p*2s + i] = sum_{a+b=i} tL[a] tR[b] + (i >= s ? tL[i-s] + tR[i-s] : 0)
 __global__ void k_tree_school(const Fr* __restrict__ tc, uint32_t s, uint32_t N, Fr* __restrict__ tc2) {
   uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -408,8 +413,12 @@ inline cudaError_t interpolate_ap(PolyCtx& pc, const QapDomain& dom, QapWork& wk
 // interpolations (a, b, c -> coefficients), one product and one division, evaluate a, b, c on the NEXT n - 1 points
 // n+1 .. 2n-1 from their Newton coefficients (a(1 + Y) / Y! = sum_k d_k / (Y - k)!: one cyclic product with the cached
 // transform of 1/i! each), form h there pointwise — Z(1 + Y) = Y! / (Y - n)! — and interpolate h ONCE over the points
-// n+1 .. 2n-1 (subproduct tree with offset n).  Same field elements as DivisorPolynomial(CombinePolynomials(..)), ~40 % fewer
-// multiplications than going through px.
+// n+1 .. 2n-1 (subproduct tree with offset n).  ~40 % fewer multiplications than going through px.
+// This interpolates the quotient only where a b - c vanishes on 1..n.  For any witness, DivisorPolynomial drops the
+// remainder, and since deg c < n = deg Z, quotient(a b - c, Z) = quotient(a b - c', Z) for c' the interpolant of the
+// products a_j b_j — for which a b - c' does vanish on 1..n.  So the values of c are replaced by a_j b_j
+// (qap_h_from_values) and C w is never formed: the same field elements as DivisorPolynomial(CombinePolynomials(..)) for
+// satisfied and unsatisfied witnesses alike.
 // The scratch of one quotient computation; a proof in flight needs its own (one per prove context).
 struct QapHWork {
   QapWork work;                 // e^-x cache etc. of the final interpolation
@@ -461,6 +470,16 @@ inline cudaError_t qap_h_from_newton(PolyCtx& pc, QapHDomain& hd, const Fr* d, s
   pc.note(8);
   return cudaGetLastError();
 }
+// vals: the values of a | b on {1..n} in blocks 0 and 1 (n-strided, Montgomery); block 2 is overwritten with the products
+// a_j b_j.  d: 3 blocks of dom.N for the Newton coefficients (dom: the QAP domain of size >= n).  h as qap_h_from_newton.
+inline cudaError_t qap_h_from_values(PolyCtx& pc, const QapDomain& dom, QapWork& wk, QapHDomain& hd, Fr* vals, Fr* d,
+                                     cudaStream_t st, QapHWork* ws = nullptr) {
+  const size_t n = hd.n;
+  B200_LAUNCH(k_row_products, nblk(n, 256), 256, st, vals, vals + n, (uint32_t)n, vals + 2 * n);
+  pc.note(1);
+  PCU(newton_coeffs(pc, dom, wk, vals, n, n, 3, d, st));
+  return qap_h_from_newton(pc, hd, d, dom.N, st, ws);
+}
 
 // ---- a sparse R1CS resident on the device ------------------------------------------------------------------
 struct SparseMat {
@@ -471,7 +490,8 @@ struct SparseMat {
 // Witness -> px / h scratch of one proof in flight on an R1CS: one per prove context, so proofs on keys of the two
 // contexts may share the R1CS and overlap.
 struct R1csWork {
-  DevBuf w_mont, vals, coef;        // witness (m), A w | B w | C w (3 x n), coefficients (3 x N), all Montgomery
+  DevBuf w_mont, vals, coef;        // witness (m), A w | B w | C w (3 x n; the quotient path: A w | B w | their products),
+                                    // coefficients (3 x N), all Montgomery
   DevBuf px_mont;                   // 2n - 1
   DevBuf h_std;                     // h = px / Z, n - 1 coefficients, standard form (h-direct branch)
   QapWork work;

@@ -145,8 +145,9 @@ int qap_px_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, Fr* d_
 }
 
 // d_w: m witness values (device, standard form; an entry >= r is read as 0 and sets bit 1 of *err) -> the n - 1
-// coefficients of h = (ax*bx - cx) / Z in ws.h_std (standard form), without forming px (qap_sparse.cuh: QapHDomain).
-// Requires n >= 2.  The domains are shared by every context: built on g_ctx[0].main and waited for on the first call.
+// coefficients of h = DivisorPolynomial(ax*bx - cx, Z) in ws.h_std (standard form), without forming px (qap_sparse.cuh:
+// QapHDomain).  The quotient does not depend on cx, so C w is not computed.  Requires n >= 2.  The domains are shared by
+// every context: built on g_ctx[0].main and waited for on the first call.
 int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
   const size_t n = r->n, m = r->m, N = pow2_at_least(n);
   if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
@@ -161,13 +162,12 @@ int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* er
   Fr* w = ws.w_mont.as<Fr>();
   k_poly_load<<<nblk(m, 256), 256, 0, st>>>(d_w_std, (uint32_t)m, (uint32_t)m, 0, 0, w, (uint32_t)m, err);
   Fr* vals = ws.vals.as<Fr>();
-  for (int k = 0; k < 3; k++)
+  for (int k = 0; k < 2; k++)
     k_spmv_csr<<<nblk(n, 128), 128, 0, st>>>(r->M[k].rowptr.as<uint32_t>(), r->M[k].col.as<uint32_t>(), r->M[k].val.as<Fr>(), w,
                                               (uint32_t)n, vals + k * n);
-  g_launches += 4;
-  Fr* coef = ws.coef.as<Fr>();   // here: the Newton coefficients of a | b | c (N-strided)
-  CU(newton_coeffs(pc, *dom, ws.work, vals, n, n, 3, coef, st));
-  CU(qap_h_from_newton(pc, *r->hd, coef, N, st, &ws.hw));
+  g_launches += 3;
+  Fr* coef = ws.coef.as<Fr>();   // here: the Newton coefficients of a | b | a*b (N-strided)
+  CU(qap_h_from_values(pc, *dom, ws.work, *r->hd, vals, coef, st, &ws.hw));
   k_poly_store<<<nblk(n - 1, 256), 256, 0, st>>>(ws.hw.coef.as<Fr>(), (uint32_t)(n - 1), 0, 1, ws.h_std.as<Fr>());
   g_launches += 1;
   CU(cudaGetLastError());

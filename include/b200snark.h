@@ -379,7 +379,10 @@ int b200_pinocchio_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs);
 /* groth16.GenerateProofs fed from the witness: px is computed on the device from the resident R1CS (b200_qap_px) and
  * never leaves HBM; otherwise identical to b200_groth16_prove (groth16/groth16.go:225-278 after the caller's
- * CombinePolynomials step, cli/main.go:339-349).  nw must equal the key's m and the R1CS's m.  Like b200_groth16_prove
+ * CombinePolynomials step, cli/main.go:339-349).  When len(Z) = n + 1 the quotient h = DivisorPolynomial(px, Z) is
+ * computed without forming px (C w is not needed: deg cx < deg Z); like the reference, it drops the remainder, so a
+ * witness that does not satisfy the R1CS gets the same proof as from b200_groth16_prove with its px (which does not
+ * verify).  nw must equal the key's m and the R1CS's m.  Like b200_groth16_prove
  * it runs on the key's prove context (B200_CFG_PK_CONTEXT) and waits with the library mutex released, so two host
  * threads proving on keys of contexts 0 and 1 overlap, also when both keys share one R1CS handle.  A sharded key needs
  * a matching communicator (b200_comm_init; SPMD, the proof is returned on every rank); without one the call returns
@@ -388,7 +391,8 @@ int b200_groth16_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w
                                const uint64_t s[4], uint64_t pi_a[12], uint64_t pi_b[24], uint64_t pi_c[12]);
 /* groth16.GenerateProofs fed from a DEVICE-resident witness (m standard-form scalars): b200_groth16_prove_witness with
  * the result left in device memory on `stream`, as in b200_groth16_prove_device (48 u64 PiA | PiC | PiB; on a sharded
- * key without a communicator, the 1 KB partial record for b200_groth16_finalize_device).
+ * key without a communicator, the 1 KB partial record for b200_groth16_finalize_device).  Any witness is proved, as
+ * by the reference: the quotient drops the remainder of px / Z, as b200_groth16_prove_device does with the same px.
  *   - No host synchronisation, except on the FIRST call for a given (R1CS, prove context) pair: that call builds the
  *     R1CS's interpolation domains (shared by both contexts) and the context's workspaces, and may synchronise.
  *   - Proofs on keys of the two prove contexts may be in flight together on two streams, also on one R1CS handle (each

@@ -498,7 +498,8 @@ int qap_interpolate(const uint32_t* values_std, uint32_t n, uint32_t* coeffs_std
   std::memcpy(coeffs_std, out.data(), (size_t)n * sizeof(Fr));
   return 0;
 }
-// h = (a b - c) / Z straight from the values of a, b, c on {1..n} (qap_sparse.cuh: QapHDomain), as qap_h_enqueue runs it
+// h = DivisorPolynomial(a b - c, Z) straight from the values of a, b, c on {1..n} (qap_sparse.cuh: QapHDomain), as
+// qap_h_enqueue runs it: the values of c are overwritten by the products a_j b_j, so any c gives the same quotient
 int qap_h_direct(const uint32_t* abc_std, uint32_t n, uint32_t* h_std) {
   size_t N = 1;
   while (N < n) N <<= 1;
@@ -508,10 +509,9 @@ int qap_h_direct(const uint32_t* abc_std, uint32_t n, uint32_t* h_std) {
   std::memcpy(v.data(), abc_std, v.size() * sizeof(Fr));
   for (auto& x : v) x = x.to_mont();
   QapWork wk;
-  if (newton_coeffs(poly_ctx(), dom, wk, v.data(), n, n, 3, d.data(), nullptr)) return 2;
   QapHDomain hd;
   if (qap_hdomain_build(poly_ctx(), hd, n, nullptr)) return 3;
-  if (qap_h_from_newton(poly_ctx(), hd, d.data(), N, nullptr)) return 4;
+  if (qap_h_from_values(poly_ctx(), dom, wk, hd, v.data(), d.data(), nullptr)) return 4;
   const Fr* c = hd.coef.as<Fr>();
   for (uint32_t i = 0; i + 1 < n; i++) {
     Fr x = c[i].from_mont();

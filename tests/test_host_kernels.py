@@ -316,6 +316,63 @@ def test_quotient_h_directly_from_the_values(lib, n):
             assert _horner(h, t) * zt % R_ == (_horner(ax, t) * _horner(bx, t) - _horner(cx, t)) % R_
 
 
+def _lagrange_at(n, t):
+    """[l_j(t)], the Lagrange basis of {1..n} at t (t not in 1..n), from factorials and one batch inversion."""
+    fact = [1] * n
+    for i in range(1, n):
+        fact[i] = fact[i - 1] * i % R_
+    den = [(t - j - 1) * fact[j] % R_ * fact[n - 1 - j] % R_ for j in range(n)]
+    pre, zt = [1] * (n + 1), 1
+    for j in range(n):
+        pre[j + 1] = pre[j] * den[j] % R_
+        zt = zt * (t - j - 1) % R_
+    inv, out = pow(pre[n], -1, R_), [0] * n
+    for j in range(n - 1, -1, -1):
+        v = zt * inv % R_ * pre[j] % R_
+        out[j] = (R_ - v) % R_ if (n - 1 - j) & 1 else v
+        inv = inv * den[j] % R_
+    return out
+
+
+@pytest.mark.parametrize("how", ["first", "last", "middle", "every", "c=0"])
+@pytest.mark.parametrize("n", [2, 3, 7, 16, 21, 40, 100, 1024, 1500])
+def test_quotient_h_directly_drops_the_remainder(lib, n, how):
+    """Values of an UNSATISFIED R1CS (c_j != a_j b_j on one row — the first, the last or n/2 — on every row, or c = 0):
+    groth16.GenerateProofs takes h = DivisorPolynomial(px, Z), the quotient with the remainder dropped
+    (r1csqap.go:213-216), and so must the direct path.  Equal to the oracle's quotient for n <= 40; above, checked through
+    h(t) Z(t) = a(t) b(t) - c(t) - rem(t) at random t, where rem = px mod Z is the interpolant of the row residuals
+    a_j b_j - c_j (all from an independent Lagrange basis at t)."""
+    rng = random.Random(7000 + n)
+    a = [rng.randrange(R_) for _ in range(n)]
+    b = [rng.randrange(R_) for _ in range(n)]
+    c = [x * y % R_ for x, y in zip(a, b)]
+    if how == "every":
+        c = [rng.randrange(R_) for _ in range(n)]
+    elif how == "c=0":
+        c = [0] * n
+    else:
+        j = {"first": 0, "last": n - 1, "middle": n // 2}[how]
+        c[j] = (c[j] + 1) % R_
+    out = np.zeros(8 * max(n - 1, 1), dtype=np.uint32)
+    assert lib.t_qap_h_direct(_ptr(_u32(a + b + c)), n, _ptr(out)) == 0
+    h = _limbs_to_ints(out, n - 1)
+    if n <= 40:
+        ax, bx, cx = (o.PF.lagrange_interpolation(v) for v in (a, b, c))
+        z = [1]
+        for i in range(1, n + 1):
+            z = o.PF.mul(z, [(-i) % R_, 1])
+        assert h == o.PF.divisor_polynomial(o.PF.sub(o.PF.mul(ax, bx), cx), z)
+    for _ in range(3 if n <= 40 else 5):
+        t = rng.randrange(n + 1, R_)
+        lag = _lagrange_at(n, t)
+        at_, bt_, ct_ = (sum(v * l for v, l in zip(vs, lag)) % R_ for vs in (a, b, c))
+        rem = sum((x * y - z_) * l for x, y, z_, l in zip(a, b, c, lag)) % R_
+        zt = 1
+        for i in range(1, n + 1):
+            zt = zt * (t - i) % R_
+        assert _horner(h, t) * zt % R_ == (at_ * bt_ - ct_ - rem) % R_, t
+
+
 @pytest.mark.parametrize("na,nb", [(13, 7), (200, 101), (1023, 513), (2600, 1300)])
 def test_division_orchestration_on_the_cpu(lib, na, nb):
     """poly_div_device (poly_host.cuh: Newton inverse series of the reversed divisor, cached transform, fused transform
