@@ -239,6 +239,13 @@ size_t bases_device_bytes(const Bases& b) {
   return s;
 }
 
+// slices: every bucket owns >= 1; a bucket above cap = 2*mean entries is cut => at most B + B/2 + 1
+uint32_t sort_max_slices(const MsmShape& sh, uint32_t slice_S) {
+  const size_t entries = (size_t)sh.vecs * sh.nwin * sh.n;
+  const uint32_t B = total_buckets(sh);
+  return slice_S ? B + (uint32_t)((entries + slice_S - 1) / slice_S) + 2 : B + B / 2 + 2;
+}
+
 int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
   ss.sh = sh;
   ss.slice_S = slice_S;
@@ -248,22 +255,20 @@ int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
   CU(ss.offsets.alloc((B + 3) * sizeof(uint32_t)));
   CU(ss.cursor.alloc((B + 2) * sizeof(uint32_t)));
   CU(ss.entries.alloc(entries * sizeof(uint32_t)));
-  // slices: every bucket owns >= 1; a bucket above cap = 2*mean entries is cut => at most B + B/2 + 1
-  ss.max_slices = B + B / 2 + 2;
-  if (slice_S) ss.max_slices = B + (uint32_t)((entries + slice_S - 1) / slice_S) + 2;
+  ss.max_slices = sort_max_slices(sh, slice_S);
   CU(ss.slice_off.alloc((B + 3) * sizeof(uint32_t)));
   CU(ss.slice_start.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
   CU(ss.slice_end.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
   return B200_OK;
 }
 
-// Bucket scratch for the shape `sh` (its vecs included) over the sort scratch `ss`: affine_S > 0 adds the batched-affine
-// buffers for ss.max_slices slices; nseg: segments per window group of the c < 7 tail.
+// Bucket scratch for the shape `sh` (its vecs included) over a sort scratch of max_slices slices: affine_S > 0 adds the
+// batched-affine buffers; nseg: segments per window group of the c < 7 tail.
 template <class F>
-int bucket_alloc(BucketScratch& bk, const MsmShape& sh, const SortScratch& ss, uint32_t affine_S, uint32_t nseg) {
+int bucket_alloc(BucketScratch& bk, const MsmShape& sh, uint32_t max_slices, uint32_t affine_S, uint32_t nseg) {
   CU(bk.buckets.alloc((size_t)total_buckets(sh) * sizeof(XYZZ<F>)));
   if (const uint32_t S = affine_S) {
-    size_t nsl = ss.max_slices;
+    size_t nsl = max_slices;
     CU(bk.nodeA.alloc(nsl * (S / 2) * sizeof(Affine<F>)));
     CU(bk.nodeB.alloc(nsl * (S / 4 ? S / 4 : 1) * sizeof(Affine<F>)));
     CU(bk.aff_pre.alloc(nsl * (S / 2) * sizeof(F)));
@@ -272,7 +277,7 @@ int bucket_alloc(BucketScratch& bk, const MsmShape& sh, const SortScratch& ss, u
     CU(bk.aff_others.alloc(nblk_max * kAffBlock * sizeof(F)));
     CU(bk.aff_btot.alloc(nblk_max * sizeof(F)));
   }
-  CU(bk.slice_out.alloc((size_t)(affine_S ? 1 : ss.max_slices) * sizeof(XYZZ<F>)));
+  CU(bk.slice_out.alloc((size_t)(affine_S ? 1 : max_slices) * sizeof(XYZZ<F>)));
   CU(bk.partials.alloc(std::max((size_t)sh.vecs * sh.groups * nseg + 1024, bucket_tail_records(sh)) * sizeof(XYZZ<F>)));
   return B200_OK;
 }
@@ -351,7 +356,7 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   // (c < 7); nseg segments per window group.  c >= 7: the scratch of launch_bucket_tail.
   b->seg = sh.nbuckets >= 256 ? 4 : 1;
   b->nseg = (sh.nbuckets + b->seg - 1) / b->seg;
-  int rc_ = bucket_alloc<F>(b->bk, sh, b->sort, b->affine_S, b->nseg);
+  int rc_ = bucket_alloc<F>(b->bk, sh, b->sort.max_slices, b->affine_S, b->nseg);
   if (rc_) return rc_;
   CU(b->result.alloc(sizeof(XYZZ<F>)));
   CU(b->out_std.alloc(3 * sizeof(F)));
@@ -653,10 +658,12 @@ bool batch_fits(const Bases* b, size_t k, size_t n) {
 // the new capacity in each dimension when a batch exceeds it.  Before the old buffers are freed the host waits for the
 // set's last batch (its `done` event); batches on one set are ordered on one stream (b200snark.h), so nothing else of
 // this set can still read them, and work on other sets and prove contexts is not waited for.
+// with_sort = false (a proving-key set whose batches reuse another set's sort of the same scalars): bucket scratch
+// only, for that sort's slices; the shape is recorded in `sort.sh`, and nothing else of `sort` is allocated.
 template <class F>
-int batch_scratch(Bases* b, uint32_t k, uint32_t n) {
+int batch_scratch(Bases* b, uint32_t k, uint32_t n, bool with_sort = true) {
   if (n == 0) n = 1;
-  if (b->batch && b->batch->vecs >= k && b->batch->sort.sh.n >= n) return B200_OK;
+  if (b->batch && b->batch->vecs >= k && b->batch->sort.sh.n >= n && (!with_sort || b->batch->sort.entries.p)) return B200_OK;
   if (b->batch) {
     CU(cudaEventSynchronize(b->batch->done));
     const uint32_t k2 = std::max(k, b->batch->vecs), n2 = std::max(n, b->batch->sort.sh.n);
@@ -667,10 +674,14 @@ int batch_scratch(Bases* b, uint32_t k, uint32_t n) {
   MsmShape sh = b->sh;
   sh.n = n;
   sh.vecs = k;
-  int rc = sort_alloc(mb->sort, sh, b->affine_S);
-  if (rc) return rc;
-  if ((rc = bucket_alloc<F>(mb->bk, sh, mb->sort, b->affine_S, b->nseg))) return rc;
-  CU(mb->scan_totals.alloc(kScanBlocks * sizeof(unsigned long long)));
+  int rc;
+  if (with_sort) {
+    if ((rc = sort_alloc(mb->sort, sh, b->affine_S))) return rc;
+    CU(mb->scan_totals.alloc(kScanBlocks * sizeof(unsigned long long)));
+  } else {
+    mb->sort.sh = sh;
+  }
+  if ((rc = bucket_alloc<F>(mb->bk, sh, sort_max_slices(sh, b->affine_S), b->affine_S, b->nseg))) return rc;
   CU(cudaEventCreateWithFlags(&mb->done, cudaEventDisableTiming));
   mb->vecs = k;
   b->batch = std::move(mb);
@@ -840,6 +851,196 @@ int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t
   Fq* o = pk->out_std.as<Fq>();
   if ((rc = groth16_witness_enqueue(pk, r1, pk->w_stage.as<Fr>(), r, s, o, st, pk->d_err_sync.as<int>()))) return rc;
   return finish_host_proof(pk, o, "groth16_prove_witness", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
+}
+
+// ---- batches: k witness-fed proofs under one key (b200_groth16_prove_witness_batch) ---------------------------------
+// Proof p is the proof of groth16_witness_enqueue for (w_p, r_p, s_p).  The four MSMs run as batched MSMs over k scalar
+// vectors (W_p = w_p ++ [1, r_p, s_p] for A, B1, B2 with one shared sort; C||PTD_p), the h-direct quotients as one batched
+// front end (qap_h_batch_enqueue), the blinding products with one warp per proof: the launches of one proof, whatever k.
+
+// Everything that is refused before anything is allocated or enqueued.
+int groth16_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_t k, const uint64_t* r, const uint64_t* s,
+                        const char* what) {
+  if (k == 0) return fail(B200_EINVAL, "%s: k = 0", what);
+  if (nw != pk->m || nw != r1->m) return fail(B200_EINVAL, "%s: witness length %zu, NVars %zu, R1CS columns %zu", what, nw, pk->m, r1->m);
+  if (pk->world != 1) return fail(B200_EINVAL, "%s: sharded key (rank %d/%d): batches need an unsharded key", what, pk->rank, pk->world);
+  const size_t npx = 2 * r1->n - 1;
+  if (npx < pk->Z.nb) return fail(B200_EINVAL, "%s: len(px) < len(Z)", what);
+  if (npx - pk->Z.nb + 1 > pk->n_h_bases)
+    return fail(B200_EINVAL, "%s: len(hx)=%zu exceeds len(PowersTauDelta)=%zu", what, npx - pk->Z.nb + 1, pk->n_h_bases);
+  const size_t terms[4] = {pk->m + 3, pk->m + 3, pk->m + 3, pk->n_c_full + pk->n_h_bases + 1};
+  for (int j = 0; j < 4; j++)
+    if (!pk->g[j] || !batch_fits(pk->g[j].get(), k, terms[j]))
+      return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
+                  pk->g[j] ? pk->g[j]->sh.nwin : 0u, terms[j], j);
+  const uint64_t N = pow2_at_least(r1->n);
+  if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
+  // the scalar vectors are laid out by 2-D copies whose row pitch (one vector) the device bounds
+  int max_pitch = 0;
+  CU(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, g_device));
+  const uint64_t widest = std::max(terms[0], terms[3]) * sizeof(Fr);
+  if (widest > (uint64_t)max_pitch)
+    return fail(B200_EINVAL, "%s: a scalar vector of %llu bytes exceeds the device's copy pitch of %d bytes", what,
+                (unsigned long long)widest, max_pitch);
+  for (size_t p = 0; p < k; p++)
+    if (fr_load_std(r + 4 * p).geq_modulus() || fr_load_std(s + 4 * p).geq_modulus())
+      return fail(B200_ERANGE, "%s: r or s of proof %zu >= field order", what, p);
+  return B200_OK;
+}
+
+// d_w: k witnesses (device, standard form, witness p at d_w + p*m); r, s: host, k x 4 limbs; d_out: k x 48 u64, proof p at
+// d_out + 48p (PiA | PiC | PiB).  After groth16_batch_check.  No host synchronisation unless a scratch grows (or the
+// first batch on this R1CS and context builds its domains).
+int groth16_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const uint64_t* r, const uint64_t* s, Fq* d_out,
+                          cudaStream_t st, int* err) {
+  const size_t m = pk->m, l1 = pk->npublic + 1, n_c_full = pk->n_c_full, n_ptd = pk->n_h_bases;
+  const size_t mw = m + 3, nch = n_c_full + n_ptd + 1, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
+  const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as groth16_witness_enqueue
+  // host: {1, r_p, s_p, -r_p s_p} and the GLV splits of (s_p, r_p)
+  std::vector<Fr> small(4 * k);
+  std::vector<GlvScalars> glv(k);
+  Fr one = Fr::zero();
+  one.l[0] = 1;
+  for (size_t p = 0; p < k; p++) {
+    Fr fr_r = fr_load_std(r + 4 * p), fr_s = fr_load_std(s + 4 * p);
+    small[4 * p] = one;
+    small[4 * p + 1] = fr_r;
+    small[4 * p + 2] = fr_s;
+    small[4 * p + 3] = (fr_r.to_mont() * fr_s.to_mont()).neg().from_mont();
+    if (glv_decompose(fr_s, glv[p].k[0], glv[p].neg[0]) || glv_decompose(fr_r, glv[p].k[1], glv[p].neg[1]))
+      return fail(B200_EINVAL, "groth16_prove_witness_batch: GLV decomposition out of range");
+  }
+  // every scratch first: growing one waits for the batch that used it last, so nothing of this batch is enqueued yet
+  R1csWork* ws;
+  int rc = r1cs_work(r1, pk->ctx, &ws);
+  if (rc) return rc;
+  R1csBatch* fb = nullptr;
+  if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+  if ((rc = groth16_batch_scratch(pk, k, false))) return rc;
+  for (int j = 0; j < 3; j++) {
+    const bool own = pk->sort_src[j] == j;
+    rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, (uint32_t)mw, own) : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)mw, own);
+    if (rc) return rc;
+  }
+  if ((rc = batch_scratch<Fq>(pk->g[3].get(), (uint32_t)k, (uint32_t)nch))) return rc;
+  for (int j = 0; j < 3; j++) {   // a set that reuses another's sort was sized for the same slices (msm_buckets' check)
+    const Bases* a = pk->g[j].get();
+    const Bases* src = pk->g[pk->sort_src[j]].get();
+    if (a->sort.max_slices != src->sort.max_slices || a->affine_S != src->affine_S || a->batch->vecs != src->batch->vecs ||
+        a->batch->sort.sh.n != src->batch->sort.sh.n)
+      return fail(B200_EINVAL, "groth16_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, pk->sort_src[j]);
+  }
+  ProveBatch& b = *pk->batch;
+  cudaStream_t s1 = pk->pctx().side[0], s2 = pk->pctx().side[1], s3 = pk->pctx().side[2];
+  if (g_serial) s1 = s2 = s3 = st;   // measurement mode (b200_profile bit 1)
+  cudaEvent_t e_in = b.ev[0], e_sorted[3] = {b.ev[1], b.ev[2], b.ev[3]}, e_a = b.ev[4], e_b1 = b.ev[5], e_b2 = b.ev[6],
+              e_ch = b.ev[7], e_prod = b.ev[8];
+  Fr* W = b.W.as<Fr>();
+  Fr* CH = b.CH.as<Fr>();
+  Fr* rs = b.rs.as<Fr>();
+  XYZZ<Fq>* rA = b.rec.as<XYZZ<Fq>>();
+  XYZZ<Fq>* rB1 = rA + k;
+  XYZZ<Fq>* rCH = rB1 + k;
+  XYZZ<Fq>* prod = rCH + k;
+  XYZZ<Fq2>* rB2 = reinterpret_cast<XYZZ<Fq2>*>(prod + 2 * k);
+  const size_t F = sizeof(Fr);
+  CU(cudaMemcpyAsync(rs, small.data(), 4 * k * F, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(b.glv.p, glv.data(), k * sizeof(GlvScalars), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpy2DAsync(W, mw * F, d_w, m * F, m * F, k, cudaMemcpyDeviceToDevice, st));          // W_p = w_p ++
+  CU(cudaMemcpy2DAsync(W + m, mw * F, rs, 4 * F, 3 * F, k, cudaMemcpyDeviceToDevice, st));       //       [1, r_p, s_p]
+  if (n_c_full) CU(cudaMemcpy2DAsync(CH, nch * F, d_w + l1, m * F, n_c_full * F, k, cudaMemcpyDeviceToDevice, st));
+  EV_REC(e_in, st);
+  // --- side stream 3: the quotients into the C||PTD vectors, then the C||PTD MSMs
+  EV_WAIT(s3, e_in);
+  PolyCtx& pc = *pk->pctx().poly;
+  Fr* chq = CH + n_c_full;
+  const uint32_t qtotal = (uint32_t)(k * (n_ptd + 1));
+  if (h_direct) {
+    if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
+    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)n_ptd,
+                                                        rs + 3, 4, qtotal, chq, (uint32_t)nch);
+  } else {   // not batched: the single-witness px and division of each witness, straight into its vector
+    for (size_t p = 0; p < k; p++) {
+      if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
+      CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, chq + p * nch, nullptr, err, s3));
+    }
+    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)n_ptd, rs + 3, 4, qtotal, chq, (uint32_t)nch);
+  }
+  g_launches += 1;
+  Bases* gch = pk->g[3].get();
+  MsmShape sh = gch->sh;
+  sh.vecs = (uint32_t)k;
+  sh.vec_stride = (uint32_t)nch;
+  if ((rc = msm_sort(gch->batch->sort, sh, CH, nch, 0, err, s3, gch->batch->scan_totals.as<unsigned long long>()))) return rc;
+  if ((rc = bucket_phase<Fq>(gch, gch->batch->sort, gch->batch->bk, (uint32_t)k, nch, rCH, s3))) return rc;
+  EV_REC(e_ch, s3);
+  // --- A, B1, B2: one batched sort of W on the main stream, the bucket phases on st / s1 / s2 (B2 first: the longest)
+  for (int j = 0; j < 3; j++) {
+    if (pk->sort_src[j] != j) continue;
+    Bases* g = pk->g[j].get();
+    sh = g->sh;
+    sh.vecs = (uint32_t)k;
+    sh.vec_stride = (uint32_t)mw;
+    if ((rc = msm_sort(g->batch->sort, sh, W, mw, 0, err, st, g->batch->scan_totals.as<unsigned long long>()))) return rc;
+    EV_REC(e_sorted[j], st);
+  }
+  cudaStream_t sk[3] = {st, s1, s2};
+  for (int j = 2; j >= 0; j--) {
+    const int src = pk->sort_src[j];
+    const SortScratch& ss = pk->g[src]->batch->sort;
+    Bases* g = pk->g[j].get();
+    if (sk[j] != st) EV_WAIT(sk[j], e_sorted[src]);
+    if (j == 2) rc = bucket_phase<Fq2>(g, ss, g->batch->bk, (uint32_t)k, mw, rB2, sk[2]);
+    else rc = bucket_phase<Fq>(g, ss, g->batch->bk, (uint32_t)k, mw, j ? rB1 : rA, sk[j]);
+    if (rc) return rc;
+  }
+  EV_REC(e_a, st);
+  EV_REC(e_b1, s1);
+  EV_REC(e_b2, s2);
+  // s_p * A_p and r_p * B1_p on side stream 1, one warp per proof, while B2 / C||PTD still run
+  EV_WAIT(s1, e_a);
+  k_groth16_products_batch<<<(unsigned)k, 32, 0, s1>>>(rA, rB1, b.glv.as<GlvScalars>(), prod);
+  EV_REC(e_prod, s1);
+  EV_WAIT(st, e_prod);
+  EV_WAIT(st, e_b2);
+  EV_WAIT(st, e_ch);
+  k_groth16_combine_batch<<<nblk(3 * k, 96), 96, 0, st>>>(rA, rB2, rCH, prod, (uint32_t)k, d_out);
+  g_launches += 2;
+  CU(cudaGetLastError());
+  // behind everything of this batch: what the next regrowth of any of its scratches waits for
+  EV_REC(b.done, st);
+  for (const auto& g : pk->g)
+    if (g && g->batch) EV_REC(g->batch->done, st);
+  if (fb) EV_REC(fb->done, st);
+  return B200_OK;
+}
+
+int groth16_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, size_t k, const uint64_t* r,
+                                const uint64_t* s, uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c, std::unique_lock<std::mutex>* lk) {
+  const char* what = "groth16_prove_witness_batch";
+  ProvingKey* pk = find_pk(h, 1);
+  R1cs* r1 = find_r1cs(hr);
+  if (!pk || !r1) return fail(B200_EINVAL, "%s: bad handle", what);
+  if (!w || !r || !s || !pi_a || !pi_b || !pi_c) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = groth16_batch_check(pk, r1, nw, k, r, s, what);
+  if (rc) return rc;
+  if ((rc = groth16_batch_scratch(pk, k, true))) return rc;
+  ProveBatch& b = *pk->batch;
+  cudaStream_t st = pk->pctx().main;
+  CU(cudaMemcpyAsync(b.w_stage.p, w, k * nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  Fq* o = b.out.as<Fq>();
+  if ((rc = groth16_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, r, s, o, st, pk->d_err_sync.as<int>()))) return rc;
+  // as finish_host_proof, for k proofs: the wait runs with the library mutex released
+  CU(cudaMemcpyAsync(b.h_out, o, k * kBatchProofWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(b.h_out + k * kBatchProofWords));
+  if (rc) return rc;
+  for (size_t p = 0; p < k; p++) {
+    const uint64_t* q = b.h_out + kBatchProofWords * p;
+    memcpy(pi_a + 12 * p, q, 12 * sizeof(uint64_t));
+    memcpy(pi_c + 12 * p, q + 12, 12 * sizeof(uint64_t));
+    memcpy(pi_b + 24 * p, q + 24, 24 * sizeof(uint64_t));
+  }
+  return B200_OK;
 }
 
 // ---- dense QAP API (small n) -------------------------------------------------
@@ -1471,6 +1672,25 @@ int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void
     return fail(B200_EINVAL, "groth16_prove_witness_device: witness length %zu, NVars %zu, R1CS columns %zu", nw, p->m, r1->m);
   return drain_on_error(groth16_witness_enqueue(p, r1, (const Fr*)d_w, r, s, (Fq*)d_out,
                                                 stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_groth16_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, size_t k, const uint64_t* r,
+                                     const uint64_t* s, uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c) {
+  std::unique_lock<std::mutex> lk(g_mu);
+  NEED_INIT();
+  return drain_on_error(groth16_prove_witness_batch(pk, r1cs, w, nw, k, r, s, pi_a, pi_b, pi_c, &lk));
+}
+int b200_groth16_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                            const uint64_t* r, const uint64_t* s, void* d_out, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  const char* what = "groth16_prove_witness_batch_device";
+  ProvingKey* p = find_pk(pk, 1);
+  R1cs* r1 = find_r1cs(r1cs);
+  if (!p || !r1 || !d_w || !r || !s || !d_out) return fail(B200_EINVAL, "%s: bad arguments", what);
+  int rc = groth16_batch_check(p, r1, nw, k, r, s, what);
+  if (rc) return rc;
+  return drain_on_error(groth16_batch_enqueue(p, r1, (const Fr*)d_w, k, r, s, (Fq*)d_out,
+                                              stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
 }
 int b200_fq12_mul_batch(const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) { B200_API_BODY(fq12_mul_batch_host(a, b, n, out)) }
 int b200_pairing_batch(const uint64_t* g1_jac, const uint64_t* g2_jac, size_t n, uint64_t* out) { B200_API_BODY(pairing_batch_host(g1_jac, g2_jac, n, out)) }

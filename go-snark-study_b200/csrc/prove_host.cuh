@@ -24,6 +24,31 @@
 // (caller's + 3 side streams): the latency-bound tails (bucket reduction, tree sum) of
 // one MSM overlap the throughput-bound accumulation of the others.
 
+// A key's scratch for batches of up to k proofs (b200_groth16_prove_witness_batch): allocated on the first batch, grown
+// (never shrunk) by a larger one after waiting for `done`, which is recorded behind the key's last batch.
+struct ProveBatch {
+  size_t k = 0;
+  DevBuf W;          // k scalar vectors w_p ++ [1, r_p, s_p] of A, B1, B2 (stride m + 3)
+  DevBuf CH;         // k scalar vectors of C||PTD: w_p[l+1..m) ++ h_p ++ 0.. ++ [-r_p s_p]
+  DevBuf rec;        // k records per set: A, B1 (G1), B2 (G2), CH (G1), then 2k products (G1)
+  DevBuf rs;         // per proof {1, r_p, s_p, -r_p s_p}, standard form
+  DevBuf glv;        // per proof GlvScalars of (s_p, r_p)
+  DevBuf w_stage;    // the host entry's witnesses
+  DevBuf out;        // the host entry's k proofs (48 u64 each)
+  uint64_t* h_out = nullptr;   // pinned landing area of the host entry: k * 48 words + the error word
+  cudaEvent_t ev[9] = {};
+  cudaEvent_t done = nullptr;
+  ProveBatch() = default;
+  ProveBatch(const ProveBatch&) = delete;
+  ProveBatch& operator=(const ProveBatch&) = delete;
+  ~ProveBatch() {
+    for (auto e : ev) if (e) cudaEventDestroy(e);
+    if (done) cudaEventDestroy(done);
+    if (h_out) cudaFreeHost(h_out);
+  }
+};
+constexpr size_t kBatchProofWords = 48;
+
 struct ProvingKey {
   int kind = 0;  // 1 Groth16, 2 Pinocchio
   size_t m = 0, npublic = 0, n_h_bases = 0;
@@ -64,6 +89,7 @@ struct ProvingKey {
   // the key's main stream.  Its own word, because those calls wait with the library mutex released: a word shared with
   // a proof on another key would report one proof's error to the other.
   DevBuf d_err_sync;
+  std::unique_ptr<ProveBatch> batch;   // b200_groth16_prove_witness_batch scratch (null until the first batch)
 };
 
 size_t pk_device_bytes(const ProvingKey& pk) {
@@ -71,6 +97,8 @@ size_t pk_device_bytes(const ProvingKey& pk) {
                         &pk.w_stage, &pk.res, &pk.out_std, &pk.rs, &pk.d_err, &pk.d_err_sync});
   for (const auto& g : pk.g)
     if (g) s += bases_device_bytes(*g);
+  if (const ProveBatch* b = pk.batch.get())
+    s += dev_bytes({&b->W, &b->CH, &b->rec, &b->rs, &b->glv, &b->w_stage, &b->out});
   return s;
 }
 
@@ -262,6 +290,37 @@ ProvingKey* find_pk(b200_pk_t h, int kind) {
   return it->second.get();
 }
 
+// Grows the key's batch scratch to k proofs (host: also the host entry's witness staging, proof buffer and pinned landing
+// area).  A regrowth first waits for the key's last batch (its `done` event), not for the device.
+int groth16_batch_scratch(ProvingKey* pk, size_t k, bool host) {
+  if (!pk->batch) {
+    auto b = std::make_unique<ProveBatch>();
+    for (auto& e : b->ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
+    pk->batch = std::move(b);
+  }
+  ProveBatch& b = *pk->batch;
+  const size_t m = pk->m, nch = pk->n_c_full + pk->n_h_bases + 1;
+  const bool grow_host = host && b.out.bytes < k * kBatchProofWords * sizeof(uint64_t);
+  if (b.k < k || grow_host) CU(cudaEventSynchronize(b.done));
+  if (b.k < k) {
+    CU(b.W.alloc(k * (m + 3) * sizeof(Fr)));
+    CU(b.CH.alloc(k * nch * sizeof(Fr)));
+    CU(b.rec.alloc(k * (5 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>))));
+    CU(b.rs.alloc(k * 4 * sizeof(Fr)));
+    CU(b.glv.alloc(k * sizeof(GlvScalars)));
+    b.k = k;
+  }
+  if (grow_host) {
+    CU(b.w_stage.alloc(k * m * sizeof(Fr)));
+    CU(b.out.alloc(k * kBatchProofWords * sizeof(uint64_t)));
+    if (b.h_out) CU(cudaFreeHost(b.h_out));
+    b.h_out = nullptr;
+    CU(cudaHostAlloc(reinterpret_cast<void**>(&b.h_out), (k * kBatchProofWords + 1) * sizeof(uint64_t), cudaHostAllocDefault));
+  }
+  return B200_OK;
+}
+
 // host F_r helpers for the blinding scalars (the reference does this with big.Int, groth16.go:274)
 Fr fr_load_std(const uint64_t* v) {
   Fr r;
@@ -288,6 +347,36 @@ __global__ void k_groth16_combine(const uint8_t* res, const XYZZ<Fq>* prod, Fq* 
   }
   if (t == 32) store_jacobian_std(*reinterpret_cast<const XYZZ<Fq>*>(res), out_a);
   if (t == 64) store_jacobian_std(*reinterpret_cast<const XYZZ<Fq2>*>(res + 512), out_b);
+}
+
+// ---- batches of k proofs under one key (b200_groth16_prove_witness_batch) ----------------------------------------------
+// The batched MSMs leave k records per set: rA[p], rB1[p], rB2[p], rCH[p].  Block p: the warp of k_groth16_products for
+// proof p, prod[2p] = s_p * A_p and prod[2p+1] = r_p * B1_p.
+__global__ void k_groth16_products_batch(const XYZZ<Fq>* rA, const XYZZ<Fq>* rB1, const GlvScalars* g, XYZZ<Fq>* prod) {
+  const uint32_t t = threadIdx.x & 31u, p = blockIdx.x;
+  const uint32_t grp = t >> 4;
+  Jacobian<Fq> pt = xyzz_to_jacobian(grp ? rB1[p] : rA[p]);
+  Jacobian<Fq> r = glv_mul_halfwarp(pt, g[p].k[grp], g[p].neg[grp], t);
+  if ((t & 15u) == 0) prod[2 * p + grp] = jacobian_to_xyzz(r);
+}
+// Thread 3p + j of k proofs: j = 0 PiC_p = CH_p + prod[2p] + prod[2p+1], j = 1 PiA_p, j = 2 PiB_p; proof p at out + 48p
+// (u64), PiA | PiC | PiB as in k_groth16_combine.
+__global__ void k_groth16_combine_batch(const XYZZ<Fq>* rA, const XYZZ<Fq2>* rB2, const XYZZ<Fq>* rCH, const XYZZ<Fq>* prod,
+                                        uint32_t k, Fq* out) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= 3 * k) return;
+  const uint32_t p = e / 3, j = e - 3 * p;
+  Fq* o = out + 12 * (size_t)p;   // 48 u64 = 12 Fq per proof
+  if (j == 0) {
+    XYZZ<Fq> c = rCH[p];
+    xyzz_add(c, prod[2 * p]);
+    xyzz_add(c, prod[2 * p + 1]);
+    store_jacobian_std(c, o + 3);
+  } else if (j == 1) {
+    store_jacobian_std(rA[p], o);
+  } else {
+    store_jacobian_std(rB2[p], reinterpret_cast<Fq2*>(o + 6));
+  }
 }
 
 

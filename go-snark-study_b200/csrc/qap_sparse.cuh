@@ -127,12 +127,63 @@ __global__ void k_spmv_csr(const uint32_t* __restrict__ rowptr, const uint32_t* 
   for (uint32_t k = rowptr[j], e = rowptr[j + 1]; k < e; k++) acc = acc + val[k] * w[col[k]];
   out[j] = acc;
 }
-// u[j] = v[j] / j! for j < n, zero up to n_pad
-__global__ void k_newton_scale(const Fr* __restrict__ v, const Fr* __restrict__ invfact, uint32_t n, uint32_t n_pad,
-                               Fr* __restrict__ u) {
-  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n_pad) return;
-  u[j] = j < n ? v[j] * invfact[j] : Fr::zero();
+// k witnesses (w_p at w + p*m, standard form) -> wt[i*k + p] (Montgomery): signal-major, so the sparse product reads
+// each non-zero's col / val once for all k.  An entry >= r is read as 0 and sets bit 1 of *err.
+__global__ void k_witness_load_batch(const Fr* __restrict__ w, uint32_t m, uint32_t k, Fr* __restrict__ wt, int* err) {
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= m * k) return;
+  uint32_t i = e / k, p = e - i * k;
+  Fr v = w[(size_t)p * m + i];
+  if (v.geq_modulus()) {
+    atomicOr(err, 2);
+    v = Fr::zero();
+  }
+  wt[e] = v.to_mont();
+}
+// Rows of A and B times k witnesses (wt: [m][k], Montgomery).  Thread (row j, tile of kSpmmTile witnesses) gathers
+// 32 * kSpmmTile contiguous bytes per non-zero and writes, for witness p, (A w_p)_j | (B w_p)_j | their product to blocks
+// 3p, 3p+1, 3p+2 of out (n-strided): the layout the quotient path takes (qap_h_batch).
+constexpr uint32_t kSpmmTile = 4;
+__device__ __forceinline__ void spmm_row(const uint32_t* __restrict__ rowptr, const uint32_t* __restrict__ col,
+                                         const Fr* __restrict__ val, const Fr* __restrict__ wt, uint32_t j, uint32_t k,
+                                         uint32_t p0, uint32_t cnt, Fr (&acc)[kSpmmTile]) {
+#pragma unroll
+  for (uint32_t t = 0; t < kSpmmTile; t++) acc[t] = Fr::zero();
+  for (uint32_t x = rowptr[j], e = rowptr[j + 1]; x < e; x++) {
+    const Fr v = val[x];
+    const Fr* src = wt + (size_t)col[x] * k + p0;
+#pragma unroll
+    for (uint32_t t = 0; t < kSpmmTile; t++)
+      if (t < cnt) acc[t] = acc[t] + v * src[t];
+  }
+}
+__global__ void k_spmm_ab(const uint32_t* __restrict__ arow, const uint32_t* __restrict__ acol, const Fr* __restrict__ aval,
+                          const uint32_t* __restrict__ brow, const uint32_t* __restrict__ bcol, const Fr* __restrict__ bval,
+                          const Fr* __restrict__ wt, uint32_t n, uint32_t k, Fr* __restrict__ out) {
+  const uint32_t tiles = (k + kSpmmTile - 1) / kSpmmTile;
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n * tiles) return;
+  const uint32_t j = e / tiles, p0 = (e - j * tiles) * kSpmmTile;
+  const uint32_t cnt = k - p0 < kSpmmTile ? k - p0 : kSpmmTile;
+  Fr a[kSpmmTile], b[kSpmmTile];
+  spmm_row(arow, acol, aval, wt, j, k, p0, cnt, a);
+  spmm_row(brow, bcol, bval, wt, j, k, p0, cnt, b);
+#pragma unroll
+  for (uint32_t t = 0; t < kSpmmTile; t++)
+    if (t < cnt) {
+      Fr* o = out + (size_t)3 * (p0 + t) * n + j;
+      o[0] = a[t];
+      o[n] = b[t];
+      o[2 * (size_t)n] = a[t] * b[t];
+    }
+}
+// u[q*n_pad + j] = v[q*vstride + j] / j! for j < n, zero up to n_pad; total = polys * n_pad
+__global__ void k_newton_scale(const Fr* __restrict__ v, uint32_t vstride, const Fr* __restrict__ invfact, uint32_t n,
+                               uint32_t n_pad, uint32_t total, Fr* __restrict__ u) {
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  uint32_t q = e / n_pad, j = e - q * n_pad;
+  u[e] = j < n ? v[(size_t)q * vstride + j] * invfact[j] : Fr::zero();
 }
 // e[k] = (-1)^k / k! for k < n, zero up to n_pad
 __global__ void k_exp_neg(const Fr* __restrict__ invfact, uint32_t n, uint32_t n_pad, Fr* __restrict__ e) {
@@ -145,6 +196,30 @@ __global__ void k_take(const Fr* __restrict__ src, uint32_t n, uint32_t N, Fr* _
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k < N) d[k] = k < n ? src[k] : Fr::zero();
 }
+// k_take on every block: d[q*N + i] = src[q*sstride + i] for i < n else 0; total = blocks * N
+__global__ void k_take_blocks(const Fr* __restrict__ src, uint32_t sstride, uint32_t n, uint32_t N, uint32_t total,
+                              Fr* __restrict__ d) {
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  uint32_t q = e / N, i = e - q * N;
+  d[e] = i < n ? src[(size_t)q * sstride + i] : Fr::zero();
+}
+// C||PTD scalar vector p (ch + p*stride, from the quotient's offset): the quotient h_p below nh (coef: blocks of cstride,
+// Montgomery -> standard form; null: already in place), zeros up to n_ptd, then tail[p*tstride] (-r_p s_p, standard form).
+// total = k * (n_ptd + 1)
+__global__ void k_quotient_store(const Fr* __restrict__ coef, uint32_t cstride, uint32_t nh, uint32_t n_ptd,
+                                 const Fr* __restrict__ tail, uint32_t tstride, uint32_t total, Fr* __restrict__ ch,
+                                 uint32_t stride) {
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  uint32_t p = e / (n_ptd + 1), i = e - p * (n_ptd + 1);
+  Fr* d = ch + (size_t)p * stride + i;
+  if (i < nh) {
+    if (coef) *d = coef[(size_t)p * cstride + i].from_mont();
+  } else {
+    *d = i < n_ptd ? Fr::zero() : tail[(size_t)p * tstride];
+  }
+}
 // leaves of the subproduct tree over the points offset+1 .. offset+N: t[k] = -(offset + k + 1)
 __global__ void k_tree_leaves(Fr* t, uint32_t N, uint32_t offset) {
   uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -156,12 +231,17 @@ __global__ void k_tree_leaves(Fr* t, uint32_t N, uint32_t offset) {
 // f[j] = j!  (from the inverse factorials: one inversion per element is avoided by the caller's host table)
 // hv[j] = (Va[Y] * Vb[Y] * Y! - Vc[Y]) * j!   with Y = n + j,  j < n - 1   — the quotient h = (a b - c) / Z at x = Y + 1
 // (a(x) = Va[Y] * Y!, Z(x) = Y! / j!); V* are the three cyclic convolutions d * (1/i!) laid out with stride M.
-__global__ void k_h_values(const Fr* __restrict__ V, uint32_t M, const Fr* __restrict__ fact, uint32_t n, Fr* __restrict__ hv) {
-  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+// Quotient q of a batch (total = quotients * n): its three convolutions at V + 3qM, its values at hv + q*n.
+__global__ void k_h_values(const Fr* __restrict__ V, uint32_t M, const Fr* __restrict__ fact, uint32_t n, uint32_t total,
+                           Fr* __restrict__ hv) {
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  uint32_t q = e / n, j = e - q * n;
   if (j + 1 >= n) return;
   uint32_t Y = n + j;
-  Fr va = V[Y], vb = V[(size_t)M + Y], vc = V[2 * (size_t)M + Y];
-  hv[j] = (va * vb * fact[Y] - vc) * fact[j];
+  const Fr* Vq = V + (size_t)3 * q * M;
+  Fr va = Vq[Y], vb = Vq[(size_t)M + Y], vc = Vq[2 * (size_t)M + Y];
+  hv[e] = (va * vb * fact[Y] - vc) * fact[j];
 }
 // c[j] = a[j] * b[j], j < n: the values the quotient path uses in place of (C w)_j (qap_h_from_values)
 __global__ void k_row_products(const Fr* __restrict__ a, const Fr* __restrict__ b, uint32_t n, Fr* __restrict__ c) {
@@ -380,7 +460,6 @@ inline cudaError_t newton_coeffs(PolyCtx& pc, const QapDomain& dom, QapWork& wk,
   const int l2 = dom.logN + 1;
   PCU(wk.U.ensure(polys * N2 * sizeof(Fr)));
   PCU(wk.E.ensure(N2 * sizeof(Fr)));
-  PCU(wk.X.ensure(polys * N * sizeof(Fr)));
   Fr* U = wk.U.as<Fr>();
   Fr* E = wk.E.as<Fr>();
   NttPlan* pl;
@@ -392,19 +471,21 @@ inline cudaError_t newton_coeffs(PolyCtx& pc, const QapDomain& dom, QapWork& wk,
     wk.n_e = n;
     wk.N_e = N;
   }
-  for (int q = 0; q < polys; q++)
-    B200_LAUNCH(k_newton_scale, nblk(N2, 256), 256, st, v + q * stride, dom.invfact.as<Fr>(), (uint32_t)n, (uint32_t)N2, U + q * N2);
+  // one launch per step for all polys: a batch of proofs issues the launches of one
+  B200_LAUNCH(k_newton_scale, nblk(polys * N2, 256), 256, st, v, (uint32_t)stride, dom.invfact.as<Fr>(), (uint32_t)n, (uint32_t)N2,
+              (uint32_t)(polys * N2), U);
   PCU(ntt_batched(pc, U, l2, polys * N2, 0, st));
   B200_LAUNCH(k_dc_pointwise, nblk(polys * N2, 256), 256, st, U, E, (uint32_t)N2, (uint32_t)(polys * N2));
   PCU(ntt_batched(pc, U, l2, polys * N2, 1, st));
-  for (int q = 0; q < polys; q++)
-    B200_LAUNCH(k_take, nblk(N, 256), 256, st, U + q * N2, (uint32_t)n, (uint32_t)N, out + q * N);   // d mod x^n, padded to N
-  pc.note(2 * polys + 2);
+  B200_LAUNCH(k_take_blocks, nblk(polys * N, 256), 256, st, U, (uint32_t)N2, (uint32_t)n, (uint32_t)N, (uint32_t)(polys * N),
+              out);   // d mod x^n, padded to N
+  pc.note(3);
   return cudaGetLastError();
 }
 inline cudaError_t interpolate_ap(PolyCtx& pc, const QapDomain& dom, QapWork& wk, const Fr* v, size_t stride, size_t n,
                                   int polys, Fr* out, cudaStream_t st) {
   PCU(newton_coeffs(pc, dom, wk, v, stride, n, polys, out, st));
+  PCU(wk.X.ensure(polys * dom.N * sizeof(Fr)));   // only the divide and conquer needs X
   return newton_to_monomial(pc, dom, out, wk.X.as<Fr>(), polys, st);
 }
 
@@ -448,26 +529,29 @@ inline cudaError_t qap_hdomain_build(PolyCtx& pc, QapHDomain& hd, size_t n, cuda
   PCU(cudaStreamSynchronize(st));
   return cudaGetLastError();
 }
-// d: Newton coefficients of a | b | c over {1..n} (3 blocks of `dstride`, from newton_coeffs on the QAP domain);
-// h_out: n - 1 coefficients of h (Montgomery) in ws->coef (ws = null: the domain's own scratch).
+// d: Newton coefficients of a | b | c over {1..n} (3 blocks of `dstride` per quotient, from newton_coeffs on the QAP
+// domain); h_out: n - 1 coefficients of each quotient q (Montgomery) in ws->coef + q * tree.N (ws = null: the domain's own
+// scratch).  One launch per step for all `quotients`.
 inline cudaError_t qap_h_from_newton(PolyCtx& pc, QapHDomain& hd, const Fr* d, size_t dstride, cudaStream_t st,
-                                     QapHWork* ws = nullptr) {
+                                     QapHWork* ws = nullptr, int quotients = 1) {
   QapHWork& w = ws ? *ws : hd;
-  const size_t n = hd.n, M = hd.M;
+  const size_t n = hd.n, M = hd.M, nv = 3 * (size_t)quotients;
   const int lm = ceil_log2(M);
-  PCU(w.V.ensure(3 * M * sizeof(Fr)));
-  PCU(w.hv.ensure(n * sizeof(Fr)));
-  PCU(w.coef.ensure(hd.tree.N * sizeof(Fr)));
+  PCU(w.V.ensure(nv * M * sizeof(Fr)));
+  PCU(w.hv.ensure(quotients * n * sizeof(Fr)));
+  PCU(w.coef.ensure(quotients * hd.tree.N * sizeof(Fr)));
   Fr* V = w.V.as<Fr>();
-  for (int q = 0; q < 3; q++) B200_LAUNCH(k_take, nblk(M, 256), 256, st, d + q * dstride, (uint32_t)n, (uint32_t)M, V + q * M);
-  PCU(ntt_batched(pc, V, lm, 3 * M, 0, st));
-  B200_LAUNCH(k_dc_pointwise, nblk(3 * M, 256), 256, st, V, hd.G.as<Fr>(), (uint32_t)M, (uint32_t)(3 * M));
-  PCU(ntt_batched(pc, V, lm, 3 * M, 1, st));
+  B200_LAUNCH(k_take_blocks, nblk(nv * M, 256), 256, st, d, (uint32_t)dstride, (uint32_t)n, (uint32_t)M, (uint32_t)(nv * M), V);
+  PCU(ntt_batched(pc, V, lm, nv * M, 0, st));
+  B200_LAUNCH(k_dc_pointwise, nblk(nv * M, 256), 256, st, V, hd.G.as<Fr>(), (uint32_t)M, (uint32_t)(nv * M));
+  PCU(ntt_batched(pc, V, lm, nv * M, 1, st));
+  pc.note(2);
   if (n >= 2) {
-    B200_LAUNCH(k_h_values, nblk(n - 1, 256), 256, st, V, (uint32_t)M, hd.tree.fact.as<Fr>(), (uint32_t)n, w.hv.as<Fr>());
-    PCU(interpolate_ap(pc, hd.tree, w.work, w.hv.as<Fr>(), n - 1, n - 1, 1, w.coef.as<Fr>(), st));
+    B200_LAUNCH(k_h_values, nblk(quotients * n, 256), 256, st, V, (uint32_t)M, hd.tree.fact.as<Fr>(), (uint32_t)n,
+                (uint32_t)(quotients * n), w.hv.as<Fr>());
+    pc.note(1);
+    PCU(interpolate_ap(pc, hd.tree, w.work, w.hv.as<Fr>(), n, n - 1, quotients, w.coef.as<Fr>(), st));
   }
-  pc.note(8);
   return cudaGetLastError();
 }
 // vals: the values of a | b on {1..n} in blocks 0 and 1 (n-strided, Montgomery); block 2 is overwritten with the products
@@ -480,12 +564,28 @@ inline cudaError_t qap_h_from_values(PolyCtx& pc, const QapDomain& dom, QapWork&
   PCU(newton_coeffs(pc, dom, wk, vals, n, n, 3, d, st));
   return qap_h_from_newton(pc, hd, d, dom.N, st, ws);
 }
+// k quotients at once: vals holds A w_p | B w_p | their products in blocks 3p, 3p+1, 3p+2 (n-strided, Montgomery: what
+// k_spmm_ab writes); d: 3k blocks of dom.N.  Quotient p lands in ws->coef + p * hd.tree.N: the field elements
+// qap_h_from_values gives for witness p, in launches that do not depend on k.
+inline cudaError_t qap_h_batch(PolyCtx& pc, const QapDomain& dom, QapWork& wk, QapHDomain& hd, const Fr* vals, Fr* d, int k,
+                               cudaStream_t st, QapHWork* ws) {
+  PCU(newton_coeffs(pc, dom, wk, vals, hd.n, hd.n, 3 * k, d, st));
+  return qap_h_from_newton(pc, hd, d, dom.N, st, ws, k);
+}
 
 // ---- a sparse R1CS resident on the device ------------------------------------------------------------------
 struct SparseMat {
   DevBuf rowptr, col, val;      // CSR (n rows)
   DevBuf cptr, crow, cval;      // CSC = CSR of the transpose (m rows): the trusted setup's A^T l(tau)
   size_t nnz = 0;
+};
+// Witnesses -> quotients scratch of a batch of k proofs (qap_h_batch), sized for `k` witnesses: grown, never shrunk.
+struct R1csBatchWork {
+  size_t k = 0;
+  DevBuf wt, vals, coef;            // witnesses [m][k]; A w_p | B w_p | products (3k x n); Newton coefficients (3k x N)
+  QapWork work;
+  QapHWork hw;
+  virtual ~R1csBatchWork() = default;
 };
 // Witness -> px / h scratch of one proof in flight on an R1CS: one per prove context, so proofs on keys of the two
 // contexts may share the R1CS and overlap.
@@ -496,6 +596,7 @@ struct R1csWork {
   DevBuf h_std;                     // h = px / Z, n - 1 coefficients, standard form (h-direct branch)
   QapWork work;
   QapHWork hw;
+  std::unique_ptr<R1csBatchWork> batch;   // batches of witnesses (allocated on the first batch)
 };
 struct R1cs {
   size_t n = 0, m = 0;

@@ -144,21 +144,28 @@ int qap_px_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, Fr* d_
   return B200_OK;
 }
 
+// The h-direct domains of r (the QAP domain and QapHDomain), built on g_ctx[0].main and waited for on first use.
+int r1cs_hdomain(R1cs* r, QapDomain** dom) {
+  int rc = get_domain(pow2_at_least(r->n), dom);
+  if (rc) return rc;
+  if (!r->hd) {
+    auto hd = std::make_unique<QapHDomain>();
+    CU(qap_hdomain_build(*g_ctx[0].poly, *hd, r->n, g_ctx[0].main));   // synchronises g_ctx[0].main
+    r->hd = std::move(hd);
+  }
+  return B200_OK;
+}
+
 // d_w: m witness values (device, standard form; an entry >= r is read as 0 and sets bit 1 of *err) -> the n - 1
 // coefficients of h = DivisorPolynomial(ax*bx - cx, Z) in ws.h_std (standard form), without forming px (qap_sparse.cuh:
 // QapHDomain).  The quotient does not depend on cx, so C w is not computed.  Requires n >= 2.  The domains are shared by
 // every context: built on g_ctx[0].main and waited for on the first call.
 int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
-  const size_t n = r->n, m = r->m, N = pow2_at_least(n);
+  const size_t n = r->n, m = r->m;
   if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
   QapDomain* dom;
-  int rc = get_domain(N, &dom);
+  int rc = r1cs_hdomain(r, &dom);
   if (rc) return rc;
-  if (!r->hd) {
-    auto hd = std::make_unique<QapHDomain>();
-    CU(qap_hdomain_build(*g_ctx[0].poly, *hd, n, g_ctx[0].main));   // synchronises g_ctx[0].main
-    r->hd = std::move(hd);
-  }
   Fr* w = ws.w_mont.as<Fr>();
   k_poly_load<<<nblk(m, 256), 256, 0, st>>>(d_w_std, (uint32_t)m, (uint32_t)m, 0, 0, w, (uint32_t)m, err);
   Fr* vals = ws.vals.as<Fr>();
@@ -170,6 +177,63 @@ int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* er
   CU(qap_h_from_values(pc, *dom, ws.work, *r->hd, vals, coef, st, &ws.hw));
   k_poly_store<<<nblk(n - 1, 256), 256, 0, st>>>(ws.hw.coef.as<Fr>(), (uint32_t)(n - 1), 0, 1, ws.h_std.as<Fr>());
   g_launches += 1;
+  CU(cudaGetLastError());
+  return B200_OK;
+}
+
+// The batch scratch of a prove context's workspace; `done` is recorded behind the last batch that used it.
+struct R1csBatch : R1csBatchWork {
+  cudaEvent_t done = nullptr;
+  ~R1csBatch() override { if (done) cudaEventDestroy(done); }
+};
+
+// Before a batch of k witnesses on the h-direct branch: builds the domains (first use) and grows the workspace's batch
+// scratch to k witnesses, every buffer the batch touches included, so that enqueueing it allocates nothing.  A regrowth
+// first waits for the last batch that used the scratch, not for the device.
+int qap_batch_prepare(R1cs* r, R1csWork& ws, size_t k, R1csBatch** out) {
+  QapDomain* dom;
+  int rc = r1cs_hdomain(r, &dom);
+  if (rc) return rc;
+  if (!ws.batch) {
+    auto b = std::make_unique<R1csBatch>();
+    CU(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
+    ws.batch = std::move(b);
+  }
+  auto* b = static_cast<R1csBatch*>(ws.batch.get());
+  if (b->k < k) {
+    CU(cudaEventSynchronize(b->done));
+    const size_t n = r->n, m = r->m, N = dom->N, M = r->hd->M, Nt = r->hd->tree.N, F = sizeof(Fr);
+    CU(b->wt.alloc(m * k * F));
+    CU(b->vals.alloc(3 * k * n * F));
+    CU(b->coef.alloc(3 * k * N * F));
+    CU(b->work.U.alloc(3 * k * 2 * N * F));
+    CU(b->hw.V.alloc(3 * k * M * F));
+    CU(b->hw.hv.alloc(k * n * F));
+    CU(b->hw.coef.alloc(k * Nt * F));
+    CU(b->hw.work.U.alloc(k * 2 * Nt * F));
+    CU(b->hw.work.X.alloc(k * Nt * F));
+    b->k = k;
+  }
+  CU(b->work.E.ensure(2 * dom->N * sizeof(Fr)));   // the cached e^-x series: allocated once
+  CU(b->hw.work.E.ensure(2 * r->hd->tree.N * sizeof(Fr)));
+  *out = b;
+  return B200_OK;
+}
+
+// d_w: k witnesses of m standard-form scalars (witness p at d_w + p*m; an entry >= r is read as 0 and sets bit 1 of
+// *err) -> quotient p (n - 1 coefficients, Montgomery) at b.hw.coef + p * tree.N.  After qap_batch_prepare for >= k.
+int qap_h_batch_enqueue(R1cs* r, R1csBatch& b, PolyCtx& pc, const Fr* d_w, size_t k, int* err, cudaStream_t st) {
+  const size_t n = r->n, m = r->m;
+  QapDomain* dom;
+  int rc = get_domain(pow2_at_least(n), &dom);
+  if (rc) return rc;
+  k_witness_load_batch<<<nblk(m * k, 256), 256, 0, st>>>(d_w, (uint32_t)m, (uint32_t)k, b.wt.as<Fr>(), err);
+  const size_t tiles = (k + kSpmmTile - 1) / kSpmmTile;
+  k_spmm_ab<<<nblk(n * tiles, 128), 128, 0, st>>>(r->M[0].rowptr.as<uint32_t>(), r->M[0].col.as<uint32_t>(), r->M[0].val.as<Fr>(),
+                                                  r->M[1].rowptr.as<uint32_t>(), r->M[1].col.as<uint32_t>(), r->M[1].val.as<Fr>(),
+                                                  b.wt.as<Fr>(), (uint32_t)n, (uint32_t)k, b.vals.as<Fr>());
+  g_launches += 2;
+  CU(qap_h_batch(pc, *dom, b.work, *r->hd, b.vals.as<Fr>(), b.coef.as<Fr>(), (int)k, st, &b.hw));
   CU(cudaGetLastError());
   return B200_OK;
 }

@@ -85,6 +85,23 @@ class DeviceProvingKey:
                                                ptr(pa), ptr(pb), ptr(pc)))
         return {"PiA": _unflatten_g1(pa)[0], "PiB": _unflatten_g2(pb)[0], "PiC": _unflatten_g1(pc)[0]}
 
+    def prove_witness_batch_limbs(self, r1cs, w_limbs, rs):
+        """k proofs in one call (b200_groth16_prove_witness_batch): ``w_limbs`` holds k witnesses (k x m x 4 limbs, or
+        k*m x 4), ``rs`` a list of k (r, s) pairs.  Proof p is prove_witness_limbs(r1cs, w_limbs[p], *rs[p])."""
+        k = len(rs)
+        w = np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
+        if k == 0 or w.shape[0] % k:
+            raise ValueError("prove_witness_batch_limbs: need k >= 1 witnesses of equal length")
+        rr = ints_to_limbs([r for r, _ in rs])
+        ss = ints_to_limbs([s for _, s in rs])
+        pa = np.zeros(12 * k, dtype=np.uint64)
+        pb = np.zeros(24 * k, dtype=np.uint64)
+        pc = np.zeros(12 * k, dtype=np.uint64)
+        check(lib().b200_groth16_prove_witness_batch(self.handle, r1cs.handle, ptr(w), w.shape[0] // k, k, ptr(rr), ptr(ss),
+                                                     ptr(pa), ptr(pb), ptr(pc)))
+        a, b, c = _unflatten_g1(pa), _unflatten_g2(pb), _unflatten_g1(pc)
+        return [{"PiA": a[p], "PiB": b[p], "PiC": c[p]} for p in range(k)]
+
     def device_bytes(self):
         return _lib.pk_device_bytes(self.handle)
 

@@ -395,6 +395,35 @@ func (k *Groth16Key) ProveWitness(r1cs *R1CS, w []*big.Int, r, s *big.Int) (piA 
 	return G1FromLimbs(a), G2FromLimbs(b), G1FromLimbs(c), nil
 }
 
+// ProveWitnessBatch is ProveWitness for k witnesses of one circuit in one call (b200_groth16_prove_witness_batch):
+// proof p is ProveWitness(r1cs, ws[p], rs[p], ss[p]).  Worth it for small circuits proved many times.
+func (k *Groth16Key) ProveWitnessBatch(r1cs *R1CS, ws [][]*big.Int, rs, ss []*big.Int) (piA [][3]*big.Int, piB [][3][2]*big.Int, piC [][3]*big.Int, err error) {
+	n := len(ws)
+	if n == 0 || len(rs) != n || len(ss) != n {
+		return nil, nil, nil, errors.New("b200: ProveWitnessBatch needs k >= 1 witnesses and k r, s")
+	}
+	var fw, fr, fs []uint64
+	for p := 0; p < n; p++ {
+		if len(ws[p]) != len(ws[0]) {
+			return nil, nil, nil, errors.New("b200: ProveWitnessBatch: witnesses of different lengths")
+		}
+		fw = append(fw, FlatFr(ws[p], Scalar)...)
+		fr = append(fr, limbs(nil, rs[p])...)
+		fs = append(fs, limbs(nil, ss[p])...)
+	}
+	a, b, c := make([]uint64, 12*n), make([]uint64, 24*n), make([]uint64, 12*n)
+	rc := C.b200_groth16_prove_witness_batch(k.h, r1cs.h, u64(fw), C.size_t(len(ws[0])), C.size_t(n), u64(fr), u64(fs), u64(a), u64(b), u64(c))
+	if err = check(rc); err != nil {
+		return
+	}
+	for p := 0; p < n; p++ {
+		piA = append(piA, G1FromLimbs(a[12*p:12*p+12]))
+		piB = append(piB, G2FromLimbs(b[24*p:24*p+24]))
+		piC = append(piC, G1FromLimbs(c[12*p:12*p+12]))
+	}
+	return
+}
+
 // ---- multi-GPU: one process per GPU, NCCL inside the library ----------------------------------------------------------
 // Rank 0 calls CommUniqueID and hands the 128 bytes to the other ranks (any side channel); every rank calls CommInit after
 // choosing its device, loads its shard with LoadGroth16Shard, and then calls key.Prove with the SAME w, px, r, s: the

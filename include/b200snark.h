@@ -404,6 +404,42 @@ int b200_groth16_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w
  *     front end, and reads the whole witness; every other rank reads only its witness ranges.                       */
 int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw,
                                       const uint64_t r[4], const uint64_t s[4], void* d_out, void* stream);
+/* k witness-fed Groth16 proofs under one key in one set of launches.  Proof p is the group element triple that
+ * b200_groth16_prove_witness(_device) returns for (w_p, r_p, s_p), satisfied witness or not (compare affine: the
+ * Jacobian representatives may differ).  Witness p is at w + p*nw*4 words (k*nw standard-form scalars, row-major); r and
+ * s are host arrays of k x 4 limbs (the host splits them for the blinding products).  Outputs: pi_a k x 12, pi_b k x 24,
+ * pi_c k x 12 words.
+ *   - One batched sort serves the A, B1 and B2 MSMs of all k proofs (scalar vectors w_p ++ [1, r_p, s_p]); C||PTD has
+ *     its own.  Each set runs one batched bucket phase (b200_msm_device_batch), the blinding products take one warp per
+ *     proof and one kernel combines the k proofs.
+ *   - len(Z) = n + 1, n >= 2 (the h-direct shape): the k quotients come from one batched front end (witness load, one
+ *     sparse product of A and B over all k witnesses, Newton coefficients, shift products, interpolation), so a batch
+ *     issues the launches of a batch of one, plus the documented extras of b200_msm_device_batch (one more launch when
+ *     k*G*2^(c-1) bucket counters of a set exceed 64 Ki, one or two per further 65535 tail rows).  Any other len(Z)
+ *     takes px and the division like the single entry, once per witness: correct, but not batched.
+ *   - Runs on the key's prove context; calls on keys of one context must be ordered.  Batches on keys of contexts 0 and
+ *     1 may be in flight together, also on one R1CS handle.  Waits with the library mutex released.
+ *   - Scratch: about k times one proof's sort, bucket and front-end scratch.  The key's (counted by
+ *     b200_pk_device_bytes: scalar vectors, records, the sets' batch sorts and bucket phases) and the R1CS workspace's
+ *     are allocated on the first batch and grown (never shrunk) by a larger one, which first waits for the previous
+ *     batch; the pinned landing area of this entry holds k*48 + 1 words.
+ *   - B200_EINVAL before anything is allocated or enqueued: k = 0, a bad handle or null pointer, nw different from the
+ *     key's m or the R1CS's m, a sharded key, or a batch too large for 32-bit indexing: k*ceil(255/c)*(m+3) sort entries
+ *     (or k times a set's buckets) reaching 2^31, the same for the C||PTD set, or 3k*2N >= 2^32 transform elements
+ *     (N = the power of two >= n).
+ *   - B200_ERANGE: any r_p or s_p >= r (before anything is enqueued); a witness entry >= r in any witness (the outputs
+ *     are left untouched, and the next call starts from a clear error word). */
+int b200_groth16_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, size_t k,
+                                     const uint64_t* r, const uint64_t* s,
+                                     uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c);
+/* b200_groth16_prove_witness_batch from device memory: d_w holds the k witnesses (standard form, witness p at
+ * d_w + p*nw*32 bytes), d_out receives k x 48 u64 on `stream`, proof p at d_out + 48p in the PiA | PiC | PiB order of
+ * b200_groth16_prove_witness_device.  r and s stay host arrays (k x 4 limbs).  No host synchronisation, except in a
+ * call that first meets a given (R1CS, prove context) pair or grows a scratch; a regrowth waits for an event recorded
+ * behind the key's previous batch, not for the device.  A witness entry >= r is read as 0 and reported by no call, as
+ * in b200_groth16_prove_witness_device; the other errors are those of the host entry. */
+int b200_groth16_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                            const uint64_t* r, const uint64_t* s, void* d_out, void* stream);
 
 /* ---- element-wise group operations, reference formulas (X,Y,Z-exact) ------------------- */
 /* bn128.G1.Add / Double / Neg / Affine (bn128/g1.go:32-170) and the G2 twins (bn128/g2.go:32-200), n independent
