@@ -24,6 +24,7 @@
 #include "comm.cuh"
 #include "shard_partition.h"
 #include "glv.cuh"
+#include "pinocchio_batch.cuh"
 #ifndef B200_NO_PAIRING
 #include "pairing.cuh"
 #include "pairing_warp.cuh"
@@ -1043,6 +1044,213 @@ int groth16_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, 
   return B200_OK;
 }
 
+// ---- witness-fed Pinocchio proving (b200_pinocchio_prove_witness and its _device / _batch twins) ---------------------------
+// snark.GenerateProofs fed from the DEVICE-resident witness d_w, as groth16_witness_enqueue: the quotient comes from the
+// resident sparse R1CS on the key's side stream 3, where the G1T MSM consumes it, so the QAP front end overlaps the seven
+// witness MSMs.  On a sharded key only the rank that holds G1T runs it; every other rank launches no QAP kernel.  d_out
+// and `record` as in pinocchio_enqueue.  No host synchronisation after the first call on an (R1CS, context) pair.
+int pinocchio_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, Fq* d_out, bool record, cudaStream_t st, int* err) {
+  const size_t npx = 2 * r1->n - 1;
+  if (!pk->g[7]) return pinocchio_enqueue(pk, d_w, nullptr, npx, 0, nullptr, d_out, record, st, err);
+  R1csWork* ws;
+  int rc = r1cs_work(r1, pk->ctx, &ws);
+  if (rc) return rc;
+  cudaStream_t sq = g_serial ? st : pk->pctx().side[2];   // measurement mode: the front end on the caller's stream
+  if (sq != st) {
+    CU(cudaEventRecord(pk->ev[0], st));
+    CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
+  }
+  PolyCtx& pc = *pk->pctx().poly;
+  if (r1->n >= 2 && pk->Z.nb == r1->n + 1) {   // h-direct, as groth16_witness_enqueue
+    if ((rc = qap_h_enqueue(r1, *ws, pc, d_w, err, sq))) return rc;
+    return pinocchio_enqueue(pk, d_w, nullptr, npx, 0, ws->h_std.as<Fr>(), d_out, record, st, err);
+  }
+  if ((rc = qap_px_enqueue(r1, *ws, pc, d_w, nullptr, nullptr, err, sq))) return rc;
+  return pinocchio_enqueue(pk, d_w, ws->px_mont.as<Fr>(), npx, /*px_mont=*/1, nullptr, d_out, record, st, err);
+}
+
+// What every witness-fed Pinocchio entry refuses before anything is allocated or enqueued.
+int pinocchio_witness_check(const ProvingKey* pk, const R1cs* r1, size_t nw, const char* what) {
+  if (nw != pk->m || nw != r1->m) return fail(B200_EINVAL, "%s: witness length %zu, NVars %zu, R1CS columns %zu", what, nw, pk->m, r1->m);
+  return pinocchio_check_px(pk, 2 * r1->n - 1, what);
+}
+
+int pinocchio_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, uint64_t* out_g1, uint64_t* pi_b,
+                            std::unique_lock<std::mutex>* lk) {
+  const char* what = "pinocchio_prove_witness";
+  ProvingKey* pk = find_pk(h, 2);
+  R1cs* r1 = find_r1cs(hr);
+  if (!pk || !r1) return fail(B200_EINVAL, "%s: bad handle", what);
+  if (!w || !out_g1 || !pi_b) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = pinocchio_witness_check(pk, r1, nw, what);
+  if (rc) return rc;
+  if (pk->world > 1 && !pinocchio_gathers(pk))
+    return fail(B200_EINVAL, "%s: sharded key (rank %d/%d) without a matching communicator: call b200_comm_init, or use "
+                             "b200_pinocchio_prove_witness_device + b200_pinocchio_finalize_records around your own all-gather",
+                what, pk->rank, pk->world);
+  cudaStream_t st = pk->pctx().main;
+  Fr* dw = pk->s1.as<Fr>();
+  CU(cudaMemcpyAsync(dw, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  Fq* o = pk->out_std.as<Fq>();
+  if ((rc = pinocchio_witness_enqueue(pk, r1, dw, o, false, st, pk->d_err_sync.as<int>()))) return rc;
+  return finish_host_proof(pk, o, what, st, lk, {{out_g1, 84}, {pi_b, 24}});
+}
+
+// ---- batches: k witness-fed Pinocchio proofs under one key (b200_pinocchio_prove_witness_batch) -------------------------
+// Proof p is the proof of pinocchio_witness_enqueue for w_p.  Pinocchio has no blinding, so the scalar vectors of the seven
+// witness MSMs are the caller's witnesses where they lie (stride m): one batched sort of d_w serves B, Bp, C, Cp, Kp, one
+// of d_w + l1 serves A, Ap, and one of the k quotient vectors serves G1T; eight batched bucket phases and one
+// finalisation kernel follow: the launches of one proof, whatever k.
+
+// Sets whose batches share one digit sort (the set's own index: it sorts), as the groups of pinocchio_enqueue.
+constexpr int kPinSortSrc[8] = {0, 0, 2, 2, 2, 2, 2, 7};
+
+int pinocchio_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_t k, const char* what) {
+  if (k == 0) return fail(B200_EINVAL, "%s: k = 0", what);
+  int rc = pinocchio_witness_check(pk, r1, nw, what);
+  if (rc) return rc;
+  if (pk->world != 1) return fail(B200_EINVAL, "%s: sharded key (rank %d/%d): batches need an unsharded key", what, pk->rank, pk->world);
+  const size_t ma = pk->m - pk->npublic - 1;
+  const size_t terms[8] = {ma, ma, pk->m, pk->m, pk->m, pk->m, pk->m, pk->n_h_bases};
+  for (int j = 0; j < 8; j++)
+    if (pk->g[j] && !batch_fits(pk->g[j].get(), k, terms[j]))
+      return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
+                  pk->g[j]->sh.nwin, terms[j], j);
+  const uint64_t N = pow2_at_least(r1->n);
+  if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
+  return B200_OK;
+}
+
+// d_w: k witnesses (device, standard form, witness p at d_w + p*m); d_out: k x 108 u64, proof p at d_out + 108p (the seven
+// G1 points, then PiB).  After pinocchio_batch_check.  No host synchronisation unless a scratch grows (or the first batch
+// on this R1CS and context builds its domains).
+int pinocchio_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq* d_out, cudaStream_t st, int* err) {
+  const size_t m = pk->m, l1 = pk->npublic + 1, ng = pk->n_h_bases, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
+  const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as pinocchio_witness_enqueue
+  const size_t terms[8] = {m - l1, m - l1, m, m, m, m, m, ng};
+  // every scratch first: growing one waits for the batch that used it last, so nothing of this batch is enqueued yet
+  R1csWork* ws;
+  int rc = r1cs_work(r1, pk->ctx, &ws);
+  if (rc) return rc;
+  R1csBatch* fb = nullptr;
+  if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+  if ((rc = pinocchio_batch_scratch(pk, k, false))) return rc;
+  for (int j = 0; j < 8; j++) {
+    if (!pk->g[j]) continue;   // A, Ap of a circuit whose signals are all public
+    const bool own = kPinSortSrc[j] == j;
+    rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own)
+                : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own);
+    if (rc) return rc;
+  }
+  for (int j = 0; j < 8; j++) {   // a set that reuses another's sort was sized for the same slices (msm_buckets' check)
+    if (!pk->g[j]) continue;
+    const Bases* a = pk->g[j].get();
+    const Bases* src = pk->g[kPinSortSrc[j]].get();
+    if (a->sh.c != src->sh.c || a->sh.table_stride != src->sh.table_stride || a->sh.rows != src->sh.rows ||
+        a->sort.max_slices != src->sort.max_slices || a->affine_S != src->affine_S || a->batch->vecs != src->batch->vecs ||
+        a->batch->sort.sh.n != src->batch->sort.sh.n)
+      return fail(B200_EINVAL, "pinocchio_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, kPinSortSrc[j]);
+  }
+  ProveBatch& b = *pk->batch;
+  cudaStream_t side[3] = {pk->pctx().side[0], pk->pctx().side[1], pk->pctx().side[2]};
+  if (g_serial) side[0] = side[1] = side[2] = st;   // measurement mode (b200_profile bit 1)
+  cudaEvent_t e_in = b.ev[0], e_sorted[2] = {b.ev[1], b.ev[2]}, e_done[3] = {b.ev[3], b.ev[4], b.ev[5]};
+  XYZZ<Fq>* rec1 = b.rec.as<XYZZ<Fq>>();                         // slot s of proof p at rec1[s*k + p]
+  XYZZ<Fq2>* rec2 = reinterpret_cast<XYZZ<Fq2>*>(rec1 + 7 * k);
+  auto sort_of = [&](int j, const Fr* sc, size_t stride, cudaStream_t s) {
+    Bases* g = pk->g[j].get();
+    MsmShape sh = g->sh;
+    sh.vecs = (uint32_t)k;
+    sh.vec_stride = (uint32_t)stride;
+    return msm_sort(g->batch->sort, sh, sc, terms[j], 0, err, s, g->batch->scan_totals.as<unsigned long long>());
+  };
+  auto buckets_of = [&](int j, cudaStream_t s) {
+    Bases* g = pk->g[j].get();
+    const SortScratch& ss = pk->g[kPinSortSrc[j]]->batch->sort;
+    if (j == 2) return bucket_phase<Fq2>(g, ss, g->batch->bk, (uint32_t)k, terms[j], rec2, s);
+    return bucket_phase<Fq>(g, ss, g->batch->bk, (uint32_t)k, terms[j], rec1 + kPinSlot[j] * k, s);
+  };
+  // sets the key does not hold (A, Ap when every signal is public) leave their records at infinity, as in pinocchio_enqueue
+  CU(cudaMemsetAsync(b.rec.p, 0, k * (7 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>)), st));
+  EV_REC(e_in, st);
+  // --- side stream 3: the k quotients into the G1T scalar vectors (zero-filled to len(G1T)), then the G1T MSMs
+  cudaStream_t s3 = side[2];
+  if (s3 != st) EV_WAIT(s3, e_in);
+  PolyCtx& pc = *pk->pctx().poly;
+  Fr* H = b.CH.as<Fr>();
+  const uint32_t qtotal = (uint32_t)(k * (ng + 1));
+  if (h_direct) {
+    if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
+    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)ng,
+                                                        nullptr, 0, qtotal, H, (uint32_t)ng);
+  } else {   // not batched: the single-witness px and division of each witness, straight into its vector
+    for (size_t p = 0; p < k; p++) {
+      if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
+      CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, H + p * ng, nullptr, err, s3));
+    }
+    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)ng, nullptr, 0, qtotal, H, (uint32_t)ng);
+  }
+  g_launches += 1;
+  if ((rc = sort_of(7, H, ng, s3))) return rc;
+  if ((rc = buckets_of(7, s3))) return rc;
+  // --- the witness MSMs: both sorts on the main stream, then the bucket phases fan out as in pinocchio_enqueue (G2 first)
+  if ((rc = sort_of(2, d_w, m, st))) return rc;
+  EV_REC(e_sorted[1], st);
+  if (pk->g[0]) {
+    if ((rc = sort_of(0, d_w + l1, m, st))) return rc;
+    EV_REC(e_sorted[0], st);
+  }
+  int next_side = 0;
+  for (int j : {2, 3, 4, 5, 6, 0, 1}) {
+    if (!pk->g[j]) continue;
+    cudaStream_t sk = j == 2 ? st : side[next_side++ % 3];   // one bucket phase stays on the main stream
+    if (sk != st) EV_WAIT(sk, e_sorted[kPinSortSrc[j] == 2 ? 1 : 0]);
+    if ((rc = buckets_of(j, sk))) return rc;
+  }
+  for (int si = 0; si < 3; si++)
+    if (side[si] != st) {
+      EV_REC(e_done[si], side[si]);
+      EV_WAIT(st, e_done[si]);
+    }
+  k_pinocchio_finalize_batch<<<nblk(7 * k, kPinFinalizeBlock) + nblk(k, kPinFinalizeBlock), kPinFinalizeBlock, 0, st>>>(
+      rec1, rec2, (uint32_t)k, d_out);
+  g_launches += 1;
+  CU(cudaGetLastError());
+  // behind everything of this batch: what the next regrowth of any of its scratches waits for
+  EV_REC(b.done, st);
+  for (const auto& g : pk->g)
+    if (g && g->batch) EV_REC(g->batch->done, st);
+  if (fb) EV_REC(fb->done, st);
+  return B200_OK;
+}
+
+int pinocchio_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, size_t k, uint64_t* out_g1,
+                                  uint64_t* pi_b, std::unique_lock<std::mutex>* lk) {
+  const char* what = "pinocchio_prove_witness_batch";
+  ProvingKey* pk = find_pk(h, 2);
+  R1cs* r1 = find_r1cs(hr);
+  if (!pk || !r1) return fail(B200_EINVAL, "%s: bad handle", what);
+  if (!w || !out_g1 || !pi_b) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = pinocchio_batch_check(pk, r1, nw, k, what);
+  if (rc) return rc;
+  if ((rc = pinocchio_batch_scratch(pk, k, true))) return rc;
+  ProveBatch& b = *pk->batch;
+  cudaStream_t st = pk->pctx().main;
+  CU(cudaMemcpyAsync(b.w_stage.p, w, k * nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  Fq* o = b.out.as<Fq>();
+  if ((rc = pinocchio_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, o, st, pk->d_err_sync.as<int>()))) return rc;
+  // as finish_host_proof, for k proofs: the wait runs with the library mutex released
+  CU(cudaMemcpyAsync(b.h_out, o, k * kHostProofWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(b.h_out + k * kHostProofWords));
+  if (rc) return rc;
+  for (size_t p = 0; p < k; p++) {
+    const uint64_t* q = b.h_out + kHostProofWords * p;
+    memcpy(out_g1 + 84 * p, q, 84 * sizeof(uint64_t));
+    memcpy(pi_b + 24 * p, q + 84, 24 * sizeof(uint64_t));
+  }
+  return B200_OK;
+}
+
 // ---- dense QAP API (small n) -------------------------------------------------
 int r1cs_to_qap_host(const uint64_t* a, const uint64_t* b, const uint64_t* c, size_t n, size_t m, uint64_t* alphas,
                      uint64_t* betas, uint64_t* gammas, uint64_t* z) {
@@ -1691,6 +1899,57 @@ int b200_groth16_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, cons
   if (rc) return rc;
   return drain_on_error(groth16_batch_enqueue(p, r1, (const Fr*)d_w, k, r, s, (Fq*)d_out,
                                               stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_pinocchio_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const void* d_px, size_t npx, void* d_out,
+                                void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  const char* what = "pinocchio_prove_device";
+  ProvingKey* p = find_pk(pk, 2);
+  if (!p || !d_w || !d_px || !d_out) return fail(B200_EINVAL, "%s: bad arguments", what);
+  if (nw != p->m) return fail(B200_EINVAL, "%s: witness length %zu != NVars %zu", what, nw, p->m);
+  int rc = pinocchio_check_px(p, npx, what);
+  if (rc) return rc;
+  return drain_on_error(pinocchio_enqueue(p, (const Fr*)d_w, (const Fr*)d_px, npx, 0, nullptr, (Fq*)d_out,
+                                          p->world > 1 && !pinocchio_gathers(p),
+                                          stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_pinocchio_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, uint64_t* out_g1,
+                                 uint64_t pi_b[24]) {
+  std::unique_lock<std::mutex> lk(g_mu);
+  NEED_INIT();
+  return drain_on_error(pinocchio_prove_witness(pk, r1cs, w, nw, out_g1, pi_b, &lk));
+}
+int b200_pinocchio_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, void* d_out, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  const char* what = "pinocchio_prove_witness_device";
+  ProvingKey* p = find_pk(pk, 2);
+  R1cs* r1 = find_r1cs(r1cs);
+  if (!p || !r1 || !d_w || !d_out) return fail(B200_EINVAL, "%s: bad arguments", what);
+  int rc = pinocchio_witness_check(p, r1, nw, what);
+  if (rc) return rc;
+  return drain_on_error(pinocchio_witness_enqueue(p, r1, (const Fr*)d_w, (Fq*)d_out, p->world > 1 && !pinocchio_gathers(p),
+                                                  stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_pinocchio_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, size_t k,
+                                       uint64_t* out_g1, uint64_t* pi_b) {
+  std::unique_lock<std::mutex> lk(g_mu);
+  NEED_INIT();
+  return drain_on_error(pinocchio_prove_witness_batch(pk, r1cs, w, nw, k, out_g1, pi_b, &lk));
+}
+int b200_pinocchio_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                              void* d_out, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  const char* what = "pinocchio_prove_witness_batch_device";
+  ProvingKey* p = find_pk(pk, 2);
+  R1cs* r1 = find_r1cs(r1cs);
+  if (!p || !r1 || !d_w || !d_out) return fail(B200_EINVAL, "%s: bad arguments", what);
+  int rc = pinocchio_batch_check(p, r1, nw, k, what);
+  if (rc) return rc;
+  return drain_on_error(pinocchio_batch_enqueue(p, r1, (const Fr*)d_w, k, (Fq*)d_out,
+                                                stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
 }
 int b200_fq12_mul_batch(const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) { B200_API_BODY(fq12_mul_batch_host(a, b, n, out)) }
 int b200_pairing_batch(const uint64_t* g1_jac, const uint64_t* g2_jac, size_t n, uint64_t* out) { B200_API_BODY(pairing_batch_host(g1_jac, g2_jac, n, out)) }

@@ -159,6 +159,15 @@ HD Jacobian<F> xyzz_to_jacobian(const XYZZ<F>& p) {
   return Jacobian<F>{p.X * zz2, p.Y * (zz2 * p.ZZ), p.ZZZ};
 }
 
+// out[0..3) = the Jacobian form of p (no inversion), standard form; infinity gives three zeros
+template <class F>
+HD void store_jacobian_std(const XYZZ<F>& p, F* out) {
+  Jacobian<F> j = xyzz_to_jacobian(p);
+  out[0] = j.X.from_mont();
+  out[1] = j.Y.from_mont();
+  out[2] = j.Z.from_mont();
+}
+
 template <class F>
 HD XYZZ<F> jacobian_to_xyzz(const Jacobian<F>& p) {
   if (p.is_inf()) return XYZZ<F>::inf();

@@ -24,18 +24,20 @@
 // (caller's + 3 side streams): the latency-bound tails (bucket reduction, tree sum) of
 // one MSM overlap the throughput-bound accumulation of the others.
 
-// A key's scratch for batches of up to k proofs (b200_groth16_prove_witness_batch): allocated on the first batch, grown
-// (never shrunk) by a larger one after waiting for `done`, which is recorded behind the key's last batch.
+// A key's scratch for batches of up to k proofs (b200_groth16_prove_witness_batch, b200_pinocchio_prove_witness_batch):
+// allocated on the first batch, grown (never shrunk) by a larger one after waiting for `done`, which is recorded behind
+// the key's last batch.  A Pinocchio key has no blinding, so it holds only the quotient vectors, the records and the host
+// entry's buffers: its other seven scalar vectors are the caller's witnesses themselves.
 struct ProveBatch {
   size_t k = 0;
   DevBuf W;          // k scalar vectors w_p ++ [1, r_p, s_p] of A, B1, B2 (stride m + 3)
-  DevBuf CH;         // k scalar vectors of C||PTD: w_p[l+1..m) ++ h_p ++ 0.. ++ [-r_p s_p]
-  DevBuf rec;        // k records per set: A, B1 (G1), B2 (G2), CH (G1), then 2k products (G1)
+  DevBuf CH;         // k scalar vectors of C||PTD: w_p[l+1..m) ++ h_p ++ 0.. ++ [-r_p s_p]; Pinocchio: of G1T, h_p ++ 0..
+  DevBuf rec;        // k records per set: A, B1 (G1), B2 (G2), CH (G1), then 2k products (G1); Pinocchio: 7k G1, then k G2
   DevBuf rs;         // per proof {1, r_p, s_p, -r_p s_p}, standard form
   DevBuf glv;        // per proof GlvScalars of (s_p, r_p)
   DevBuf w_stage;    // the host entry's witnesses
-  DevBuf out;        // the host entry's k proofs (48 u64 each)
-  uint64_t* h_out = nullptr;   // pinned landing area of the host entry: k * 48 words + the error word
+  DevBuf out;        // the host entry's k proofs (48 u64 each; Pinocchio: 108)
+  uint64_t* h_out = nullptr;   // pinned landing area of the host entry: the k proofs + the error word
   cudaEvent_t ev[9] = {};
   cudaEvent_t done = nullptr;
   ProveBatch() = default;
@@ -89,7 +91,7 @@ struct ProvingKey {
   // the key's main stream.  Its own word, because those calls wait with the library mutex released: a word shared with
   // a proof on another key would report one proof's error to the other.
   DevBuf d_err_sync;
-  std::unique_ptr<ProveBatch> batch;   // b200_groth16_prove_witness_batch scratch (null until the first batch)
+  std::unique_ptr<ProveBatch> batch;   // scratch of the key's batches of proofs (null until the first batch)
 };
 
 size_t pk_device_bytes(const ProvingKey& pk) {
@@ -124,14 +126,6 @@ __device__ XYZZ<F> xyzz_mul_scalar(const XYZZ<F>& p, const Fr& k) {
     }
   }
   return r;
-}
-
-template <class F>
-__device__ void store_jacobian_std(const XYZZ<F>& p, F* out) {
-  Jacobian<F> j = xyzz_to_jacobian(p);
-  out[0] = j.X.from_mont();
-  out[1] = j.Y.from_mont();
-  out[2] = j.Z.from_mont();
 }
 
 // Partial-result record of one rank: A (G1 XYZZ @ +0), B1 (@ +256), B2 (G2 XYZZ @ +512),
@@ -687,37 +681,30 @@ int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2,
   return B200_OK;
 }
 
-// On the key's prove context; waits with the library mutex held.  d_rec_out != nullptr: leave this rank's 2 KB record of
-// XYZZ results there (device) — the form the one-GPU tests use to emulate N ranks.
-int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px, size_t npx, uint64_t* out_g1,
-                    uint64_t* pi_b, uint8_t* d_rec_out = nullptr) {
-  ProvingKey* pk = find_pk(h, 2);
-  if (!pk) return fail(B200_EINVAL, "pinocchio_prove: bad proving-key handle");
-  if (!w || !px || (!d_rec_out && (!out_g1 || !pi_b))) return fail(B200_EINVAL, "pinocchio_prove: null pointer");
-  size_t m = pk->m, l1 = pk->npublic + 1;
-  if (nw != m) return fail(B200_EINVAL, "pinocchio_prove: witness length %zu != NVars %zu", nw, m);
-  if (npx < pk->Z.nb) return fail(B200_EINVAL, "pinocchio_prove: len(px) < len(Z)");
+// len(px) against the key, as snark.GenerateProofs would index G1T (snark.go:284-286)
+int pinocchio_check_px(const ProvingKey* pk, size_t npx, const char* what) {
+  if (npx < pk->Z.nb) return fail(B200_EINVAL, "%s: len(px) < len(Z)", what);
   size_t nq = npx - pk->Z.nb + 1;
-  if (nq > pk->n_h_bases) return fail(B200_EINVAL, "pinocchio_prove: len(hx)=%zu exceeds len(G1T)=%zu", nq, pk->n_h_bases);
-  const bool sharded = pk->world > 1;
-  const bool gather = sharded && !d_rec_out;
-  if (gather && !(comm_active() && g_comm.world == pk->world && g_comm.rank == pk->rank))
-    return fail(B200_EINVAL, "pinocchio_prove: sharded key (rank %d/%d) without a matching communicator (b200_comm_init)",
-                pk->rank, pk->world);
-  cudaStream_t st = pk->pctx().main;
+  if (nq > pk->n_h_bases) return fail(B200_EINVAL, "%s: len(hx)=%zu exceeds len(G1T)=%zu", what, nq, pk->n_h_bases);
+  return B200_OK;
+}
+// A proof on this key ends in the all-gather of the ranks' records (sharded, with a matching communicator).
+bool pinocchio_gathers(const ProvingKey* pk) {
+  return pk->world > 1 && comm_active() && g_comm.world == pk->world && g_comm.rank == pk->rank;
+}
+
+// Enqueue one Pinocchio proof on `st` from the DEVICE-resident witness d_w (m standard-form scalars).  The quotient, read
+// only by the rank that holds G1T: d_h_std (npx - len(Z) + 1 coefficients, standard form, ready on the key's side stream
+// 3) when given, else px / Z from d_px (npx coefficients, Montgomery form when px_mont) on that stream.  d_out receives
+// the proof (7 G1 Jacobian points and PiB, 108 u64, standard form) or, with `record`, this rank's 2 KB record of XYZZ
+// results.  After pinocchio_check_px.  No host synchronisation.  A scalar >= r is read as 0 and sets bit 1 of *err.
+int pinocchio_enqueue(ProvingKey* pk, const Fr* d_w, const Fr* d_px, size_t npx, int px_mont, const Fr* d_h_std, Fq* d_out,
+                      bool record, cudaStream_t st, int* err) {
+  const size_t m = pk->m, l1 = pk->npublic + 1, nq = npx - pk->Z.nb + 1;
   const cudaStream_t* side = pk->pctx().side;
-  int* err = pk->d_err_sync.as<int>();
   cudaEvent_t e_in = pk->ev[0], e_sorted[2] = {pk->ev[1], pk->ev[2]}, e_done[3] = {pk->ev[3], pk->ev[4], pk->ev[5]};
-  Fr* dw = pk->s1.as<Fr>();
-  Fr* dh = pk->s3.as<Fr>();
   uint8_t* res = pk->res.as<uint8_t>();
-  CU(cudaMemcpyAsync(dw, w, m * sizeof(Fr), cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(res, 0, kPinRecordBytes, st));        // slots this rank does not own stay at infinity
-  if (pk->g[7]) {
-    CU(pk->px.ensure(npx * sizeof(Fr)));
-    const size_t px_off = pk->Z.nb - 1;   // the top nq coefficients are all the division reads (see groth16_prove)
-    CU(cudaMemcpyAsync(pk->px.as<Fr>() + px_off, reinterpret_cast<const Fr*>(px) + px_off, nq * sizeof(Fr), cudaMemcpyHostToDevice, st));
-  }
   EV_REC(e_in, st);
   int rc;
   int next_side = 0;
@@ -728,7 +715,11 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
     cudaStream_t s3 = side[2];
     used[2] = true;
     EV_WAIT(s3, e_in);
-    CU(poly_div_device(*pk->pctx().poly, pk->Z, pk->px.as<Fr>(), npx, 0, dh, nullptr, err, s3));
+    const Fr* dh = d_h_std;
+    if (!dh) {
+      CU(poly_div_device(*pk->pctx().poly, pk->Z, d_px, npx, px_mont, pk->s3.as<Fr>(), nullptr, err, s3));
+      dh = pk->s3.as<Fr>();
+    }
     if ((rc = msm_enqueue<Fq>(pk->g[7].get(), dh, nq, 0, slot_g1(7), err, s3))) return rc;
   }
   // two scalar vectors: w[l+1..m) feeds PiA, PiAp (snark.go:265-268); w feeds PiB, PiBp, PiC, PiCp, PiKp (:270-278).
@@ -739,7 +730,7 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
     for (int q = 0; q < 5; q++)
       if (groups[gi][q] >= 0 && pk->g[groups[gi][q]]) { holder[gi] = groups[gi][q]; break; }
     if (holder[gi] < 0) continue;
-    const Fr* sc = gi == 0 ? dw + l1 : dw;
+    const Fr* sc = gi == 0 ? d_w + l1 : d_w;
     const size_t cnt = gi == 0 ? m - l1 : m;
     if ((rc = msm_sort(pk->g[holder[gi]]->sort, pk->g[holder[gi]]->sh, sc, cnt, 0, err, st))) return rc;
     EV_REC(e_sorted[gi], st);
@@ -768,22 +759,78 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
       EV_REC(e_done[si], side[si]);
       EV_WAIT(st, e_done[si]);
     }
-  if (d_rec_out) {
-    CU(cudaMemcpyAsync(d_rec_out, res, kPinRecordBytes, cudaMemcpyDeviceToDevice, st));
-    CU(cudaGetLastError());
-    return check_err_flag("pinocchio_prove_record", err, st);
-  }
-  Fq* o = pk->out_std.as<Fq>();
-  if (gather) {
+  if (record) {
+    CU(cudaMemcpyAsync(d_out, res, kPinRecordBytes, cudaMemcpyDeviceToDevice, st));
+  } else if (pk->world > 1) {
     CU(pk->gather.ensure(kPinRecordBytes * (size_t)pk->world));
     ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPinRecordBytes, ncclUint8, pk->pctx().comm, st);
     if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
-    k_pinocchio_gather_finalize<<<1, 64, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, o, reinterpret_cast<Fq2*>(o + 21));
+    k_pinocchio_gather_finalize<<<1, 64, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, d_out, reinterpret_cast<Fq2*>(d_out + 21));
   } else {
-    k_pinocchio_finalize<<<1, 64, 0, st>>>(res, o, reinterpret_cast<Fq2*>(o + 21));
+    k_pinocchio_finalize<<<1, 64, 0, st>>>(res, d_out, reinterpret_cast<Fq2*>(d_out + 21));
   }
   CU(cudaGetLastError());
+  return B200_OK;
+}
+
+// On the key's prove context; waits with the library mutex held.  d_rec_out != nullptr: leave this rank's 2 KB record of
+// XYZZ results there (device) — the form the one-GPU tests use to emulate N ranks.
+int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px, size_t npx, uint64_t* out_g1,
+                    uint64_t* pi_b, uint8_t* d_rec_out = nullptr) {
+  ProvingKey* pk = find_pk(h, 2);
+  if (!pk) return fail(B200_EINVAL, "pinocchio_prove: bad proving-key handle");
+  if (!w || !px || (!d_rec_out && (!out_g1 || !pi_b))) return fail(B200_EINVAL, "pinocchio_prove: null pointer");
+  size_t m = pk->m;
+  if (nw != m) return fail(B200_EINVAL, "pinocchio_prove: witness length %zu != NVars %zu", nw, m);
+  int rc = pinocchio_check_px(pk, npx, "pinocchio_prove");
+  if (rc) return rc;
+  if (pk->world > 1 && !d_rec_out && !pinocchio_gathers(pk))
+    return fail(B200_EINVAL, "pinocchio_prove: sharded key (rank %d/%d) without a matching communicator (b200_comm_init)",
+                pk->rank, pk->world);
+  cudaStream_t st = pk->pctx().main;
+  int* err = pk->d_err_sync.as<int>();
+  Fr* dw = pk->s1.as<Fr>();
+  CU(cudaMemcpyAsync(dw, w, m * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  if (pk->g[7]) {
+    CU(pk->px.ensure(npx * sizeof(Fr)));
+    const size_t px_off = pk->Z.nb - 1;   // the top nq coefficients are all the division reads (see groth16_prove)
+    CU(cudaMemcpyAsync(pk->px.as<Fr>() + px_off, reinterpret_cast<const Fr*>(px) + px_off, (npx - px_off) * sizeof(Fr),
+                       cudaMemcpyHostToDevice, st));
+  }
+  if (d_rec_out) {
+    if ((rc = pinocchio_enqueue(pk, dw, pk->px.as<Fr>(), npx, 0, nullptr, reinterpret_cast<Fq*>(d_rec_out), true, st, err))) return rc;
+    return check_err_flag("pinocchio_prove_record", err, st);
+  }
+  Fq* o = pk->out_std.as<Fq>();
+  if ((rc = pinocchio_enqueue(pk, dw, pk->px.as<Fr>(), npx, 0, nullptr, o, false, st, err))) return rc;
   return finish_host_proof(pk, o, "pinocchio_prove", st, nullptr, {{out_g1, 84}, {pi_b, 24}});
+}
+
+// Grows a Pinocchio key's batch scratch to k proofs (host: also the host entry's witness staging, proof buffer and pinned
+// landing area), as groth16_batch_scratch does for a Groth16 key.
+int pinocchio_batch_scratch(ProvingKey* pk, size_t k, bool host) {
+  if (!pk->batch) {
+    auto b = std::make_unique<ProveBatch>();
+    for (auto& e : b->ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
+    pk->batch = std::move(b);
+  }
+  ProveBatch& b = *pk->batch;
+  const bool grow_host = host && b.out.bytes < k * kHostProofWords * sizeof(uint64_t);
+  if (b.k < k || grow_host) CU(cudaEventSynchronize(b.done));
+  if (b.k < k) {
+    CU(b.CH.alloc(k * pk->n_h_bases * sizeof(Fr)));
+    CU(b.rec.alloc(k * (7 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>))));
+    b.k = k;
+  }
+  if (grow_host) {
+    CU(b.w_stage.alloc(k * pk->m * sizeof(Fr)));
+    CU(b.out.alloc(k * kHostProofWords * sizeof(uint64_t)));
+    if (b.h_out) CU(cudaFreeHost(b.h_out));
+    b.h_out = nullptr;
+    CU(cudaHostAlloc(reinterpret_cast<void**>(&b.h_out), (k * kHostProofWords + 1) * sizeof(uint64_t), cudaHostAllocDefault));
+  }
+  return B200_OK;
 }
 
 // one-GPU emulation of the collective: sum `world` gathered records (device) -> the proof (host)

@@ -206,7 +206,7 @@ __global__ void k_take_blocks(const Fr* __restrict__ src, uint32_t sstride, uint
 }
 // C||PTD scalar vector p (ch + p*stride, from the quotient's offset): the quotient h_p below nh (coef: blocks of cstride,
 // Montgomery -> standard form; null: already in place), zeros up to n_ptd, then tail[p*tstride] (-r_p s_p, standard form).
-// total = k * (n_ptd + 1)
+// total = k * (n_ptd + 1).  A null tail writes none: the G1T scalar vectors of Pinocchio proofs (stride = n_ptd = len(G1T)).
 __global__ void k_quotient_store(const Fr* __restrict__ coef, uint32_t cstride, uint32_t nh, uint32_t n_ptd,
                                  const Fr* __restrict__ tail, uint32_t tstride, uint32_t total, Fr* __restrict__ ch,
                                  uint32_t stride) {
@@ -216,8 +216,10 @@ __global__ void k_quotient_store(const Fr* __restrict__ coef, uint32_t cstride, 
   Fr* d = ch + (size_t)p * stride + i;
   if (i < nh) {
     if (coef) *d = coef[(size_t)p * cstride + i].from_mont();
-  } else {
-    *d = i < n_ptd ? Fr::zero() : tail[(size_t)p * tstride];
+  } else if (i < n_ptd) {
+    *d = Fr::zero();
+  } else if (tail) {
+    *d = tail[(size_t)p * tstride];
   }
 }
 // leaves of the subproduct tree over the points offset+1 .. offset+N: t[k] = -(offset + k + 1)

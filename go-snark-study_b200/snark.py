@@ -46,6 +46,32 @@ class DeviceProvingKey:
         proof["PiB"] = _unflatten_g2(pb)[0]
         return proof
 
+    def prove_witness_limbs(self, r1cs, w_limbs):
+        """The proof from the witness alone (b200_pinocchio_prove_witness): px, or the quotient directly, is computed on
+        the device from ``r1cs`` (an r1csqap.SparseR1CS of the same circuit)."""
+        g1 = np.zeros(84, dtype=np.uint64)
+        pb = np.zeros(24, dtype=np.uint64)
+        check(lib().b200_pinocchio_prove_witness(self.handle, r1cs.handle, ptr(w_limbs), w_limbs.shape[0], ptr(g1), ptr(pb)))
+        proof = dict(zip(_ORDER, _unflatten_g1(g1)))
+        proof["PiB"] = _unflatten_g2(pb)[0]
+        return proof
+
+    def prove_witness_batch_limbs(self, r1cs, w_limbs):
+        """k proofs in one call (b200_pinocchio_prove_witness_batch): ``w_limbs`` holds k witnesses (k x m x 4 limbs).
+        Proof p is prove_witness_limbs(r1cs, w_limbs[p])."""
+        w = np.ascontiguousarray(w_limbs, dtype=np.uint64)
+        if w.ndim != 3 or w.shape[0] == 0 or w.shape[2] != 4:
+            raise ValueError("prove_witness_batch_limbs: need k >= 1 witnesses as a k x m x 4 array")
+        k, m = w.shape[0], w.shape[1]
+        g1 = np.zeros(84 * k, dtype=np.uint64)
+        pb = np.zeros(24 * k, dtype=np.uint64)
+        check(lib().b200_pinocchio_prove_witness_batch(self.handle, r1cs.handle, ptr(w), m, k, ptr(g1), ptr(pb)))
+        p1, p2 = _unflatten_g1(g1), _unflatten_g2(pb)
+        proofs = [dict(zip(_ORDER, p1[7 * p:7 * p + 7])) for p in range(k)]
+        for p in range(k):
+            proofs[p]["PiB"] = p2[p]
+        return proofs
+
     def device_bytes(self):
         return _lib.pk_device_bytes(self.handle)
 

@@ -424,6 +424,72 @@ func (k *Groth16Key) ProveWitnessBatch(r1cs *R1CS, ws [][]*big.Int, rs, ss []*bi
 	return
 }
 
+// ---- snark.GenerateProofs (Pinocchio) fed from the witness -------------------------------------------------------------
+// PinocchioKey is a snark.Pk resident on the device (b200_pinocchio_pk_load).
+type PinocchioKey struct{ h C.b200_pk_t }
+
+// PinocchioProof is snark.Proof (snark.go:38-47).
+type PinocchioProof struct {
+	PiA, PiAp, PiBp, PiC, PiCp, PiH, PiKp [3]*big.Int
+	PiB                                   [3][2]*big.Int
+}
+
+// LoadPinocchio uploads snark.Pk: a, ap, bp, c, cp, kp and b (G2) hold one point per signal.
+func LoadPinocchio(a, ap [][3]*big.Int, b [][3][2]*big.Int, bp, c, cp, kp, g1t [][3]*big.Int, z []*big.Int, nPublic int) (*PinocchioKey, error) {
+	k := &PinocchioKey{}
+	rc := C.b200_pinocchio_pk_load(u64(FlatG1(a)), u64(FlatG1(ap)), u64(FlatG2(b)), u64(FlatG1(bp)), u64(FlatG1(c)),
+		u64(FlatG1(cp)), u64(FlatG1(kp)), C.size_t(len(a)), u64(FlatG1(g1t)), C.size_t(len(g1t)), u64(FlatFr(z, Coeff)),
+		C.size_t(len(z)), C.size_t(nPublic), 0, &k.h)
+	if err := check(rc); err != nil {
+		return nil, err
+	}
+	return k, nil
+}
+
+func (k *PinocchioKey) Free() { C.b200_pk_free(k.h) }
+
+func pinocchioProof(g1, b []uint64) *PinocchioProof {
+	pt := func(i int) [3]*big.Int { return G1FromLimbs(g1[12*i : 12*i+12]) }
+	return &PinocchioProof{PiA: pt(0), PiAp: pt(1), PiBp: pt(2), PiC: pt(3), PiCp: pt(4), PiH: pt(5), PiKp: pt(6), PiB: G2FromLimbs(b)}
+}
+
+// ProveWitness is snark.GenerateProofs fed from the witness: px never leaves the device (b200_pinocchio_prove_witness).
+func (k *PinocchioKey) ProveWitness(r1cs *R1CS, w []*big.Int) (*PinocchioProof, error) {
+	fw := FlatFr(w, Scalar)
+	g1, b := make([]uint64, 84), make([]uint64, 24)
+	rc := C.b200_pinocchio_prove_witness(k.h, r1cs.h, u64(fw), C.size_t(len(w)), u64(g1), u64(b))
+	if err := check(rc); err != nil {
+		return nil, err
+	}
+	return pinocchioProof(g1, b), nil
+}
+
+// ProveWitnessBatch is ProveWitness for k witnesses of one circuit in one call (b200_pinocchio_prove_witness_batch):
+// proof p is ProveWitness(r1cs, ws[p]).  Worth it for small circuits proved many times.
+func (k *PinocchioKey) ProveWitnessBatch(r1cs *R1CS, ws [][]*big.Int) ([]*PinocchioProof, error) {
+	n := len(ws)
+	if n == 0 {
+		return nil, errors.New("b200: ProveWitnessBatch needs k >= 1 witnesses")
+	}
+	var fw []uint64
+	for p := 0; p < n; p++ {
+		if len(ws[p]) != len(ws[0]) {
+			return nil, errors.New("b200: ProveWitnessBatch: witnesses of different lengths")
+		}
+		fw = append(fw, FlatFr(ws[p], Scalar)...)
+	}
+	g1, b := make([]uint64, 84*n), make([]uint64, 24*n)
+	rc := C.b200_pinocchio_prove_witness_batch(k.h, r1cs.h, u64(fw), C.size_t(len(ws[0])), C.size_t(n), u64(g1), u64(b))
+	if err := check(rc); err != nil {
+		return nil, err
+	}
+	proofs := make([]*PinocchioProof, n)
+	for p := range proofs {
+		proofs[p] = pinocchioProof(g1[84*p:84*p+84], b[24*p:24*p+24])
+	}
+	return proofs, nil
+}
+
 // ---- multi-GPU: one process per GPU, NCCL inside the library ----------------------------------------------------------
 // Rank 0 calls CommUniqueID and hands the 128 bytes to the other ranks (any side channel); every rank calls CommInit after
 // choosing its device, loads its shard with LoadGroth16Shard, and then calls key.Prove with the SAME w, px, r, s: the

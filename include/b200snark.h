@@ -441,6 +441,78 @@ int b200_groth16_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint6
 int b200_groth16_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
                                             const uint64_t* r, const uint64_t* s, void* d_out, void* stream);
 
+/* ---- Pinocchio from device memory, from the witness, and in batches ----------------------------------------------------
+ * The twins of the Groth16 entries above for snark.GenerateProofs (snark.go:254-289).  Pinocchio has no blinding, so there
+ * is no r or s.  Output layout everywhere: the 7 Jacobian G1 points in the order of b200_pinocchio_prove (PiA, PiAp, PiBp,
+ * PiC, PiCp, PiH, PiKp; 84 u64) and PiB (24 u64), standard form; in device memory those 108 u64 are contiguous (the G1
+ * block, then PiB).  All of them run on the key's prove context (B200_CFG_PK_CONTEXT); two proofs on keys of ONE context
+ * must be ordered by the caller, proofs on keys of contexts 0 and 1 may be in flight together.                           */
+/* b200_pinocchio_prove with the witness and px already resident in DEVICE memory (standard form) and the 108-u64 proof
+ * left in device memory on `stream`; no host synchronisation.  As in b200_groth16_prove_device, a witness entry or a px
+ * coefficient >= r is read as 0, and neither this call nor any later one reports it (nor a proof on another key).
+ * B200_EINVAL: a bad handle (a Groth16 key included), a null pointer, nw different from the key's m, len(px) < len(Z),
+ * len(hx) > len(G1T).  On a sharded key (b200_pinocchio_pk_load_shard) only the rank that holds G1T reads px; with a
+ * matching communicator d_out receives the whole proof on every rank, without one the rank's 2 KB record (the layout of
+ * b200_pinocchio_prove_record_device) for b200_pinocchio_finalize_records.                                            */
+int b200_pinocchio_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const void* d_px, size_t npx, void* d_out,
+                                void* stream);
+/* snark.GenerateProofs fed from the witness: the quotient is computed on the device from the resident R1CS and never
+ * leaves HBM; otherwise identical to b200_pinocchio_prove with px = CombinePolynomials(w, R1CSToQAP(a, b, c)).  When
+ * len(Z) = n + 1 and n >= 2 the quotient h = DivisorPolynomial(px, Z) is computed without forming px (C w is not needed);
+ * any other len(Z) takes px (b200_qap_px) and the key's division.  Like the reference it drops the remainder, so a witness
+ * that does not satisfy the R1CS gets the proof b200_pinocchio_prove gives for that witness and its px (which does not
+ * verify).  The front end runs on the stream the G1T MSM runs on, beside the seven witness MSMs.  nw must equal the key's
+ * m and the R1CS's m.  Unlike b200_pinocchio_prove it waits with the library mutex released, so two host threads proving
+ * on keys of contexts 0 and 1 overlap, also when both keys share one R1CS handle.  A witness entry >= r gives B200_ERANGE
+ * from the key's own error word; the outputs are left untouched and the next call starts from a clear word.  A sharded
+ * key needs a matching communicator (SPMD, the proof is returned on every rank); without one the call returns
+ * B200_EINVAL — use b200_pinocchio_prove_witness_device + b200_pinocchio_finalize_records instead.                      */
+int b200_pinocchio_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, uint64_t* out_g1,
+                                 uint64_t pi_b[24]);
+/* b200_pinocchio_prove_witness from a DEVICE-resident witness (m standard-form scalars), the result left in device
+ * memory on `stream` as in b200_pinocchio_prove_device.
+ *   - No host synchronisation, except on the FIRST call for a given (R1CS, prove context) pair: that call builds the
+ *     R1CS's interpolation domains (shared by both contexts) and the context's workspace, and may synchronise.
+ *   - Proofs on keys of the two prove contexts may be in flight together on two streams, also on one R1CS handle (each
+ *     context has its own workspace on the R1CS, which a Groth16 key of that context shares).
+ *   - A witness entry >= r is read as 0 and reported by no call, as in b200_pinocchio_prove_device.
+ *   - A bad handle, a null pointer, nw different from the key's m or the R1CS's m, or an R1CS whose quotient does not fit
+ *     the key (len(px) = 2n - 1 < len(Z), len(hx) > len(G1T)) returns B200_EINVAL.
+ *   - On a sharded key only the rank that holds G1T runs the QAP front end (on the whole witness); every other rank
+ *     launches no QAP kernel.  Without a matching communicator d_out receives the rank's 2 KB record.                   */
+int b200_pinocchio_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, void* d_out,
+                                        void* stream);
+/* k witness-fed Pinocchio proofs under one key in one set of launches.  Proof p is the group-element octuple that
+ * b200_pinocchio_prove_witness(_device) returns for w_p, satisfied witness or not (compare affine: the Jacobian
+ * representatives may differ).  Witness p is at w + p*nw*4 words; outputs: out_g1 k x 84, pi_b k x 24 words.
+ *   - Three batched sorts, eight batched bucket phases (b200_msm_device_batch), whatever k.  The scalar vectors of the
+ *     seven witness MSMs are the witnesses where they lie: one sort of w_p (stride nw) serves B, Bp, C, Cp, Kp, one of
+ *     w_p[NPublic+1..) serves A, Ap, one of the k quotient vectors serves G1T; one kernel writes the k proofs.
+ *   - len(Z) = n + 1, n >= 2 (the h-direct shape): the k quotients come from one batched front end, so a batch issues the
+ *     launches of a batch of one, plus the documented extras of b200_msm_device_batch.  Any other len(Z) takes px and the
+ *     division like the single entry, once per witness: correct, but not batched.
+ *   - Waits with the library mutex released; batches on keys of contexts 0 and 1 may be in flight together, also on one
+ *     R1CS handle.
+ *   - Scratch: about k times one proof's sort, bucket and front-end scratch.  The key's (counted by b200_pk_device_bytes:
+ *     quotient vectors, records, the eight sets' batch sorts and bucket phases) and the R1CS workspace's are allocated on
+ *     the first batch and grown (never shrunk) by a larger one, which first waits for the previous batch; the pinned
+ *     landing area of this entry holds k*108 + 1 words.
+ *   - B200_EINVAL before anything is allocated or enqueued: k = 0, a bad handle or null pointer, the size mismatches of
+ *     the single entry, a sharded key, or a batch too large for 32-bit indexing: k*ceil(255/c)*terms sort entries (or k
+ *     times a set's buckets) of any of the eight sets reaching 2^31, or 3k*2N >= 2^32 transform elements (N = the power
+ *     of two >= n).
+ *   - B200_ERANGE: a witness entry >= r in any witness (the outputs are left untouched, and the next call starts from a
+ *     clear error word). */
+int b200_pinocchio_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, size_t k,
+                                       uint64_t* out_g1, uint64_t* pi_b);
+/* b200_pinocchio_prove_witness_batch from device memory: d_w holds the k witnesses (standard form, witness p at
+ * d_w + p*nw*32 bytes), d_out receives k x 108 u64 on `stream`, proof p at d_out + 108p.  No host synchronisation, except
+ * in a call that first meets a given (R1CS, prove context) pair or grows a scratch; a regrowth waits for an event
+ * recorded behind the key's previous batch, not for the device.  A witness entry >= r is read as 0 and reported by no
+ * call; the other errors are those of the host entry. */
+int b200_pinocchio_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                              void* d_out, void* stream);
+
 /* ---- element-wise group operations, reference formulas (X,Y,Z-exact) ------------------- */
 /* bn128.G1.Add / Double / Neg / Affine (bn128/g1.go:32-170) and the G2 twins (bn128/g2.go:32-200), n independent
  * operations per call.  Affine writes (x, y) per point, infinity as (0, 0) like G1.Affine.                            */
