@@ -146,6 +146,18 @@ def build_host_pinocchio_batch(force=False):
     return target
 
 
+def build_host_shard_batch(force=False):
+    """g++ build of the kernels of batched proving on key shards (k_groth16_finalize_batch, k_quotient_store with a
+    source offset, k_pinocchio_gather_finalize_batch) over csrc/host_stub (CPU test vehicle, tests/test_host_shard_batch.py)."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    target = os.path.join(LIBDIR, "libb200_host_shard_batch.so")
+    if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):
+        return target
+    _run(["g++", "-O2", "-std=c++17", "-pthread", "-x", "c++", "-shared", "-fPIC", "-Wno-psabi", "-I", os.path.join(HOSTTEST, "host_stub"),
+          "-I", HOSTTEST, "-I", CSRC, "-o", target, os.path.join(HOSTTEST, "shard_batch_test.cpp")])
+    return target
+
+
 def build_shard_partition(force=False):
     """g++ build of csrc/shard_partition.h behind a C entry point (CPU test vehicle, tests/test_shard_partition.py)."""
     os.makedirs(LIBDIR, exist_ok=True)

@@ -101,11 +101,15 @@ _SIGNATURES = {
     "b200_groth16_prove_witness_device": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_groth16_prove_witness_batch": [_h, _h, _vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp],
     "b200_groth16_prove_witness_batch_device": [_h, _h, _vp, _sz, _sz, _vp, _vp, _vp, _vp],
+    "b200_groth16_prove_witness_batch_partial_device": [_h, _h, _vp, _sz, _sz, _vp, _vp, _vp, _vp],
+    "b200_groth16_finalize_batch_device": [_h, _vp, _int, _sz, _vp, _vp],
     "b200_pinocchio_prove_device": [_h, _vp, _sz, _vp, _sz, _vp, _vp],
     "b200_pinocchio_prove_witness": [_h, _h, _vp, _sz, _vp, _vp],
     "b200_pinocchio_prove_witness_device": [_h, _h, _vp, _sz, _vp, _vp],
     "b200_pinocchio_prove_witness_batch": [_h, _h, _vp, _sz, _sz, _vp, _vp],
     "b200_pinocchio_prove_witness_batch_device": [_h, _h, _vp, _sz, _sz, _vp, _vp],
+    "b200_pinocchio_prove_witness_batch_record_device": [_h, _h, _vp, _sz, _sz, _vp, _vp],
+    "b200_pinocchio_finalize_records_batch_device": [_vp, _int, _sz, _vp, _vp],
     "b200_profile": [_int],
     "b200_profile_read": [ctypes.POINTER(ctypes.c_double)],
 }

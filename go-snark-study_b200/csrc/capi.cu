@@ -25,6 +25,7 @@
 #include "shard_partition.h"
 #include "glv.cuh"
 #include "pinocchio_batch.cuh"
+#include "shard_batch.cuh"
 #ifndef B200_NO_PAIRING
 #include "pairing.cuh"
 #include "pairing_warp.cuh"
@@ -106,12 +107,16 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+// A failed allocation is not sticky, but the runtime keeps it as its last error: it is cleared here, so that the next
+// call's cudaGetLastError() after a launch does not report it (a batch that did not fit would fail every later key load).
 #define CU(call)                                                                             \
   do {                                                                                       \
     cudaError_t e_ = (call);                                                                 \
-    if (e_ != cudaSuccess)                                                                   \
+    if (e_ != cudaSuccess) {                                                                 \
+      if (e_ == cudaErrorMemoryAllocation) cudaGetLastError();                               \
       return fail(e_ == cudaErrorMemoryAllocation ? B200_ENOMEM : B200_ECUDA, "%s:%d %s: %s", \
                   __FILE__, __LINE__, #call, cudaGetErrorString(e_));                        \
+    }                                                                                        \
   } while (0)
 
 #define NEED_INIT()                                                                      \
@@ -312,6 +317,20 @@ int check_err_flag(const char* what, int* d_err, cudaStream_t st = nullptr, std:
   return B200_OK;
 }
 
+// The window shape of a base set of n points with c-bit windows, t = B200_CFG_TABLE_WINDOWS as it was at the set's load.
+MsmShape msm_shape(size_t n, int c, int t) {
+  MsmShape sh{};
+  sh.n = (uint32_t)n;
+  sh.c = (uint32_t)c;
+  sh.nwin = (255 + c - 1) / c;
+  sh.nbuckets = 1u << (c - 1);
+  sh.table_stride = (uint32_t)n;
+  // B200_CFG_TABLE_WINDOWS: keep t of the nwin window rows; window w reads row w mod t and feeds bucket group w / t
+  sh.rows = t > 0 && (uint32_t)t < sh.nwin ? (uint32_t)t : sh.nwin;
+  sh.groups = (sh.nwin + sh.rows - 1) / sh.rows;
+  return sh;
+}
+
 // prefer_affine: batched-affine bucket accumulation (6 multiplies per add instead of 10) whenever the buckets are
 // populated enough to amortise its per-round launches; since the per-round inversion became a binary-Euclid warp
 // it also wins for a stand-alone MSM.  A proving-key
@@ -324,15 +343,8 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   auto b = std::make_unique<Bases>();
   b->group = group;
   b->n = n;
+  b->sh = msm_shape(n, c, g_table_windows);
   MsmShape& sh = b->sh;
-  sh.n = (uint32_t)n;
-  sh.c = (uint32_t)c;
-  sh.nwin = (255 + c - 1) / c;
-  sh.nbuckets = 1u << (c - 1);
-  sh.table_stride = (uint32_t)n;
-  // B200_CFG_TABLE_WINDOWS: keep t of the nwin window rows; window w reads row w mod t and feeds bucket group w / t
-  sh.rows = g_table_windows > 0 && (uint32_t)g_table_windows < sh.nwin ? (uint32_t)g_table_windows : sh.nwin;
-  sh.groups = (sh.nwin + sh.rows - 1) / sh.rows;
   const bool reduced = sh.rows < sh.nwin;
   if ((uint64_t)sh.nwin * n >= (1ull << 31)) return fail(B200_EINVAL, "nwin*n exceeds 2^31 entries");
   CU(b->table.alloc((size_t)sh.rows * n * sizeof(Affine<F>)));
@@ -651,9 +663,10 @@ int msm_enqueue(Bases* b, const Fr* d_scalars, size_t n, int mont, XYZZ<F>* d_ou
 // Term i of vector p is scalar p*stride + i times base i; vector p's digits go to its own window groups, so one recode,
 // one counting sort, one accumulation and one tail serve all k vectors.  Populations per bucket, and so the slice cap,
 // the lanes per bucket and the accumulation kernel, are those of one vector.
-bool batch_fits(const Bases* b, size_t k, size_t n) {
-  return (uint64_t)k * b->sh.nwin * n < (1ull << 31) && (uint64_t)k * total_buckets(b->sh) + 3 < (1ull << 31);
+bool batch_fits(const MsmShape& sh, size_t k, size_t n) {
+  return (uint64_t)k * sh.nwin * n < (1ull << 31) && (uint64_t)k * total_buckets(sh) + 3 < (1ull << 31);
 }
+bool batch_fits(const Bases* b, size_t k, size_t n) { return batch_fits(b->sh, k, n); }
 
 // The batch scratch of `b` for k vectors of n terms: allocated on the first batch, regrown to the larger of the old and
 // the new capacity in each dimension when a batch exceeds it.  Before the old buffers are freed the host waits for the
@@ -858,25 +871,42 @@ int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t
 // Proof p is the proof of groth16_witness_enqueue for (w_p, r_p, s_p).  The four MSMs run as batched MSMs over k scalar
 // vectors (W_p = w_p ++ [1, r_p, s_p] for A, B1, B2 with one shared sort; C||PTD_p), the h-direct quotients as one batched
 // front end (qap_h_batch_enqueue), the blinding products with one warp per proof: the launches of one proof, whatever k.
+// On a key shard every vector is the rank's part of it (G16Slices), and the batch ends in k partial records.
 
-// Everything that is refused before anything is allocated or enqueued.
+// Everything that is refused before anything is allocated or enqueued.  On a key shard every refusal is decided on
+// values every rank of the shard shares (the arguments, the R1CS, every rank's cut), so all ranks return the same code
+// and none is left waiting in the all-gather of its peers.
 int groth16_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_t k, const uint64_t* r, const uint64_t* s,
                         const char* what) {
   if (k == 0) return fail(B200_EINVAL, "%s: k = 0", what);
   if (nw != pk->m || nw != r1->m) return fail(B200_EINVAL, "%s: witness length %zu, NVars %zu, R1CS columns %zu", what, nw, pk->m, r1->m);
-  if (pk->world != 1) return fail(B200_EINVAL, "%s: sharded key (rank %d/%d): batches need an unsharded key", what, pk->rank, pk->world);
   const size_t npx = 2 * r1->n - 1;
   if (npx < pk->Z.nb) return fail(B200_EINVAL, "%s: len(px) < len(Z)", what);
   if (npx - pk->Z.nb + 1 > pk->n_h_bases)
     return fail(B200_EINVAL, "%s: len(hx)=%zu exceeds len(PowersTauDelta)=%zu", what, npx - pk->Z.nb + 1, pk->n_h_bases);
   const size_t terms[4] = {pk->m + 3, pk->m + 3, pk->m + 3, pk->n_c_full + pk->n_h_bases + 1};
-  for (int j = 0; j < 4; j++)
-    if (!pk->g[j] || !batch_fits(pk->g[j].get(), k, terms[j]))
-      return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
-                  pk->g[j] ? pk->g[j]->sh.nwin : 0u, terms[j], j);
+  if (pk->world == 1) {
+    for (int j = 0; j < 4; j++)
+      if (!pk->g[j] || !batch_fits(pk->g[j].get(), k, terms[j]))
+        return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
+                    pk->g[j] ? pk->g[j]->sh.nwin : 0u, terms[j], j);
+  } else {   // the largest part any rank holds: the shape each rank's set was built with, from its cut
+    for (int g = 0; g < pk->world; g++) {
+      const G16Slices sl = g16_slices(pk, g);
+      for (int j = 0; j < 4; j++) {
+        const size_t n = sl.terms[j];
+        if (!n) continue;
+        const MsmShape sh = msm_shape(n, pk->window_bits ? pk->window_bits : pick_window_bits(n), pk->table_windows);
+        if (!batch_fits(sh, k, n))
+          return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d on rank %d/%d exceed 2^31",
+                      what, k, sh.nwin, n, j, g, pk->world);
+      }
+    }
+  }
   const uint64_t N = pow2_at_least(r1->n);
   if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
-  // the scalar vectors are laid out by 2-D copies whose row pitch (one vector) the device bounds
+  // the scalar vectors are laid out by 2-D copies whose row pitch (one vector, one witness) the device bounds; the
+  // unsharded widths bound every rank's
   int max_pitch = 0;
   CU(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, g_device));
   const uint64_t widest = std::max(terms[0], terms[3]) * sizeof(Fr);
@@ -889,14 +919,33 @@ int groth16_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_t 
   return B200_OK;
 }
 
-// d_w: k witnesses (device, standard form, witness p at d_w + p*m); r, s: host, k x 4 limbs; d_out: k x 48 u64, proof p at
-// d_out + 48p (PiA | PiC | PiB).  After groth16_batch_check.  No host synchronisation unless a scratch grows (or the
-// first batch on this R1CS and context builds its domains).
-int groth16_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const uint64_t* r, const uint64_t* s, Fq* d_out,
-                          cudaStream_t st, int* err) {
-  const size_t m = pk->m, l1 = pk->npublic + 1, n_c_full = pk->n_c_full, n_ptd = pk->n_h_bases;
-  const size_t mw = m + 3, nch = n_c_full + n_ptd + 1, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
+// A sharded key whose batches end in the all-gather: a communicator of the key's world (its rank checked by the caller).
+bool groth16_gathers(const ProvingKey* pk) { return pk->world > 1 && comm_active() && g_comm.world == pk->world; }
+
+// The entries that return proofs: a sharded key needs its communicator (checked before anything is enqueued).
+int groth16_batch_comm_check(const ProvingKey* pk, const char* what) {
+  if (pk->world == 1) return B200_OK;
+  if (!groth16_gathers(pk))
+    return fail(B200_EINVAL, "%s: sharded key (rank %d/%d) without a matching communicator: call b200_comm_init, or use "
+                             "b200_groth16_prove_witness_batch_partial_device + b200_groth16_finalize_batch_device around "
+                             "your own all-gather", what, pk->rank, pk->world);
+  if (g_comm.rank != pk->rank) return fail(B200_EINVAL, "%s: key shard %d on communicator rank %d", what, pk->rank, g_comm.rank);
+  return B200_OK;
+}
+
+// d_w: k witnesses (device, standard form, witness p at d_w + p*m); r, s: host, k x 4 limbs.  d_recs null (one GPU only):
+// k proofs at d_proofs + 48p (u64, PiA | PiC | PiB).  Else k partial records of this rank at d_recs + 1 KB * p.  After
+// groth16_batch_check.  No host synchronisation unless a scratch grows (or the first batch on this R1CS and context
+// builds its domains).  Records no `done` event (groth16_batch_enqueue does, behind what reads the records).
+int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const uint64_t* r, const uint64_t* s,
+                        Fq* d_proofs, uint8_t* d_recs, cudaStream_t st, int* err, R1csBatch** fb_used) {
+  const size_t m = pk->m, l1 = pk->npublic + 1, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
   const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as groth16_witness_enqueue
+  const G16Slices sl = g16_slices(pk, pk->rank);
+  size_t woff[3];
+  g16_w_layout(pk, sl, woff);
+  const size_t nch = sl.terms[3], n_c = sl.n_c, n_p = sl.n_p;
+  const bool quotient = pk->g[3] && pk_needs_px(pk);   // only a rank that holds PowersTauDelta indices runs the front end
   // host: {1, r_p, s_p, -r_p s_p} and the GLV splits of (s_p, r_p)
   std::vector<Fr> small(4 * k);
   std::vector<GlvScalars> glv(k);
@@ -912,19 +961,25 @@ int groth16_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, con
       return fail(B200_EINVAL, "groth16_prove_witness_batch: GLV decomposition out of range");
   }
   // every scratch first: growing one waits for the batch that used it last, so nothing of this batch is enqueued yet
-  R1csWork* ws;
-  int rc = r1cs_work(r1, pk->ctx, &ws);
-  if (rc) return rc;
+  R1csWork* ws = nullptr;
   R1csBatch* fb = nullptr;
-  if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+  int rc;
+  if (quotient) {
+    if ((rc = r1cs_work(r1, pk->ctx, &ws))) return rc;
+    if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+  }
+  *fb_used = fb;
   if ((rc = groth16_batch_scratch(pk, k, false))) return rc;
   for (int j = 0; j < 3; j++) {
+    if (!pk->g[j]) continue;
     const bool own = pk->sort_src[j] == j;
-    rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, (uint32_t)mw, own) : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)mw, own);
+    const uint32_t n = (uint32_t)sl.terms[j];
+    rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, n, own) : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, n, own);
     if (rc) return rc;
   }
-  if ((rc = batch_scratch<Fq>(pk->g[3].get(), (uint32_t)k, (uint32_t)nch))) return rc;
+  if (pk->g[3] && (rc = batch_scratch<Fq>(pk->g[3].get(), (uint32_t)k, (uint32_t)nch))) return rc;
   for (int j = 0; j < 3; j++) {   // a set that reuses another's sort was sized for the same slices (msm_buckets' check)
+    if (!pk->g[j]) continue;
     const Bases* a = pk->g[j].get();
     const Bases* src = pk->g[pk->sort_src[j]].get();
     if (a->sort.max_slices != src->sort.max_slices || a->affine_S != src->affine_S || a->batch->vecs != src->batch->vecs ||
@@ -947,68 +1002,126 @@ int groth16_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, con
   const size_t F = sizeof(Fr);
   CU(cudaMemcpyAsync(rs, small.data(), 4 * k * F, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(b.glv.p, glv.data(), k * sizeof(GlvScalars), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpy2DAsync(W, mw * F, d_w, m * F, m * F, k, cudaMemcpyDeviceToDevice, st));          // W_p = w_p ++
-  CU(cudaMemcpy2DAsync(W + m, mw * F, rs, 4 * F, 3 * F, k, cudaMemcpyDeviceToDevice, st));       //       [1, r_p, s_p]
-  if (n_c_full) CU(cudaMemcpy2DAsync(CH, nch * F, d_w + l1, m * F, n_c_full * F, k, cudaMemcpyDeviceToDevice, st));
-  EV_REC(e_in, st);
-  // --- side stream 3: the quotients into the C||PTD vectors, then the C||PTD MSMs
-  EV_WAIT(s3, e_in);
-  PolyCtx& pc = *pk->pctx().poly;
-  Fr* chq = CH + n_c_full;
-  const uint32_t qtotal = (uint32_t)(k * (n_ptd + 1));
-  if (h_direct) {
-    if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
-    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)n_ptd,
-                                                        rs + 3, 4, qtotal, chq, (uint32_t)nch);
-  } else {   // not batched: the single-witness px and division of each witness, straight into its vector
-    for (size_t p = 0; p < k; p++) {
-      if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
-      CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, chq + p * nch, nullptr, err, s3));
-    }
-    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)n_ptd, rs + 3, 4, qtotal, chq, (uint32_t)nch);
+  // a shard's sets it does not hold, and its products when it holds no part of A or B1, stay at infinity
+  if (pk->world > 1) CU(cudaMemsetAsync(b.rec.p, 0, b.rec.bytes, st));
+  for (int j = 0; j < 3; j++) {    // W_p = w_p[lo_j, hi_j) ++ [1, r_p, s_p] (the latter with set j's tail)
+    if (!pk->g[j] || pk->sort_src[j] != j) continue;
+    const size_t nt = sl.terms[j], cnt = sl.hi[j] - sl.lo[j];
+    Fr* Wj = W + k * woff[j];
+    if (cnt) CU(cudaMemcpy2DAsync(Wj, nt * F, d_w + sl.lo[j], m * F, cnt * F, k, cudaMemcpyDeviceToDevice, st));
+    if (sl.tail[j]) CU(cudaMemcpy2DAsync(Wj + cnt, nt * F, rs, 4 * F, 3 * F, k, cudaMemcpyDeviceToDevice, st));
   }
-  g_launches += 1;
-  Bases* gch = pk->g[3].get();
-  MsmShape sh = gch->sh;
-  sh.vecs = (uint32_t)k;
-  sh.vec_stride = (uint32_t)nch;
-  if ((rc = msm_sort(gch->batch->sort, sh, CH, nch, 0, err, s3, gch->batch->scan_totals.as<unsigned long long>()))) return rc;
-  if ((rc = bucket_phase<Fq>(gch, gch->batch->sort, gch->batch->bk, (uint32_t)k, nch, rCH, s3))) return rc;
+  if (pk->g[3] && n_c) CU(cudaMemcpy2DAsync(CH, nch * F, d_w + l1 + sl.c_lo, m * F, n_c * F, k, cudaMemcpyDeviceToDevice, st));
+  EV_REC(e_in, st);
+  // --- side stream 3: the quotients into the C||PTD vectors (h_p[p_lo, p_lo + n_p), zeros beyond len(h), -r_p s_p with
+  // the tail), then the C||PTD MSMs
+  EV_WAIT(s3, e_in);
+  if (quotient) {
+    PolyCtx& pc = *pk->pctx().poly;
+    Fr* chq = CH + n_c;
+    const uint32_t qtotal = (uint32_t)(k * (n_p + 1));
+    const Fr* tail = sl.tail[3] ? rs + 3 : nullptr;
+    if (h_direct) {
+      if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
+      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)n_p,
+                                                          tail, 4, qtotal, chq, (uint32_t)nch, (uint32_t)sl.p_lo);
+    } else {   // not batched: the single-witness px and division of each witness, into its vector (a shard: its slice)
+      const bool direct = sl.p_lo == 0 && nq <= n_p;
+      const size_t have = nq > sl.p_lo ? std::min(nq - sl.p_lo, n_p) : 0;   // quotient coefficients inside the slice
+      for (size_t p = 0; p < k; p++) {
+        if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
+        CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, direct ? chq + p * nch : pk->h_full.as<Fr>(), nullptr, err, s3));
+        if (!direct && have)
+          CU(cudaMemcpyAsync(chq + p * nch, pk->h_full.as<Fr>() + sl.p_lo, have * F, cudaMemcpyDeviceToDevice, s3));
+      }
+      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)n_p, tail, 4, qtotal, chq,
+                                                          (uint32_t)nch, (uint32_t)sl.p_lo);
+    }
+    g_launches += 1;
+  }
+  MsmShape sh;
+  if (Bases* gch = pk->g[3].get()) {
+    sh = gch->sh;
+    sh.vecs = (uint32_t)k;
+    sh.vec_stride = (uint32_t)nch;
+    if ((rc = msm_sort(gch->batch->sort, sh, CH, nch, 0, err, s3, gch->batch->scan_totals.as<unsigned long long>()))) return rc;
+    if ((rc = bucket_phase<Fq>(gch, gch->batch->sort, gch->batch->bk, (uint32_t)k, nch, rCH, s3))) return rc;
+  }
   EV_REC(e_ch, s3);
-  // --- A, B1, B2: one batched sort of W on the main stream, the bucket phases on st / s1 / s2 (B2 first: the longest)
+  // --- A, B1, B2: one batched sort per distinct slice on the main stream, the bucket phases on st / s1 / s2 (B2 first:
+  // the longest)
   for (int j = 0; j < 3; j++) {
-    if (pk->sort_src[j] != j) continue;
+    if (!pk->g[j] || pk->sort_src[j] != j) continue;
     Bases* g = pk->g[j].get();
     sh = g->sh;
     sh.vecs = (uint32_t)k;
-    sh.vec_stride = (uint32_t)mw;
-    if ((rc = msm_sort(g->batch->sort, sh, W, mw, 0, err, st, g->batch->scan_totals.as<unsigned long long>()))) return rc;
+    sh.vec_stride = (uint32_t)sl.terms[j];
+    if ((rc = msm_sort(g->batch->sort, sh, W + k * woff[j], sl.terms[j], 0, err, st, g->batch->scan_totals.as<unsigned long long>()))) return rc;
     EV_REC(e_sorted[j], st);
   }
   cudaStream_t sk[3] = {st, s1, s2};
   for (int j = 2; j >= 0; j--) {
+    if (!pk->g[j]) continue;
     const int src = pk->sort_src[j];
     const SortScratch& ss = pk->g[src]->batch->sort;
     Bases* g = pk->g[j].get();
     if (sk[j] != st) EV_WAIT(sk[j], e_sorted[src]);
-    if (j == 2) rc = bucket_phase<Fq2>(g, ss, g->batch->bk, (uint32_t)k, mw, rB2, sk[2]);
-    else rc = bucket_phase<Fq>(g, ss, g->batch->bk, (uint32_t)k, mw, j ? rB1 : rA, sk[j]);
+    if (j == 2) rc = bucket_phase<Fq2>(g, ss, g->batch->bk, (uint32_t)k, sl.terms[j], rB2, sk[2]);
+    else rc = bucket_phase<Fq>(g, ss, g->batch->bk, (uint32_t)k, sl.terms[j], j ? rB1 : rA, sk[j]);
     if (rc) return rc;
   }
   EV_REC(e_a, st);
   EV_REC(e_b1, s1);
   EV_REC(e_b2, s2);
-  // s_p * A_p and r_p * B1_p on side stream 1, one warp per proof, while B2 / C||PTD still run
+  // s_p * A_p and r_p * B1_p on side stream 1, one warp per proof, while B2 / C||PTD still run; a shard that holds no
+  // part of A or B1 skips them (its products are infinity, as in groth16_enqueue)
   EV_WAIT(s1, e_a);
-  k_groth16_products_batch<<<(unsigned)k, 32, 0, s1>>>(rA, rB1, b.glv.as<GlvScalars>(), prod);
+  if (pk->g[0] || pk->g[1]) {
+    k_groth16_products_batch<<<(unsigned)k, 32, 0, s1>>>(rA, rB1, b.glv.as<GlvScalars>(), prod);
+    g_launches += 1;
+  }
   EV_REC(e_prod, s1);
   EV_WAIT(st, e_prod);
   EV_WAIT(st, e_b2);
   EV_WAIT(st, e_ch);
-  k_groth16_combine_batch<<<nblk(3 * k, 96), 96, 0, st>>>(rA, rB2, rCH, prod, (uint32_t)k, d_out);
-  g_launches += 2;
+  if (!d_recs) {
+    k_groth16_combine_batch<<<nblk(3 * k, 96), 96, 0, st>>>(rA, rB2, rCH, prod, (uint32_t)k, d_proofs);
+  } else {   // fold the products into each proof's C part: k partial records
+    CU(cudaMemsetAsync(d_recs, 0, k * kPartialBytes, st));
+    k_groth16_fold_products_batch<<<nblk(k, 64), 64, 0, st>>>(rA, rB1, rB2, rCH, prod, (uint32_t)k, d_recs);
+  }
+  g_launches += 1;
   CU(cudaGetLastError());
+  return B200_OK;
+}
+
+// The k proofs of a batch at d_out + 48p (u64), or with `records` this rank's k partial records at d_out + 1 KB * p.  A
+// sharded key without `records` computes its records, all-gathers them (k records per rank, on the key's prove-context
+// communicator, on `st`) and finalises: every rank receives the k proofs.  After groth16_batch_check and, without
+// `records`, groth16_batch_comm_check.  Once the records' scratch exists the all-gather runs whatever else fails, so no
+// peer is left waiting; the error is then returned and nothing is finalised.
+int groth16_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const uint64_t* r, const uint64_t* s, Fq* d_out,
+                          bool records, cudaStream_t st, int* err) {
+  int rc;
+  R1csBatch* fb = nullptr;   // the front end's scratch, if the batch used it
+  if (pk->world == 1 || records) {
+    rc = groth16_batch_parts(pk, r1, d_w, k, r, s, d_out, records ? reinterpret_cast<uint8_t*>(d_out) : nullptr, st, err, &fb);
+  } else {
+    if ((rc = groth16_batch_scratch(pk, k, false))) return rc;
+    CU(pk->gather.ensure(kPartialBytes * k * (size_t)pk->world));
+    ProveBatch& b = *pk->batch;
+    rc = groth16_batch_parts(pk, r1, d_w, k, r, s, nullptr, b.parts.as<uint8_t>(), st, err, &fb);
+    ncclResult_t nrc = g_comm.api.AllGather(b.parts.p, pk->gather.p, kPartialBytes * k, ncclUint8, pk->pctx().comm, st);
+    if (rc) return rc;
+    if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
+    k_groth16_finalize_batch<<<groth16_finalize_blocks((uint32_t)k), kG16FinalizeBlock, 0, st>>>(pk->gather.as<uint8_t>(), pk->world,
+                                                                                                   (uint32_t)k, d_out);
+    g_launches += 1;
+    CU(cudaGetLastError());
+  }
+  if (rc) return rc;
   // behind everything of this batch: what the next regrowth of any of its scratches waits for
+  ProveBatch& b = *pk->batch;
   EV_REC(b.done, st);
   for (const auto& g : pk->g)
     if (g && g->batch) EV_REC(g->batch->done, st);
@@ -1025,12 +1138,15 @@ int groth16_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, 
   if (!w || !r || !s || !pi_a || !pi_b || !pi_c) return fail(B200_EINVAL, "%s: null pointer", what);
   int rc = groth16_batch_check(pk, r1, nw, k, r, s, what);
   if (rc) return rc;
+  if ((rc = groth16_batch_comm_check(pk, what))) return rc;
   if ((rc = groth16_batch_scratch(pk, k, true))) return rc;
   ProveBatch& b = *pk->batch;
   cudaStream_t st = pk->pctx().main;
-  CU(cudaMemcpyAsync(b.w_stage.p, w, k * nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  // a shard that runs no QAP front end reads only its witness ranges
+  if (pk->world == 1) CU(cudaMemcpyAsync(b.w_stage.p, w, k * nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  else if ((rc = stage_witness(pk, w, pk_needs_px(pk), st, b.w_stage.as<Fr>(), k))) return rc;
   Fq* o = b.out.as<Fq>();
-  if ((rc = groth16_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, r, s, o, st, pk->d_err_sync.as<int>()))) return rc;
+  if ((rc = groth16_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, r, s, o, false, st, pk->d_err_sync.as<int>()))) return rc;
   // as finish_host_proof, for k proofs: the wait runs with the library mutex released
   CU(cudaMemcpyAsync(b.h_out, o, k * kBatchProofWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(b.h_out + k * kBatchProofWords));
@@ -1105,39 +1221,71 @@ int pinocchio_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size
 // Sets whose batches share one digit sort (the set's own index: it sorts), as the groups of pinocchio_enqueue.
 constexpr int kPinSortSrc[8] = {0, 0, 2, 2, 2, 2, 2, 7};
 
+// Everything refused before anything is allocated or enqueued.  On a key shard the sets' sizes are the same on every rank
+// (whole MSMs are dealt) and every set is checked with the shape its owner built it with, so every rank of the shard
+// returns the same code.
 int pinocchio_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_t k, const char* what) {
   if (k == 0) return fail(B200_EINVAL, "%s: k = 0", what);
   int rc = pinocchio_witness_check(pk, r1, nw, what);
   if (rc) return rc;
-  if (pk->world != 1) return fail(B200_EINVAL, "%s: sharded key (rank %d/%d): batches need an unsharded key", what, pk->rank, pk->world);
   const size_t ma = pk->m - pk->npublic - 1;
   const size_t terms[8] = {ma, ma, pk->m, pk->m, pk->m, pk->m, pk->m, pk->n_h_bases};
-  for (int j = 0; j < 8; j++)
-    if (pk->g[j] && !batch_fits(pk->g[j].get(), k, terms[j]))
-      return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
-                  pk->g[j]->sh.nwin, terms[j], j);
+  for (int j = 0; j < 8; j++) {
+    if (pk->world == 1) {
+      if (pk->g[j] && !batch_fits(pk->g[j].get(), k, terms[j]))
+        return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
+                    pk->g[j]->sh.nwin, terms[j], j);
+    } else if (terms[j]) {
+      const MsmShape sh = msm_shape(terms[j], pk->window_bits ? pk->window_bits : pick_window_bits(terms[j]), pk->table_windows);
+      if (!batch_fits(sh, k, terms[j]))
+        return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
+                    sh.nwin, terms[j], j);
+    }
+  }
   const uint64_t N = pow2_at_least(r1->n);
   if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
   return B200_OK;
 }
 
-// d_w: k witnesses (device, standard form, witness p at d_w + p*m); d_out: k x 108 u64, proof p at d_out + 108p (the seven
-// G1 points, then PiB).  After pinocchio_batch_check.  No host synchronisation unless a scratch grows (or the first batch
-// on this R1CS and context builds its domains).
-int pinocchio_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq* d_out, cudaStream_t st, int* err) {
+// The entries that return proofs: a sharded key needs its communicator (checked before anything is enqueued).
+int pinocchio_batch_comm_check(const ProvingKey* pk, const char* what) {
+  if (pk->world == 1 || pinocchio_gathers(pk)) return B200_OK;
+  return fail(B200_EINVAL, "%s: sharded key (rank %d/%d) without a matching communicator: call b200_comm_init, or use "
+                           "b200_pinocchio_prove_witness_batch_record_device + b200_pinocchio_finalize_records_batch_device "
+                           "around your own all-gather", what, pk->rank, pk->world);
+}
+
+// d_w: k witnesses (device, standard form, witness p at d_w + p*m).  d_recs null (one GPU only): k proofs at d_out + 108p
+// (u64: the seven G1 points, then PiB).  Else this rank's k records at d_recs + 2 KB * p, the slots of sets it does not
+// own at infinity.  A key shard runs only the sets it owns (pinocchio_owners): a sort group whose sorting set lives on
+// another rank is sorted by its first owned member, and only the G1T owner runs the QAP front end.  After
+// pinocchio_batch_check.  No host synchronisation unless a scratch grows (or the first batch on this R1CS and context
+// builds its domains).  Records no `done` event (pinocchio_batch_enqueue does, behind what reads the records).
+int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq* d_out, uint8_t* d_recs, cudaStream_t st,
+                          int* err, R1csBatch** fb_used) {
   const size_t m = pk->m, l1 = pk->npublic + 1, ng = pk->n_h_bases, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
   const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as pinocchio_witness_enqueue
   const size_t terms[8] = {m - l1, m - l1, m, m, m, m, m, ng};
+  // the set that sorts for set j: the first set of j's group (kPinSortSrc) this key holds
+  int src[8];
+  for (int j = 0; j < 8; j++) {
+    src[j] = -1;
+    for (int q = 0; q < 8 && src[j] < 0; q++)
+      if (kPinSortSrc[q] == kPinSortSrc[j] && pk->g[q]) src[j] = q;
+  }
   // every scratch first: growing one waits for the batch that used it last, so nothing of this batch is enqueued yet
-  R1csWork* ws;
-  int rc = r1cs_work(r1, pk->ctx, &ws);
-  if (rc) return rc;
+  R1csWork* ws = nullptr;
   R1csBatch* fb = nullptr;
-  if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+  int rc;
+  if (pk->g[7]) {
+    if ((rc = r1cs_work(r1, pk->ctx, &ws))) return rc;
+    if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+  }
+  *fb_used = fb;
   if ((rc = pinocchio_batch_scratch(pk, k, false))) return rc;
   for (int j = 0; j < 8; j++) {
-    if (!pk->g[j]) continue;   // A, Ap of a circuit whose signals are all public
-    const bool own = kPinSortSrc[j] == j;
+    if (!pk->g[j]) continue;   // a set another rank owns, or A, Ap of a circuit whose signals are all public
+    const bool own = src[j] == j;
     rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own)
                 : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own);
     if (rc) return rc;
@@ -1145,11 +1293,11 @@ int pinocchio_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, F
   for (int j = 0; j < 8; j++) {   // a set that reuses another's sort was sized for the same slices (msm_buckets' check)
     if (!pk->g[j]) continue;
     const Bases* a = pk->g[j].get();
-    const Bases* src = pk->g[kPinSortSrc[j]].get();
-    if (a->sh.c != src->sh.c || a->sh.table_stride != src->sh.table_stride || a->sh.rows != src->sh.rows ||
-        a->sort.max_slices != src->sort.max_slices || a->affine_S != src->affine_S || a->batch->vecs != src->batch->vecs ||
-        a->batch->sort.sh.n != src->batch->sort.sh.n)
-      return fail(B200_EINVAL, "pinocchio_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, kPinSortSrc[j]);
+    const Bases* sb = pk->g[src[j]].get();
+    if (a->sh.c != sb->sh.c || a->sh.table_stride != sb->sh.table_stride || a->sh.rows != sb->sh.rows ||
+        a->sort.max_slices != sb->sort.max_slices || a->affine_S != sb->affine_S || a->batch->vecs != sb->batch->vecs ||
+        a->batch->sort.sh.n != sb->batch->sort.sh.n)
+      return fail(B200_EINVAL, "pinocchio_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, src[j]);
   }
   ProveBatch& b = *pk->batch;
   cudaStream_t side[3] = {pk->pctx().side[0], pk->pctx().side[1], pk->pctx().side[2]};
@@ -1166,57 +1314,107 @@ int pinocchio_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, F
   };
   auto buckets_of = [&](int j, cudaStream_t s) {
     Bases* g = pk->g[j].get();
-    const SortScratch& ss = pk->g[kPinSortSrc[j]]->batch->sort;
+    const SortScratch& ss = pk->g[src[j]]->batch->sort;
     if (j == 2) return bucket_phase<Fq2>(g, ss, g->batch->bk, (uint32_t)k, terms[j], rec2, s);
     return bucket_phase<Fq>(g, ss, g->batch->bk, (uint32_t)k, terms[j], rec1 + kPinSlot[j] * k, s);
   };
-  // sets the key does not hold (A, Ap when every signal is public) leave their records at infinity, as in pinocchio_enqueue
+  // sets the key does not hold (another rank's; A, Ap when every signal is public) leave their records at infinity, as in
+  // pinocchio_enqueue
   CU(cudaMemsetAsync(b.rec.p, 0, k * (7 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>)), st));
   EV_REC(e_in, st);
-  // --- side stream 3: the k quotients into the G1T scalar vectors (zero-filled to len(G1T)), then the G1T MSMs
+  // --- side stream 3 (the G1T owner): the k quotients into the G1T scalar vectors (zero-filled to len(G1T)), then the
+  // G1T MSMs
   cudaStream_t s3 = side[2];
-  if (s3 != st) EV_WAIT(s3, e_in);
-  PolyCtx& pc = *pk->pctx().poly;
-  Fr* H = b.CH.as<Fr>();
-  const uint32_t qtotal = (uint32_t)(k * (ng + 1));
-  if (h_direct) {
-    if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
-    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)ng,
-                                                        nullptr, 0, qtotal, H, (uint32_t)ng);
-  } else {   // not batched: the single-witness px and division of each witness, straight into its vector
-    for (size_t p = 0; p < k; p++) {
-      if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
-      CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, H + p * ng, nullptr, err, s3));
+  if (pk->g[7]) {
+    if (s3 != st) EV_WAIT(s3, e_in);
+    PolyCtx& pc = *pk->pctx().poly;
+    Fr* H = b.CH.as<Fr>();
+    const uint32_t qtotal = (uint32_t)(k * (ng + 1));
+    if (h_direct) {
+      if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
+      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)ng,
+                                                          nullptr, 0, qtotal, H, (uint32_t)ng);
+    } else {   // not batched: the single-witness px and division of each witness, straight into its vector
+      for (size_t p = 0; p < k; p++) {
+        if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
+        CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, H + p * ng, nullptr, err, s3));
+      }
+      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)ng, nullptr, 0, qtotal, H, (uint32_t)ng);
     }
-    k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)ng, nullptr, 0, qtotal, H, (uint32_t)ng);
+    g_launches += 1;
+    if ((rc = sort_of(7, H, ng, s3))) return rc;
+    if ((rc = buckets_of(7, s3))) return rc;
   }
-  g_launches += 1;
-  if ((rc = sort_of(7, H, ng, s3))) return rc;
-  if ((rc = buckets_of(7, s3))) return rc;
-  // --- the witness MSMs: both sorts on the main stream, then the bucket phases fan out as in pinocchio_enqueue (G2 first)
-  if ((rc = sort_of(2, d_w, m, st))) return rc;
-  EV_REC(e_sorted[1], st);
-  if (pk->g[0]) {
-    if ((rc = sort_of(0, d_w + l1, m, st))) return rc;
+  // --- the witness MSMs: the sorts on the main stream, then the bucket phases fan out as in pinocchio_enqueue (G2 first);
+  // the first set issued stays on the main stream
+  const int group_src[2] = {src[0] >= 0 ? src[0] : src[1], src[2]};   // w[l1..) for A, Ap; w for B .. Kp
+  if (group_src[1] >= 0) {
+    if ((rc = sort_of(group_src[1], d_w, m, st))) return rc;
+    EV_REC(e_sorted[1], st);
+  }
+  if (group_src[0] >= 0) {
+    if ((rc = sort_of(group_src[0], d_w + l1, m, st))) return rc;
     EV_REC(e_sorted[0], st);
   }
   int next_side = 0;
+  bool first = true;
+  bool used[3] = {false, false, pk->g[7] != nullptr};   // G1T runs on side stream 3
   for (int j : {2, 3, 4, 5, 6, 0, 1}) {
     if (!pk->g[j]) continue;
-    cudaStream_t sk = j == 2 ? st : side[next_side++ % 3];   // one bucket phase stays on the main stream
+    cudaStream_t sk = st;
+    if (!first) {
+      const int si = next_side++ % 3;
+      sk = side[si];
+      used[si] = true;
+    }
+    first = false;
     if (sk != st) EV_WAIT(sk, e_sorted[kPinSortSrc[j] == 2 ? 1 : 0]);
     if ((rc = buckets_of(j, sk))) return rc;
   }
   for (int si = 0; si < 3; si++)
-    if (side[si] != st) {
+    if (side[si] != st && (used[si] || pk->world == 1)) {
       EV_REC(e_done[si], side[si]);
       EV_WAIT(st, e_done[si]);
     }
-  k_pinocchio_finalize_batch<<<nblk(7 * k, kPinFinalizeBlock) + nblk(k, kPinFinalizeBlock), kPinFinalizeBlock, 0, st>>>(
-      rec1, rec2, (uint32_t)k, d_out);
+  if (!d_recs) {
+    k_pinocchio_finalize_batch<<<nblk(7 * k, kPinFinalizeBlock) + nblk(k, kPinFinalizeBlock), kPinFinalizeBlock, 0, st>>>(
+        rec1, rec2, (uint32_t)k, d_out);
+  } else {
+    CU(cudaMemsetAsync(d_recs, 0, k * kPinRecordBytes, st));
+    k_pinocchio_records_batch<<<nblk(8 * k, 256), 256, 0, st>>>(rec1, rec2, (uint32_t)k, d_recs);
+  }
   g_launches += 1;
   CU(cudaGetLastError());
+  return B200_OK;
+}
+
+// The k proofs of a batch at d_out + 108p (u64), or with `records` this rank's k records at d_out + 2 KB * p.  A sharded
+// key without `records` computes its records, all-gathers them (k records per rank, on the key's prove-context
+// communicator, on `st`) and finalises: every rank receives the k proofs.  After pinocchio_batch_check and, without
+// `records`, pinocchio_batch_comm_check.  Once the records' scratch exists the all-gather runs whatever else fails, so no
+// peer is left waiting; the error is then returned and nothing is finalised.
+int pinocchio_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq* d_out, bool records, cudaStream_t st,
+                            int* err) {
+  int rc;
+  R1csBatch* fb = nullptr;
+  if (pk->world == 1 || records) {
+    rc = pinocchio_batch_parts(pk, r1, d_w, k, d_out, records ? reinterpret_cast<uint8_t*>(d_out) : nullptr, st, err, &fb);
+  } else {
+    if ((rc = pinocchio_batch_scratch(pk, k, false))) return rc;
+    CU(pk->gather.ensure(kPinRecordBytes * k * (size_t)pk->world));
+    ProveBatch& b = *pk->batch;
+    rc = pinocchio_batch_parts(pk, r1, d_w, k, nullptr, b.parts.as<uint8_t>(), st, err, &fb);
+    ncclResult_t nrc = g_comm.api.AllGather(b.parts.p, pk->gather.p, kPinRecordBytes * k, ncclUint8, pk->pctx().comm, st);
+    if (rc) return rc;
+    if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
+    k_pinocchio_gather_finalize_batch<<<pinocchio_finalize_blocks((uint32_t)k), kPinFinalizeBlock, 0, st>>>(
+        pk->gather.as<uint8_t>(), pk->world, (uint32_t)k, d_out);
+    g_launches += 1;
+    CU(cudaGetLastError());
+  }
+  if (rc) return rc;
   // behind everything of this batch: what the next regrowth of any of its scratches waits for
+  ProveBatch& b = *pk->batch;
   EV_REC(b.done, st);
   for (const auto& g : pk->g)
     if (g && g->batch) EV_REC(g->batch->done, st);
@@ -1233,12 +1431,13 @@ int pinocchio_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w
   if (!w || !out_g1 || !pi_b) return fail(B200_EINVAL, "%s: null pointer", what);
   int rc = pinocchio_batch_check(pk, r1, nw, k, what);
   if (rc) return rc;
+  if ((rc = pinocchio_batch_comm_check(pk, what))) return rc;
   if ((rc = pinocchio_batch_scratch(pk, k, true))) return rc;
   ProveBatch& b = *pk->batch;
   cudaStream_t st = pk->pctx().main;
   CU(cudaMemcpyAsync(b.w_stage.p, w, k * nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
   Fq* o = b.out.as<Fq>();
-  if ((rc = pinocchio_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, o, st, pk->d_err_sync.as<int>()))) return rc;
+  if ((rc = pinocchio_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, o, false, st, pk->d_err_sync.as<int>()))) return rc;
   // as finish_host_proof, for k proofs: the wait runs with the library mutex released
   CU(cudaMemcpyAsync(b.h_out, o, k * kHostProofWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(b.h_out + k * kHostProofWords));
@@ -1897,8 +2096,34 @@ int b200_groth16_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, cons
   if (!p || !r1 || !d_w || !r || !s || !d_out) return fail(B200_EINVAL, "%s: bad arguments", what);
   int rc = groth16_batch_check(p, r1, nw, k, r, s, what);
   if (rc) return rc;
-  return drain_on_error(groth16_batch_enqueue(p, r1, (const Fr*)d_w, k, r, s, (Fq*)d_out,
+  if ((rc = groth16_batch_comm_check(p, what))) return rc;
+  return drain_on_error(groth16_batch_enqueue(p, r1, (const Fr*)d_w, k, r, s, (Fq*)d_out, false,
                                               stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_groth16_prove_witness_batch_partial_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                                    const uint64_t* r, const uint64_t* s, void* d_parts, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  const char* what = "groth16_prove_witness_batch_partial_device";
+  ProvingKey* p = find_pk(pk, 1);
+  R1cs* r1 = find_r1cs(r1cs);
+  if (!p || !r1 || !d_w || !r || !s || !d_parts) return fail(B200_EINVAL, "%s: bad arguments", what);
+  int rc = groth16_batch_check(p, r1, nw, k, r, s, what);
+  if (rc) return rc;
+  return drain_on_error(groth16_batch_enqueue(p, r1, (const Fr*)d_w, k, r, s, (Fq*)d_parts, true,
+                                              stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_groth16_finalize_batch_device(b200_pk_t pk, const void* d_parts, int world, size_t k, void* d_out, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  if (!find_pk(pk, 1) || !d_parts || !d_out || world < 1 || k == 0 || k > 0xffffffffull)
+    return fail(B200_EINVAL, "groth16_finalize_batch_device: bad arguments");
+  cudaStream_t st = stream ? (cudaStream_t)stream : g_ctx[0].main;
+  k_groth16_finalize_batch<<<groth16_finalize_blocks((uint32_t)k), kG16FinalizeBlock, 0, st>>>((const uint8_t*)d_parts, world,
+                                                                                                 (uint32_t)k, (Fq*)d_out);
+  g_launches += 1;
+  CU(cudaGetLastError());
+  return B200_OK;
 }
 int b200_pinocchio_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const void* d_px, size_t npx, void* d_out,
                                 void* stream) {
@@ -1948,8 +2173,34 @@ int b200_pinocchio_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, co
   if (!p || !r1 || !d_w || !d_out) return fail(B200_EINVAL, "%s: bad arguments", what);
   int rc = pinocchio_batch_check(p, r1, nw, k, what);
   if (rc) return rc;
-  return drain_on_error(pinocchio_batch_enqueue(p, r1, (const Fr*)d_w, k, (Fq*)d_out,
+  if ((rc = pinocchio_batch_comm_check(p, what))) return rc;
+  return drain_on_error(pinocchio_batch_enqueue(p, r1, (const Fr*)d_w, k, (Fq*)d_out, false,
                                                 stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_pinocchio_prove_witness_batch_record_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                                     void* d_records, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  const char* what = "pinocchio_prove_witness_batch_record_device";
+  ProvingKey* p = find_pk(pk, 2);
+  R1cs* r1 = find_r1cs(r1cs);
+  if (!p || !r1 || !d_w || !d_records) return fail(B200_EINVAL, "%s: bad arguments", what);
+  int rc = pinocchio_batch_check(p, r1, nw, k, what);
+  if (rc) return rc;
+  return drain_on_error(pinocchio_batch_enqueue(p, r1, (const Fr*)d_w, k, (Fq*)d_records, true,
+                                                stream ? (cudaStream_t)stream : g_ctx[0].main, p->d_err.as<int>()));
+}
+int b200_pinocchio_finalize_records_batch_device(const void* d_records, int world, size_t k, void* d_out, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  if (!d_records || !d_out || world < 1 || k == 0 || k >= (1ull << 28))
+    return fail(B200_EINVAL, "pinocchio_finalize_records_batch_device: bad arguments");
+  cudaStream_t st = stream ? (cudaStream_t)stream : g_ctx[0].main;
+  k_pinocchio_gather_finalize_batch<<<pinocchio_finalize_blocks((uint32_t)k), kPinFinalizeBlock, 0, st>>>(
+      (const uint8_t*)d_records, world, (uint32_t)k, (Fq*)d_out);
+  g_launches += 1;
+  CU(cudaGetLastError());
+  return B200_OK;
 }
 int b200_fq12_mul_batch(const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) { B200_API_BODY(fq12_mul_batch_host(a, b, n, out)) }
 int b200_pairing_batch(const uint64_t* g1_jac, const uint64_t* g2_jac, size_t n, uint64_t* out) { B200_API_BODY(pairing_batch_host(g1_jac, g2_jac, n, out)) }

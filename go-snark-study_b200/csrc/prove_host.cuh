@@ -37,6 +37,7 @@ struct ProveBatch {
   DevBuf glv;        // per proof GlvScalars of (s_p, r_p)
   DevBuf w_stage;    // the host entry's witnesses
   DevBuf out;        // the host entry's k proofs (48 u64 each; Pinocchio: 108)
+  DevBuf parts;      // a sharded key's k partial records (1 KB each), the input of the all-gather
   uint64_t* h_out = nullptr;   // pinned landing area of the host entry: the k proofs + the error word
   cudaEvent_t ev[9] = {};
   cudaEvent_t done = nullptr;
@@ -65,6 +66,11 @@ struct ProvingKey {
   bool tail[4] = {false, false, false, false};        // this rank also holds set k's blinding points
   size_t n_c_full = 0;                                // length of the C part of the C||PTD set (m - npublic - 1)
   int sort_src[3] = {0, 1, 2};                        // set k reuses the digit sort of set sort_src[k] (same scalars)
+  // every rank's cut, the set lengths, and the window bits and table rows the sets were built with: what a batch's
+  // refusals are decided on, so that every rank of the shard decides them alike
+  std::vector<ShardCut> cuts;
+  size_t len[4] = {0, 0, 0, 0};
+  int window_bits = 0, table_windows = 0;
   DevBuf s4;                                          // extra scalar vector (non-shared case)
   DevBuf h_full;              // full quotient (sharded mode)
   DevBuf gather;              // all-gathered partial records (world x 1 KB), when a communicator is active
@@ -100,7 +106,7 @@ size_t pk_device_bytes(const ProvingKey& pk) {
   for (const auto& g : pk.g)
     if (g) s += bases_device_bytes(*g);
   if (const ProveBatch* b = pk.batch.get())
-    s += dev_bytes({&b->W, &b->CH, &b->rec, &b->rs, &b->glv, &b->w_stage, &b->out});
+    s += dev_bytes({&b->W, &b->CH, &b->rec, &b->rs, &b->glv, &b->w_stage, &b->out, &b->parts});
   return s;
 }
 
@@ -128,28 +134,11 @@ __device__ XYZZ<F> xyzz_mul_scalar(const XYZZ<F>& p, const Fr& k) {
   return r;
 }
 
-// Partial-result record of one rank: A (G1 XYZZ @ +0), B1 (@ +256), B2 (G2 XYZZ @ +512),
-// CH (@ +768) — 1 KB; `parts` holds nparts consecutive records (1 on a single GPU,
-// world_size after the NCCL all-gather).  rs = {r, s} standard form.
-// out: PiA (3 Fq) | PiC (3 Fq) | PiB (3 Fq2), Jacobian, standard form.
-constexpr size_t kPartialBytes = 1024;
-// Sharded mode.  Each rank has already folded s*A_part + r*B1_part into its C part (linear in the partial
-// sums, so this is done per rank, overlapped with its other MSMs); what remains after the all-gather is
-// three point sums: A (slot @+0), B2 (@+512), C (@+768).
-__global__ void k_groth16_finalize(const uint8_t* parts, int nparts, Fq* out_a, Fq* out_c, Fq2* out_b) {
-  uint32_t t = threadIdx.x;
-  if (t == 0 || t == 32) {
-    int off = t == 0 ? 0 : 768;
-    XYZZ<Fq> acc = *reinterpret_cast<const XYZZ<Fq>*>(parts + off);
-    for (int p = 1; p < nparts; p++) xyzz_add(acc, *reinterpret_cast<const XYZZ<Fq>*>(parts + kPartialBytes * p + off));
-    store_jacobian_std(acc, t == 0 ? out_a : out_c);
-  }
-  if (t == 64) {
-    XYZZ<Fq2> acc = *reinterpret_cast<const XYZZ<Fq2>*>(parts + 512);
-    for (int p = 1; p < nparts; p++) xyzz_add(acc, *reinterpret_cast<const XYZZ<Fq2>*>(parts + kPartialBytes * p + 512));
-    store_jacobian_std(acc, out_b);
-  }
-}
+// Partial-result record of one rank: kPartialBytes (shard_batch.cuh); `parts` holds nparts consecutive records (1 on a
+// single GPU, world_size after the NCCL all-gather), summed by k_groth16_finalize_batch with k = 1.  Sharded mode: each
+// rank has already folded s*A_part + r*B1_part into its C part (linear in the partial sums, so this is done per rank,
+// overlapped with its other MSMs); what remains after the all-gather is three point sums: A (slot @+0), B2 (@+512),
+// C (@+768).
 // in place: CH part (@+768) += prod[0] + prod[1]
 __global__ void k_groth16_fold_products(uint8_t* res, const XYZZ<Fq>* prod) {
   if (threadIdx.x | blockIdx.x) return;
@@ -220,6 +209,9 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   const double wgt[4] = {w_ab, w_ab, g_w_g2 / 100.0, 1.0};
   std::vector<ShardCut> cuts((size_t)world);
   shard_partition(len, wgt, world, cuts.data());   // equal pieces of the weighted line (shard_partition.h)
+  for (int k = 0; k < 4; k++) pk->len[k] = len[k];
+  pk->window_bits = c;
+  pk->table_windows = g_table_windows;
   for (int k = 0; k < 4; k++) {
     pk->lo[k] = cuts[(size_t)rank].lo[k];
     pk->hi[k] = cuts[(size_t)rank].hi[k];
@@ -272,6 +264,7 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   CU(pk->s3.alloc((m + n_ptd + 4) * sizeof(Fr)));
   CU(pk->s4.alloc((m + 4) * sizeof(Fr)));
   if (world > 1) CU(pk->h_full.alloc((m + n_ptd + 4) * sizeof(Fr)));
+  pk->cuts = std::move(cuts);
   uint64_t h = g_next_pk++;
   g_pks[h] = std::move(pk);
   *out = h;
@@ -284,8 +277,51 @@ ProvingKey* find_pk(b200_pk_t h, int kind) {
   return it->second.get();
 }
 
+// One rank's part of a Groth16 proof: set j in {A, B1, B2} reads w[lo_j, hi_j), ++ [1, r, s] when the rank holds the
+// set's tail; C||PTD reads w[l1 + c_lo, l1 + c_lo + n_c) ++ h[p_lo, p_lo + n_p), ++ [-r s] with the tail.  terms[j]: the
+// length of set j's scalar vector, 0 if the rank holds none of it (one GPU: m + 3, and n_c_full + len(PTD) + 1).
+// Computed from the cuts of any rank, so every rank can size every rank's part.
+struct G16Slices {
+  size_t lo[4], hi[4], terms[4];
+  bool tail[4];
+  size_t c_lo, n_c, p_lo, n_p;
+};
+G16Slices g16_slices(const ProvingKey* pk, int rank) {
+  G16Slices sl{};
+  const ShardCut& ct = pk->cuts[(size_t)rank];
+  for (int j = 0; j < 4; j++) {
+    sl.lo[j] = ct.lo[j];
+    sl.hi[j] = ct.hi[j];
+    sl.tail[j] = sl.hi[j] == pk->len[j] && (sl.lo[j] < sl.hi[j] || (rank == pk->world - 1 && pk->len[j] == 0));
+    sl.terms[j] = sl.hi[j] - sl.lo[j] + (sl.tail[j] ? (j < 3 ? 3 : 1) : 0);
+  }
+  const size_t ncf = pk->n_c_full;
+  sl.c_lo = std::min(sl.lo[3], ncf);
+  sl.n_c = std::min(sl.hi[3], ncf) - sl.c_lo;
+  sl.p_lo = sl.lo[3] > ncf ? sl.lo[3] - ncf : 0;
+  sl.n_p = (sl.hi[3] > ncf ? sl.hi[3] - ncf : 0) - sl.p_lo;
+  return sl;
+}
+// Where the A / B1 / B2 vectors of a batch live in its W: per proof, one vector per digit sort (sets that share a sort
+// share its vector), vector j of proof p at W + k*woff[j] + p*terms[j].  Returns the scalars per proof (one GPU: m + 3).
+size_t g16_w_layout(const ProvingKey* pk, const G16Slices& sl, size_t woff[3]) {
+  size_t total = 0;
+  for (int j = 0; j < 3; j++) {
+    woff[j] = 0;
+    if (!pk->g[j]) continue;
+    if (pk->sort_src[j] == j) {
+      woff[j] = total;
+      total += sl.terms[j];
+    } else {
+      woff[j] = woff[pk->sort_src[j]];
+    }
+  }
+  return total;
+}
+
 // Grows the key's batch scratch to k proofs (host: also the host entry's witness staging, proof buffer and pinned landing
-// area).  A regrowth first waits for the key's last batch (its `done` event), not for the device.
+// area).  A regrowth first waits for the key's last batch (its `done` event), not for the device.  A sharded key's
+// vectors are those of its own part (G16Slices), and it keeps k partial records for the all-gather.
 int groth16_batch_scratch(ProvingKey* pk, size_t k, bool host) {
   if (!pk->batch) {
     auto b = std::make_unique<ProveBatch>();
@@ -294,15 +330,19 @@ int groth16_batch_scratch(ProvingKey* pk, size_t k, bool host) {
     pk->batch = std::move(b);
   }
   ProveBatch& b = *pk->batch;
-  const size_t m = pk->m, nch = pk->n_c_full + pk->n_h_bases + 1;
+  const size_t m = pk->m;
+  const G16Slices sl = g16_slices(pk, pk->rank);
+  size_t woff[3];
+  const size_t nw = g16_w_layout(pk, sl, woff), nch = pk->g[3] ? sl.terms[3] : 0;
   const bool grow_host = host && b.out.bytes < k * kBatchProofWords * sizeof(uint64_t);
   if (b.k < k || grow_host) CU(cudaEventSynchronize(b.done));
   if (b.k < k) {
-    CU(b.W.alloc(k * (m + 3) * sizeof(Fr)));
+    CU(b.W.alloc(k * nw * sizeof(Fr)));
     CU(b.CH.alloc(k * nch * sizeof(Fr)));
     CU(b.rec.alloc(k * (5 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>))));
     CU(b.rs.alloc(k * 4 * sizeof(Fr)));
     CU(b.glv.alloc(k * sizeof(GlvScalars)));
+    if (pk->world > 1) CU(b.parts.alloc(k * kPartialBytes));
     b.k = k;
   }
   if (grow_host) {
@@ -323,7 +363,7 @@ Fr fr_load_std(const uint64_t* v) {
 }
 
 // ---- blinding products s*A and r*B1 (groth16.go:272-273): GLV half-warps (glv.cuh) -----------------------------
-// One warp, all 32 lanes: lanes 0..15 -> prod[0] = s*A, lanes 16..31 -> prod[1] = r*B1 (res layout as in k_groth16_finalize).
+// One warp, all 32 lanes: lanes 0..15 -> prod[0] = s*A, lanes 16..31 -> prod[1] = r*B1 (the partial record layout, shard_batch.cuh).
 __global__ void k_groth16_products(const uint8_t* res, GlvScalars g, XYZZ<Fq>* prod) {
   const uint32_t t = threadIdx.x & 31u;
   const uint32_t grp = t >> 4;
@@ -500,7 +540,7 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
       CU(pk->gather.ensure(kPartialBytes * (size_t)pk->world));
       ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPartialBytes, ncclUint8, pk->pctx().comm, st);
       if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
-      k_groth16_finalize<<<1, 96, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, d_out, d_out + 3, reinterpret_cast<Fq2*>(d_out + 6));
+      k_groth16_finalize_batch<<<groth16_finalize_blocks(1), kG16FinalizeBlock, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, 1, d_out);
       g_launches += 2;
     } else {
       CU(cudaMemcpyAsync(d_out, res, kPartialBytes, cudaMemcpyDeviceToDevice, st));
@@ -515,7 +555,7 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
 int groth16_finalize_enqueue(ProvingKey* pk, const uint8_t* d_parts, int nparts, const uint64_t* r, const uint64_t* s,
                              Fq* d_out, cudaStream_t st) {
   (void)pk; (void)r; (void)s;  // r, s were consumed per rank (their products are already inside the C parts)
-  k_groth16_finalize<<<1, 96, 0, st>>>(d_parts, nparts, d_out, d_out + 3, reinterpret_cast<Fq2*>(d_out + 6));
+  k_groth16_finalize_batch<<<groth16_finalize_blocks(1), kG16FinalizeBlock, 0, st>>>(d_parts, nparts, 1, d_out);
   g_launches += 1;
   CU(cudaGetLastError());
   return B200_OK;
@@ -533,11 +573,21 @@ int check_sharded_host_call(const ProvingKey* pk, const char* what, const char* 
   return B200_OK;
 }
 
-// Upload the host witness into pk->w_stage on `st`: all of it, or only the index ranges this rank's MSMs read.
-int stage_witness(ProvingKey* pk, const uint64_t* w, bool all, cudaStream_t st) {
-  CU(pk->w_stage.ensure(pk->m * sizeof(Fr)));
+// Upload the host witness into pk->w_stage on `st`: all of it, or only the index ranges this rank's MSMs read.  dst:
+// nwit witnesses (row-major, m scalars each) into dst instead, each staged alike (a batch's).
+int stage_witness(ProvingKey* pk, const uint64_t* w, bool all, cudaStream_t st, Fr* dst = nullptr, size_t nwit = 1) {
+  if (!dst) {
+    CU(pk->w_stage.ensure(pk->m * sizeof(Fr)));
+    dst = pk->w_stage.as<Fr>();
+  }
+  const Fr* src = reinterpret_cast<const Fr*>(w);
+  const size_t pitch = pk->m * sizeof(Fr);
+  auto upload = [&](size_t lo, size_t cnt) {
+    return nwit == 1 ? cudaMemcpyAsync(dst + lo, src + lo, cnt * sizeof(Fr), cudaMemcpyHostToDevice, st)
+                     : cudaMemcpy2DAsync(dst + lo, pitch, src + lo, pitch, cnt * sizeof(Fr), nwit, cudaMemcpyHostToDevice, st);
+  };
   if (all) {
-    CU(cudaMemcpyAsync(pk->w_stage.p, w, pk->m * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    CU(upload(0, pk->m));
     return B200_OK;
   }
   const size_t l1 = pk->npublic + 1, ncf = pk->n_c_full;
@@ -551,8 +601,7 @@ int stage_witness(ProvingKey* pk, const uint64_t* w, bool all, cudaStream_t st) 
     bool dup = false;
     for (int j = 0; j < k; j++) dup = dup || (lo[j] <= lo[k] && hi[k] <= hi[j] && lo[j] < hi[j]);
     if (dup) continue;
-    CU(cudaMemcpyAsync(pk->w_stage.as<Fr>() + lo[k], reinterpret_cast<const Fr*>(w) + lo[k], (hi[k] - lo[k]) * sizeof(Fr),
-                       cudaMemcpyHostToDevice, st));
+    CU(upload(lo[k], hi[k] - lo[k]));
   }
   return B200_OK;
 }
@@ -609,7 +658,6 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
 // Pinocchio result slots (XYZZ, 256 B each): 0 PiA, 1 PiAp, 2 PiBp, 3 PiC, 4 PiCp, 5 PiH, 6 PiKp, 7 PiB (G2).
 // Base sets g[k]: 0 A, 1 Ap, 2 B (G2), 3 Bp, 4 C, 5 Cp, 6 Kp, 7 G1T.
 constexpr int kPinSlot[8] = {0, 1, 7, 2, 3, 4, 6, 5};
-constexpr size_t kPinRecordBytes = 8 * 256;
 
 // Sharded mode (world > 1): the eight MSMs are independent objects, so whole MSMs are dealt to the ranks — greedy
 // longest-first onto the least loaded rank by term count (a G2 term ~2.8 G1 terms) — and no MSM is split.  `owner[k]` is the
@@ -628,20 +676,8 @@ void pinocchio_owners(size_t m, size_t l1, size_t n_g1t, int world, int owner[8]
   }
 }
 
-// sum the world records slot by slot (every slot is non-infinity on exactly one rank) -> standard-form outputs
-__global__ void k_pinocchio_gather_finalize(const uint8_t* recs, int world, Fq* out_g1, Fq2* out_b) {
-  uint32_t t = threadIdx.x;
-  if (t < 7) {
-    XYZZ<Fq> acc = XYZZ<Fq>::inf();
-    for (int g = 0; g < world; g++) xyzz_add(acc, *reinterpret_cast<const XYZZ<Fq>*>(recs + kPinRecordBytes * g + 256 * t));
-    store_jacobian_std(acc, out_g1 + 3 * t);
-  }
-  if (t == 32) {
-    XYZZ<Fq2> acc = XYZZ<Fq2>::inf();
-    for (int g = 0; g < world; g++) xyzz_add(acc, *reinterpret_cast<const XYZZ<Fq2>*>(recs + kPinRecordBytes * g + 256 * 7));
-    store_jacobian_std(acc, out_b);
-  }
-}
+// The world records of one proof are summed slot by slot by k_pinocchio_gather_finalize_batch (pinocchio_batch.cuh) with
+// k = 1: every slot is non-infinity on exactly one rank.
 
 int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2, const uint64_t* bp,
                       const uint64_t* c, const uint64_t* cp, const uint64_t* kp, size_t m, const uint64_t* g1t,
@@ -660,6 +696,8 @@ int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2,
   size_t l1 = npublic + 1;
   pk->rank = rank;
   pk->world = world;
+  pk->window_bits = wb;
+  pk->table_windows = g_table_windows;
   int owner[8];
   pinocchio_owners(m, l1, n_g1t, world, owner);
   auto mine = [&](int k) { return owner[k] == rank; };
@@ -765,7 +803,7 @@ int pinocchio_enqueue(ProvingKey* pk, const Fr* d_w, const Fr* d_px, size_t npx,
     CU(pk->gather.ensure(kPinRecordBytes * (size_t)pk->world));
     ncclResult_t nrc = g_comm.api.AllGather(res, pk->gather.p, kPinRecordBytes, ncclUint8, pk->pctx().comm, st);
     if (nrc != ncclSuccess) return fail(B200_ECOMM, "ncclAllGather: %s", g_comm.api.GetErrorString(nrc));
-    k_pinocchio_gather_finalize<<<1, 64, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, d_out, reinterpret_cast<Fq2*>(d_out + 21));
+    k_pinocchio_gather_finalize_batch<<<pinocchio_finalize_blocks(1), kPinFinalizeBlock, 0, st>>>(pk->gather.as<uint8_t>(), pk->world, 1, d_out);
   } else {
     k_pinocchio_finalize<<<1, 64, 0, st>>>(res, d_out, reinterpret_cast<Fq2*>(d_out + 21));
   }
@@ -821,6 +859,7 @@ int pinocchio_batch_scratch(ProvingKey* pk, size_t k, bool host) {
   if (b.k < k) {
     CU(b.CH.alloc(k * pk->n_h_bases * sizeof(Fr)));
     CU(b.rec.alloc(k * (7 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>))));
+    if (pk->world > 1) CU(b.parts.alloc(k * kPinRecordBytes));
     b.k = k;
   }
   if (grow_host) {
@@ -838,7 +877,7 @@ int pinocchio_finalize_records(const uint8_t* d_recs, int world, uint64_t* out_g
   if (!d_recs || world < 1 || !out_g1 || !pi_b) return fail(B200_EINVAL, "pinocchio_finalize: bad arguments");
   DevBuf o;
   CU(o.alloc(64 * sizeof(Fq)));
-  k_pinocchio_gather_finalize<<<1, 64, 0, g_ctx[0].main>>>(d_recs, world, o.as<Fq>(), reinterpret_cast<Fq2*>(o.as<Fq>() + 21));
+  k_pinocchio_gather_finalize_batch<<<pinocchio_finalize_blocks(1), kPinFinalizeBlock, 0, g_ctx[0].main>>>(d_recs, world, 1, o.as<Fq>());
   CU(cudaGetLastError());
   uint64_t host_out[(21 + 6) * 4];
   CU(cudaMemcpyAsync(host_out, o.p, sizeof host_out, cudaMemcpyDeviceToHost, g_ctx[0].main));

@@ -204,20 +204,21 @@ __global__ void k_take_blocks(const Fr* __restrict__ src, uint32_t sstride, uint
   uint32_t q = e / N, i = e - q * N;
   d[e] = i < n ? src[(size_t)q * sstride + i] : Fr::zero();
 }
-// C||PTD scalar vector p (ch + p*stride, from the quotient's offset): the quotient h_p below nh (coef: blocks of cstride,
-// Montgomery -> standard form; null: already in place), zeros up to n_ptd, then tail[p*tstride] (-r_p s_p, standard form).
-// total = k * (n_ptd + 1).  A null tail writes none: the G1T scalar vectors of Pinocchio proofs (stride = n_ptd = len(G1T)).
+// C||PTD scalar vector p (ch + p*stride, from the quotient's offset): n_ptd slots holding h_p[off + i] for off + i < nh
+// (coef: blocks of cstride, Montgomery -> standard form; null: already in place) and zeros beyond, then tail[p*tstride]
+// (-r_p s_p, standard form).  total = k * (n_ptd + 1).  A null tail writes none: the G1T scalar vectors of Pinocchio
+// proofs (stride = n_ptd = len(G1T)), and the vectors of a key shard that does not hold the blinding point.  off > 0:
+// a key shard whose PowersTauDelta slice starts at index off, with n_ptd the slots of its slice.
 __global__ void k_quotient_store(const Fr* __restrict__ coef, uint32_t cstride, uint32_t nh, uint32_t n_ptd,
                                  const Fr* __restrict__ tail, uint32_t tstride, uint32_t total, Fr* __restrict__ ch,
-                                 uint32_t stride) {
+                                 uint32_t stride, uint32_t off = 0) {
   uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= total) return;
   uint32_t p = e / (n_ptd + 1), i = e - p * (n_ptd + 1);
   Fr* d = ch + (size_t)p * stride + i;
-  if (i < nh) {
-    if (coef) *d = coef[(size_t)p * cstride + i].from_mont();
-  } else if (i < n_ptd) {
-    *d = Fr::zero();
+  if (i < n_ptd) {
+    if (i + off >= nh) *d = Fr::zero();
+    else if (coef) *d = coef[(size_t)p * cstride + off + i].from_mont();
   } else if (tail) {
     *d = tail[(size_t)p * tstride];
   }

@@ -87,7 +87,9 @@ class DeviceProvingKey:
 
     def prove_witness_batch_limbs(self, r1cs, w_limbs, rs):
         """k proofs in one call (b200_groth16_prove_witness_batch): ``w_limbs`` holds k witnesses (k x m x 4 limbs, or
-        k*m x 4), ``rs`` a list of k (r, s) pairs.  Proof p is prove_witness_limbs(r1cs, w_limbs[p], *rs[p])."""
+        k*m x 4), ``rs`` a list of k (r, s) pairs.  Proof p is prove_witness_limbs(r1cs, w_limbs[p], *rs[p]).  On a key
+        shard with a matching communicator (b200_comm_init, every rank calling with the same arguments) each rank
+        computes its part of the k proofs, one all-gather of k records runs, and every rank gets all k proofs."""
         k = len(rs)
         w = np.ascontiguousarray(w_limbs, dtype=np.uint64).reshape(-1, 4)
         if k == 0 or w.shape[0] % k:

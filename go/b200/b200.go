@@ -396,7 +396,9 @@ func (k *Groth16Key) ProveWitness(r1cs *R1CS, w []*big.Int, r, s *big.Int) (piA 
 }
 
 // ProveWitnessBatch is ProveWitness for k witnesses of one circuit in one call (b200_groth16_prove_witness_batch):
-// proof p is ProveWitness(r1cs, ws[p], rs[p], ss[p]).  Worth it for small circuits proved many times.
+// proof p is ProveWitness(r1cs, ws[p], rs[p], ss[p]).  Worth it for small circuits proved many times.  On a
+// LoadGroth16Shard key it works after CommInit, SPMD: every rank passes the same witnesses and r, s, computes its part
+// of the k proofs, and receives all k proofs after one all-gather.
 func (k *Groth16Key) ProveWitnessBatch(r1cs *R1CS, ws [][]*big.Int, rs, ss []*big.Int) (piA [][3]*big.Int, piB [][3][2]*big.Int, piC [][3]*big.Int, err error) {
 	n := len(ws)
 	if n == 0 || len(rs) != n || len(ss) != n {
@@ -446,6 +448,21 @@ func LoadPinocchio(a, ap [][3]*big.Int, b [][3][2]*big.Int, bp, c, cp, kp, g1t [
 	return k, nil
 }
 
+// LoadPinocchioShard loads rank `rank` of a `world`-way shard of a Pinocchio key (b200_pinocchio_pk_load_shard): whole
+// MSMs are dealt to the ranks.  After CommInit, ProveWitness and ProveWitnessBatch on it are SPMD calls that return the
+// whole proofs on every rank.
+func LoadPinocchioShard(a, ap [][3]*big.Int, b [][3][2]*big.Int, bp, c, cp, kp, g1t [][3]*big.Int, z []*big.Int, nPublic,
+	rank, world int) (*PinocchioKey, error) {
+	k := &PinocchioKey{}
+	rc := C.b200_pinocchio_pk_load_shard(u64(FlatG1(a)), u64(FlatG1(ap)), u64(FlatG2(b)), u64(FlatG1(bp)), u64(FlatG1(c)),
+		u64(FlatG1(cp)), u64(FlatG1(kp)), C.size_t(len(a)), u64(FlatG1(g1t)), C.size_t(len(g1t)), u64(FlatFr(z, Coeff)),
+		C.size_t(len(z)), C.size_t(nPublic), 0, C.int(rank), C.int(world), &k.h)
+	if err := check(rc); err != nil {
+		return nil, err
+	}
+	return k, nil
+}
+
 func (k *PinocchioKey) Free() { C.b200_pk_free(k.h) }
 
 func pinocchioProof(g1, b []uint64) *PinocchioProof {
@@ -465,7 +482,8 @@ func (k *PinocchioKey) ProveWitness(r1cs *R1CS, w []*big.Int) (*PinocchioProof, 
 }
 
 // ProveWitnessBatch is ProveWitness for k witnesses of one circuit in one call (b200_pinocchio_prove_witness_batch):
-// proof p is ProveWitness(r1cs, ws[p]).  Worth it for small circuits proved many times.
+// proof p is ProveWitness(r1cs, ws[p]).  Worth it for small circuits proved many times.  On a LoadPinocchioShard key
+// it works after CommInit, SPMD: every rank passes the same witnesses and receives all k proofs after one all-gather.
 func (k *PinocchioKey) ProveWitnessBatch(r1cs *R1CS, ws [][]*big.Int) ([]*PinocchioProof, error) {
 	n := len(ws)
 	if n == 0 {

@@ -424,11 +424,24 @@ int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void
  *     are allocated on the first batch and grown (never shrunk) by a larger one, which first waits for the previous
  *     batch; the pinned landing area of this entry holds k*48 + 1 words.
  *   - B200_EINVAL before anything is allocated or enqueued: k = 0, a bad handle or null pointer, nw different from the
- *     key's m or the R1CS's m, a sharded key, or a batch too large for 32-bit indexing: k*ceil(255/c)*(m+3) sort entries
- *     (or k times a set's buckets) reaching 2^31, the same for the C||PTD set, or 3k*2N >= 2^32 transform elements
- *     (N = the power of two >= n).
+ *     key's m or the R1CS's m, a sharded key without a matching communicator (use
+ *     b200_groth16_prove_witness_batch_partial_device + b200_groth16_finalize_batch_device around your own all-gather),
+ *     or a batch too large for 32-bit indexing: k*ceil(255/c)*(m+3) sort entries (or k times a set's buckets) reaching
+ *     2^31, the same for the C||PTD set, or 3k*2N >= 2^32 transform elements (N = the power of two >= n).
  *   - B200_ERANGE: any r_p or s_p >= r (before anything is enqueued); a witness entry >= r in any witness (the outputs
- *     are left untouched, and the next call starts from a clear error word). */
+ *     are left untouched, and the next call starts from a clear error word).
+ *   - A sharded key (b200_groth16_pk_load_shard) with a matching communicator (b200_comm_init; SPMD, every rank calls
+ *     with the same witnesses, r and s): each rank computes its part of the k proofs (the launches of its part of one
+ *     proof, whatever k), one ncclAllGather of k 1 KB records per rank runs on the key's prove-context communicator
+ *     on the key's main stream, and one launch finalises: every rank returns all k proofs.  Only the witness ranges the
+ *     rank reads are uploaded (all of each witness on a rank that needs px).  The size refusals above are decided on
+ *     the largest part ANY rank of the shard holds, so every rank returns the same code before anything is enqueued.
+ *     A device allocation failure (B200_ENOMEM / B200_ECUDA) while the batch's scratch grows can happen on some ranks only:
+ *     those ranks return before the all-gather and their peers wait in it; once the scratch exists, the all-gather runs
+ *     whatever else fails.
+ *     A witness entry >= r: the ranks that read it return B200_ERANGE, the others B200_OK with proofs that are not
+ *     those of the witnesses (the all-gather runs either way).  Scratch: k times the rank's slices, k records and a
+ *     gather buffer of world*k records, grown and never shrunk, counted by b200_pk_device_bytes. */
 int b200_groth16_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, size_t k,
                                      const uint64_t* r, const uint64_t* s,
                                      uint64_t* pi_a, uint64_t* pi_b, uint64_t* pi_c);
@@ -440,6 +453,29 @@ int b200_groth16_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint6
  * in b200_groth16_prove_witness_device; the other errors are those of the host entry. */
 int b200_groth16_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
                                             const uint64_t* r, const uint64_t* s, void* d_out, void* stream);
+/* This rank's part of b200_groth16_prove_witness_batch_device on a key shard, for a caller that runs its own collective
+ * or emulates the ranks on one GPU: d_parts receives k partial records of 1 KB on `stream`, record p at
+ * d_parts + 1024p, in the layout of b200_groth16_prove_device's single record (A @ +0, B1 @ +256, B2 @ +512, the C part
+ * with s_p*A_part + r_p*B1_part folded in @ +768; XYZZ; a set the rank does not hold is infinity).
+ *   - It never gathers, with or without a communicator.  A world == 1 key gives its k records too (the finalize input
+ *     for world = 1).
+ *   - Only a rank that holds PowersTauDelta indices (b200_groth16_shard_info needs_px) runs the QAP front end (one
+ *     batched front end for the h-direct shape) and reads whole witnesses; a rank that holds no part of A or B1 runs
+ *     no blinding products.  Launches: those of the rank's part of one proof, whatever k, plus the documented extras of
+ *     b200_msm_device_batch.
+ *   - Synchronisation, scratch and the error word as in b200_groth16_prove_witness_batch_device (a witness entry >= r
+ *     is read as 0 and reported by no call).
+ *   - B200_EINVAL before anything is allocated or enqueued: k = 0, a bad handle or null pointer, nw different from the
+ *     key's m or the R1CS's m, or a batch too large for 32-bit indexing on the largest part of ANY rank of the shard
+ *     (the same answer on every rank's key).  B200_ERANGE: any r_p or s_p >= r. */
+int b200_groth16_prove_witness_batch_partial_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                                    const uint64_t* r, const uint64_t* s, void* d_parts, void* stream);
+/* world x k partial records -> k proofs, one launch on `stream` (null: the library stream), no host synchronisation.
+ * The record of rank g for proof p is at d_parts + 1024*(g*k + p): what ncclAllGather of k KB per rank leaves.  d_out
+ * receives k x 48 u64, proof p at d_out + 48p (PiA | PiC | PiB, Jacobian, standard form); proof p equals what
+ * b200_groth16_finalize_device gives for that proof's world records.  pk only names the key (any rank's).
+ *   - B200_EINVAL: a bad handle, a null pointer, world < 1, k = 0 or k >= 2^32. */
+int b200_groth16_finalize_batch_device(b200_pk_t pk, const void* d_parts, int world, size_t k, void* d_out, void* stream);
 
 /* ---- Pinocchio from device memory, from the witness, and in batches ----------------------------------------------------
  * The twins of the Groth16 entries above for snark.GenerateProofs (snark.go:254-289).  Pinocchio has no blinding, so there
@@ -498,11 +534,18 @@ int b200_pinocchio_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const vo
  *     the first batch and grown (never shrunk) by a larger one, which first waits for the previous batch; the pinned
  *     landing area of this entry holds k*108 + 1 words.
  *   - B200_EINVAL before anything is allocated or enqueued: k = 0, a bad handle or null pointer, the size mismatches of
- *     the single entry, a sharded key, or a batch too large for 32-bit indexing: k*ceil(255/c)*terms sort entries (or k
- *     times a set's buckets) of any of the eight sets reaching 2^31, or 3k*2N >= 2^32 transform elements (N = the power
- *     of two >= n).
+ *     the single entry, a sharded key without a matching communicator (use
+ *     b200_pinocchio_prove_witness_batch_record_device + b200_pinocchio_finalize_records_batch_device around your own
+ *     all-gather), or a batch too large for 32-bit indexing: k*ceil(255/c)*terms sort entries (or k times a set's
+ *     buckets) of any of the eight sets reaching 2^31, or 3k*2N >= 2^32 transform elements (N = the power of two >= n).
  *   - B200_ERANGE: a witness entry >= r in any witness (the outputs are left untouched, and the next call starts from a
- *     clear error word). */
+ *     clear error word).
+ *   - A sharded key with a matching communicator (b200_comm_init; SPMD, every rank passes the same witnesses): each rank
+ *     runs only the sets it owns, one ncclAllGather of k 2 KB records per rank runs on the key's prove-context
+ *     communicator, and one launch finalises: every rank returns all k proofs.  The size refusals are decided on every
+ *     set of the key, owned or not, so every rank returns the same code; an allocation failure while the scratch grows
+ *     can happen on some ranks only, and their peers then wait in the all-gather.  A witness entry >= r: the ranks that
+ *     read it return B200_ERANGE, the others B200_OK with proofs that are not those of the witnesses. */
 int b200_pinocchio_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, size_t k,
                                        uint64_t* out_g1, uint64_t* pi_b);
 /* b200_pinocchio_prove_witness_batch from device memory: d_w holds the k witnesses (standard form, witness p at
@@ -512,6 +555,25 @@ int b200_pinocchio_prove_witness_batch(b200_pk_t pk, b200_r1cs_t r1cs, const uin
  * call; the other errors are those of the host entry. */
 int b200_pinocchio_prove_witness_batch_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
                                               void* d_out, void* stream);
+/* This rank's part of b200_pinocchio_prove_witness_batch_device on a key shard (b200_pinocchio_pk_load_shard), for a
+ * caller that runs its own collective or emulates the ranks on one GPU: d_records receives k records of 2 KB on
+ * `stream`, record p at d_records + 2048p, in the layout of b200_pinocchio_prove_record_device's single record (eight
+ * XYZZ slots of 256 B: PiA, PiAp, PiBp, PiC, PiCp, PiH, PiKp, PiB; a set the rank does not own is infinity).
+ *   - It never gathers, with or without a communicator; a world == 1 key gives its k records too.
+ *   - Only the sets the rank owns run (whole MSMs are dealt to the ranks); a sort group whose sorting set lives on another
+ *     rank is sorted by the first set of the group the rank owns; only the rank that owns G1T runs the QAP front end.
+ *   - Synchronisation, scratch and the error word as in b200_pinocchio_prove_witness_batch_device.
+ *   - B200_EINVAL before anything is allocated or enqueued: k = 0, a bad handle or null pointer, nw different from the
+ *     key's m or the R1CS's m, or a batch too large for 32-bit indexing on any set of the key, owned or not (the same
+ *     answer on every rank's key). */
+int b200_pinocchio_prove_witness_batch_record_device(b200_pk_t pk, b200_r1cs_t r1cs, const void* d_w, size_t nw, size_t k,
+                                                     void* d_records, void* stream);
+/* world x k records -> k proofs, one launch on `stream` (null: the library stream), no host synchronisation.  The
+ * record of rank g for proof p is at d_records + 2048*(g*k + p): what ncclAllGather of 2k KB per rank leaves.  d_out
+ * receives k x 108 u64, proof p at d_out + 108p (the seven G1 points, then PiB); proof p equals what
+ * b200_pinocchio_finalize_records gives for that proof's world records.
+ *   - B200_EINVAL: a null pointer, world < 1, k = 0 or k >= 2^28. */
+int b200_pinocchio_finalize_records_batch_device(const void* d_records, int world, size_t k, void* d_out, void* stream);
 
 /* ---- element-wise group operations, reference formulas (X,Y,Z-exact) ------------------- */
 /* bn128.G1.Add / Double / Neg / Affine (bn128/g1.go:32-170) and the G2 twins (bn128/g2.go:32-200), n independent
