@@ -2,6 +2,7 @@
 package is importable from the repository tree after build().
 
   build_cuda()        nvcc -> go-snark-study_b200/lib/libb200snark.so   (the product: sm_90a only)
+  build_gpu_arith()   nvcc -> go-snark-study_b200/lib/libb200_gpu_arith.so  (device test vehicle of the same headers)
   build_host_arith()  g++  -> go-snark-study_b200/lib/libb200_host_arith.so (CPU unit-test vehicle)
   build_oracle()      gcc  -> oracle/_build/liboracle.so             (test infrastructure)
 """
@@ -15,6 +16,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIBDIR = os.path.join(PKG, "lib")
 ORACLE = os.path.join(ROOT, "oracle")
 HOSTTEST = os.path.join(ROOT, "tests", "host")     # CPU test vehicles for the kernel headers (g++, no CUDA)
+DEVTEST = os.path.join(ROOT, "tests", "device")    # device test vehicles for the kernel headers (nvcc, sm_90a)
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CUDA_SOURCES = ["capi.cu"]
@@ -60,6 +62,22 @@ def build_cuda(force=False):
     cmd = [NVCC, *NVCC_FLAGS, "-I", os.path.join(ROOT, "include"), "-I", CSRC,
            "-o", target, *[os.path.join(CSRC, s) for s in CUDA_SOURCES]]
     _run(cmd, log=os.path.join(LIBDIR, "nvcc_build.log"))
+    return target
+
+
+def build_gpu_arith(force=False):
+    """nvcc build of tests/device/arith_device.cu with the product's own flags (device test vehicle for the arithmetic
+    headers, tests/test_gpu_arith.py).  Not linked into libb200snark.so."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    target = os.path.join(LIBDIR, "libb200_gpu_arith.so")
+    src = os.path.join(DEVTEST, "arith_device.cu")
+    if not force and not _newer(target, _all_sources(exts=(".cuh", ".h")) + [src]):
+        return target
+    if not os.path.exists(NVCC):
+        if os.path.exists(target):
+            return target          # GPU box without a toolchain change: use the shipped build
+        raise RuntimeError("nvcc not found and no prebuilt libb200_gpu_arith.so")
+    _run([NVCC, *NVCC_FLAGS, "-I", CSRC, "-o", target, src], log=os.path.join(LIBDIR, "nvcc_gpu_arith.log"))
     return target
 
 

@@ -25,8 +25,8 @@ void ec_ops(int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
     A = xyzz_dbl(A);
   } else if (op == 3) {  // via jacobian round trip
     A = jacobian_to_xyzz(xyzz_to_jacobian(A));
-  }
-  Affine<F> r = xyzz_to_affine(A);
+  }  // op 4: none (the affine conversion by the vartime inversion)
+  Affine<F> r = op == 4 ? xyzz_to_affine<F, true>(A) : xyzz_to_affine(A);
   store(out, r.x.from_mont());
   store(out + W, r.y.from_mont());
 }
@@ -44,8 +44,10 @@ void jac_ops(int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
 }  // namespace
 
 extern "C" {
-// op: 0 add 1 sub 2 mul 3 inverse 4 neg ; field: 0 Fq, 1 Fr ; standard-form in/out
-void t_fp_op(int field, int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
+// op: 0 add 1 sub 2 mul 3 inverse 4 neg 5 sqr 6 inverse_vartime ; field: 0 Fq, 1 Fr ; standard-form in/out.
+// Returns 1 if the op left a Montgomery representative >= p (the conversion out of Montgomery form would hide it).
+int t_fp_op(int field, int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
+  int noncanon = 0;
   auto run = [&](auto tag) {
     using F = decltype(tag);
     F x = load<F>(a).to_mont(), y = load<F>(b).to_mont(), r;
@@ -54,14 +56,18 @@ void t_fp_op(int field, int op, const uint32_t* a, const uint32_t* b, uint32_t* 
       case 1: r = x - y; break;
       case 2: r = x * y; break;
       case 3: r = x.inverse(); break;
+      case 5: r = x.sqr(); break;
       case 6: r = x.inverse_vartime(); break;
       default: r = x.neg(); break;
     }
+    noncanon = r.geq_modulus();
     store(out, r.from_mont());
   };
   if (field == 0) run(Fq{}); else run(Fr{});
+  return noncanon;
 }
-void t_fq2_op(int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
+// op: 0 add 1 sub 2 mul 3 inverse 4 sqr 5 neg 6 inverse_vartime ; returns 1 if a component was left >= p (as t_fp_op)
+int t_fq2_op(int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
   Fq2 x = load<Fq2>(a).to_mont(), y = load<Fq2>(b).to_mont(), r;
   switch (op) {
     case 0: r = x + y; break;
@@ -73,6 +79,7 @@ void t_fq2_op(int op, const uint32_t* a, const uint32_t* b, uint32_t* out) {
     default: r = x.neg(); break;
   }
   store(out, r.from_mont());
+  return r.geq_modulus();
 }
 // w[0..16) = a * b as plain 512-bit integers (any 256-bit operands)
 void t_mul_full(int k, const uint32_t* a, const uint32_t* b, uint32_t* w) {

@@ -1,7 +1,9 @@
 """CPU unit tests of the kernel arithmetic headers (fp.cuh / fp2.cuh / ec.cuh)
 compiled for the host through the carry-flag emulation in hd.cuh, checked
-against the oracle.  Exercises exactly the chain logic the device code runs;
-no GPU needed.  (The -m gpu tests repeat this on the device.)"""
+against the oracle.  Exercises the chain logic the device code runs, on the
+edge vectors of tests/arith_edges.py; no GPU needed.  tests/test_gpu_arith.py
+(-m gpu) runs the same vectors through the same headers compiled by nvcc for
+sm_90a, in both the inlined and the outlined build variants."""
 import ctypes
 import os
 import random
@@ -9,6 +11,7 @@ import random
 import numpy as np
 import pytest
 
+import arith_edges
 import build as b200build
 from oracle import ref_py as o
 
@@ -42,6 +45,14 @@ def call(fn, *args, nout):
     return from_u32(out, nout)
 
 
+def call_canon(fn, *args, nout):
+    """call() of t_fp_op / t_fq2_op that also requires the Montgomery result to be canonical (< p): the conversion out
+    of Montgomery form reduces, so a missing final subtraction shows only in this flag."""
+    out = np.zeros(8 * nout, dtype=np.uint32)
+    assert fn(*args, ptr(out)) == 0, "Montgomery result >= p"
+    return from_u32(out, nout)
+
+
 EDGE = [0, 1, 2, 3]
 
 
@@ -51,6 +62,27 @@ def samples(p, rng, k=200):
     return vals
 
 
+@pytest.mark.parametrize("field,p", [(0, Q), (1, R)], ids=["Fq", "Fr"])
+def test_fp_edge_pairs(lib, field, p):
+    """Every pair of the shared edge set (standard-form edges and their Montgomery preimages) through add, sub and mul,
+    every edge through neg, sqr and both inversions, and geq_modulus at either side of p."""
+    E = arith_edges.edges(p)
+    bufs = [to_u32([v]) for v in E]
+    for a, A in zip(E, bufs):
+        for b, B in zip(E, bufs):
+            assert call_canon(lib.t_fp_op, field, 0, ptr(A), ptr(B), nout=1)[0] == (a + b) % p, (hex(a), hex(b))
+            assert call_canon(lib.t_fp_op, field, 1, ptr(A), ptr(B), nout=1)[0] == (a - b) % p, (hex(a), hex(b))
+            assert call_canon(lib.t_fp_op, field, 2, ptr(A), ptr(B), nout=1)[0] == a * b % p, (hex(a), hex(b))
+        assert call_canon(lib.t_fp_op, field, 4, ptr(A), ptr(A), nout=1)[0] == (-a) % p, hex(a)
+        assert call_canon(lib.t_fp_op, field, 5, ptr(A), ptr(A), nout=1)[0] == a * a % p, hex(a)
+        inv = pow(a, -1, p) if a else 0
+        assert call_canon(lib.t_fp_op, field, 3, ptr(A), ptr(A), nout=1)[0] == inv, hex(a)
+        assert call_canon(lib.t_fp_op, field, 6, ptr(A), ptr(A), nout=1)[0] == inv, hex(a)
+        assert lib.t_geq(field, ptr(A)) == 0, hex(a)
+    for v in (p, p + 1, p + (1 << 32), (1 << 256) - 1, (1 << 255), p | 0xffffffff):
+        assert lib.t_geq(field, ptr(to_u32([v]))) == 1, hex(v)
+
+
 @pytest.mark.parametrize("field,p", [(0, Q), (1, R)])
 def test_fp_ops(lib, field, p):
     rng = random.Random(1234 + field)
@@ -58,18 +90,18 @@ def test_fp_ops(lib, field, p):
     for i, a in enumerate(vs):
         b = vs[(i * 7 + 3) % len(vs)]
         A, B = to_u32([a]), to_u32([b])
-        assert call(lib.t_fp_op, field, 0, ptr(A), ptr(B), nout=1)[0] == (a + b) % p
-        assert call(lib.t_fp_op, field, 1, ptr(A), ptr(B), nout=1)[0] == (a - b) % p
-        assert call(lib.t_fp_op, field, 2, ptr(A), ptr(B), nout=1)[0] == (a * b) % p
-        assert call(lib.t_fp_op, field, 4, ptr(A), ptr(B), nout=1)[0] == (-a) % p
+        assert call_canon(lib.t_fp_op, field, 0, ptr(A), ptr(B), nout=1)[0] == (a + b) % p
+        assert call_canon(lib.t_fp_op, field, 1, ptr(A), ptr(B), nout=1)[0] == (a - b) % p
+        assert call_canon(lib.t_fp_op, field, 2, ptr(A), ptr(B), nout=1)[0] == (a * b) % p
+        assert call_canon(lib.t_fp_op, field, 4, ptr(A), ptr(B), nout=1)[0] == (-a) % p
     for a in vs[:40]:
         A = to_u32([a])
         exp = pow(a, -1, p) if a else 0
-        assert call(lib.t_fp_op, field, 3, ptr(A), ptr(A), nout=1)[0] == exp
+        assert call_canon(lib.t_fp_op, field, 3, ptr(A), ptr(A), nout=1)[0] == exp
     for a in vs + [1 << k for k in range(0, 254, 7)] + [p - (1 << k) for k in range(1, 250, 11)]:
         A = to_u32([a])                               # binary-Euclid inversion: same value as a^(p-2)
         exp = pow(a, -1, p) if a else 0
-        assert call(lib.t_fp_op, field, 6, ptr(A), ptr(A), nout=1)[0] == exp
+        assert call_canon(lib.t_fp_op, field, 6, ptr(A), ptr(A), nout=1)[0] == exp
     assert lib.t_geq(field, ptr(to_u32([p]))) == 1
     assert lib.t_geq(field, ptr(to_u32([p - 1]))) == 0
     assert lib.t_geq(field, ptr(to_u32([(1 << 256) - 1]))) == 1
@@ -120,6 +152,40 @@ def test_fq2_ops(lib):
         if a != (0, 0) and i < 25:
             assert tuple(call(lib.t_fq2_op, 3, ptr(A), ptr(B), nout=2)) == F2.inverse(a)  # fq2.go:99-108
             assert tuple(call(lib.t_fq2_op, 6, ptr(A), ptr(B), nout=2)) == F2.inverse(a)
+
+
+def test_wide_edges(lib):
+    """mul_full on every pair of the shared wide edges (up to (2^256 - 1)^2) and redc_wide on the shared reduction edges
+    (up to t = p * 2^256 - 1), for both moduli."""
+    W = arith_edges.wide_edges()
+    for a in W:
+        for b in W:
+            out = np.zeros(16, dtype=np.uint32)
+            lib.t_mul_full(0, ptr(to_u32([a])), ptr(to_u32([b])), ptr(out))
+            assert int.from_bytes(out.tobytes(), "little") == a * b, (hex(a), hex(b))
+    for field, p in ((0, Q), (1, R)):
+        rinv = pow(1 << 256, -1, p)
+        for t in arith_edges.redc_edges(p):
+            out = np.zeros(8, dtype=np.uint32)
+            lib.t_redc_wide(field, 0, ptr(np.frombuffer(t.to_bytes(64, "little"), dtype=np.uint32).copy()), ptr(out))
+            assert int.from_bytes(out.tobytes(), "little") == t * rinv % p, (field, hex(t))
+
+
+def test_fq2_edge_components(lib):
+    """F_q^2 products, squares, sums and differences with components drawn from the shared edge set, including the
+    lazy-reduction extremes in Montgomery form: a0 b0 = 0 with a1 b1 maximal (the representatives p - 1) and the reverse."""
+    F2 = o.BN.Fq2
+    E = arith_edges.edges(Q)
+    m1 = arith_edges.montgomery_preimages(Q, [Q - 1])[0]       # Montgomery representative p - 1
+    pairs = [((0, m1), (x, m1)) for x in E] + [((m1, 0), (m1, x)) for x in E]
+    rng = random.Random(5)
+    pairs += [((rng.choice(E), rng.choice(E)), (rng.choice(E), rng.choice(E))) for _ in range(1500)]
+    for a, b in pairs:
+        A, B = to_u32(a), to_u32(b)
+        assert tuple(call_canon(lib.t_fq2_op, 2, ptr(A), ptr(B), nout=2)) == F2.mul(a, b), (a, b)
+        assert tuple(call_canon(lib.t_fq2_op, 0, ptr(A), ptr(B), nout=2)) == F2.add(a, b), (a, b)
+        assert tuple(call_canon(lib.t_fq2_op, 1, ptr(A), ptr(B), nout=2)) == F2.sub(a, b), (a, b)
+        assert tuple(call_canon(lib.t_fq2_op, 4, ptr(A), ptr(B), nout=2)) == F2.square(a), a
 
 
 def test_fq2_lazy_reduction_extremes(lib):
