@@ -10,7 +10,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libb200snark.so")
 CFG_ACC_MODE, ACC_AUTO, ACC_AFFINE, ACC_XYZZ = 1, 0, 1, 2
 CFG_TMA_STAGING = 2
 CFG_SHARD_W_AB, CFG_SHARD_W_G2, CFG_SHARD_AFFINE_MIN_G1, CFG_SHARD_AFFINE_MIN_G2 = 10, 11, 12, 13
-CFG_PAIRING_KERNEL = 5  # b200_pairing_batch: 0 default (one warp per pairing), 1 one thread per pairing, 2 one warp
+CFG_PAIRING_KERNEL = 5  # b200_pairing_batch: 0 auto (a warp per pairing up to 2048, a thread above), 1 thread, 2 warp
 CFG_PK_CONTEXT = 4    # prove context (0 / 1) of proving keys loaded afterwards: two proofs in flight
 CFG_TABLE_WINDOWS = 14  # stored window rows t of base sets / keys loaded afterwards (0: all; fewer: less memory, slower)
 

@@ -42,9 +42,21 @@ def _unflatten_g2(arr):
 
 
 def reduce_scalar(e):
-    """What the cgo shim sends for a *big.Int scalar: |e| mod r (the reference's
-    MulScalar consumes |e| — Fq.Copy goes through Bytes(), fields/fq.go:138-140)."""
-    return abs(int(e)) % R
+    """The m in [0, r) with the reference's MulScalar(P, e) == m * P as group elements, for every P of order r.
+
+    MulScalar consumes |e| (Fq.Copy goes through Bytes(), fields/fq.go:138-140) and runs its MSB-first double-and-add
+    over every bit of it (bn128/g1.go:140-155, g2.go:142-181) with an Add that has no doubling branch (SURVEY H6).
+    Below r the accumulator never meets P, so m = |e|.  For |e| >= r it can: when the doubled prefix is P itself and the
+    next bit is set, Add(P, P) returns infinity and the walk restarts from there.  So m is |e| mod r only when no
+    prefix hits that case; e = r + 2 gives m = 0, not 2.  The C ABI takes m and refuses scalars >= r (B200_ERANGE)."""
+    e = abs(int(e))
+    if e < R:
+        return e
+    m = 0
+    for i in range(e.bit_length() - 1, -1, -1):
+        d = 2 * m % R
+        m = (0 if d == 1 else (d + 1) % R) if (e >> i) & 1 else d   # d == 1 and the bit set: Add(P, P) -> infinity
+    return m
 
 
 class BaseSet:
@@ -142,8 +154,8 @@ class _Group:
 
     def MulScalar(self, p, e):
         """bn128.G1.MulScalar / bn128.G2.MulScalar.  NOTE: the reference consumes
-        all bits of |e|; this mirror reduces mod r first (same group element;
-        identical X,Y,Z whenever |e| < r)."""
+        all bits of |e|; this mirror first maps e with reduce_scalar (the same
+        group element for every e; identical X,Y,Z whenever |e| < r)."""
         return self.MulScalarBatch([p], [e])[0]
 
     # element-wise group law with the reference's formulas (X,Y,Z-exact): g1.go:32-170 / g2.go:32-200

@@ -49,7 +49,9 @@ func limbs(dst []uint64, x *big.Int) []uint64 {
 }
 
 // Scalar is what crosses the ABI for a *big.Int scalar: |e| mod r (the reference's MulScalar
-// consumes |e|: fields/fq.go:138-140).
+// consumes |e|: fields/fq.go:138-140).  For |e| >= r that is not always the reference's group
+// element: its double-and-add meets Add(P, P) = infinity for crafted values such as r + 2.  The
+// Python binding's bn128.reduce_scalar has the rule that matches; this function does not have it yet.
 func Scalar(e *big.Int) *big.Int { return new(big.Int).Mod(new(big.Int).Abs(e), R) }
 
 // Coeff is what crosses the ABI for a polynomial coefficient: e mod r (Euclidean, like Fq.Add/Mul).

@@ -299,8 +299,10 @@ int b200_poly_eval_batch(const uint64_t* polys, size_t m, size_t n, const uint64
 int b200_zero_poly(size_t n, uint64_t* out);
 
 /* ---- verifier side (SURVEY §8f row 2) ------------------------------------------------------------------ */
-/* out[i] = Bn128.Pairing(g1[i], g2[i]) (bn128/bn128.go:179-186): optimal-ate Miller loop + the reference's plain
- * final exponentiation, one GPU thread per pairing; 48 uint64 per result in the reference's [2][3][2]*big.Int order.
+/* out[i] = Bn128.Pairing(g1[i], g2[i]) (bn128/bn128.go:179-186): optimal-ate Miller loop + a fast final
+ * exponentiation (easy part, then the hard part by the BN parameter) that gives the same F_q^12 value as the
+ * reference's plain f^((q^12-1)/r); 48 uint64 per result in the reference's [2][3][2]*big.Int order.  The kernel is
+ * B200_CFG_PAIRING_KERNEL's: by default one warp per pairing up to 2048 pairings per call, one thread per pairing above.
  * Bit-identical to the reference (golden: externalVerif/circom-test/verification_key.json vk_alfabeta_12).
  * A G2 point at infinity returns B200_EINVAL where the reference panics "q1[2] != Fq2.One()" (bn128.go:238-241);
  * a G1 point at infinity is processed like the reference does (Affine -> (0,0)).                                    */

@@ -112,7 +112,7 @@ def test_verify_many_public_signals_edge_values(mods):
             moved = list(pubs)
             moved[j] = (moved[j] + 1) % R
             assert not groth16.VerifyProof(vk, proof, moved), j
-        assert groth16.VerifyProof(vk, proof, [p + R for p in pubs])          # publicSignals are taken mod r (MulScalar of a big.Int)
+        assert groth16.VerifyProof(vk, proof, [p + R for p in pubs])          # p + r: MulScalar's walk gives p for these p (not for all)
     assert o.groth16_verify(vk, proof, pubs)
 
 
