@@ -176,6 +176,18 @@ def build_host_shard_batch(force=False):
     return target
 
 
+def build_host_short_z(force=False):
+    """g++ build of the quotient by len(Z) = n (circuits with m = n + 1 signals: k_short_z_lambda, k_short_z_dot,
+    k_quotient_store_shifted after the batched front end) over csrc/host_stub (CPU test vehicle, tests/test_host_short_z.py)."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    target = os.path.join(LIBDIR, "libb200_host_short_z.so")
+    if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):
+        return target
+    _run(["g++", "-O2", "-std=c++17", "-pthread", "-x", "c++", "-shared", "-fPIC", "-Wno-psabi", "-I", os.path.join(HOSTTEST, "host_stub"),
+          "-I", HOSTTEST, "-I", CSRC, "-o", target, os.path.join(HOSTTEST, "short_z_test.cpp")])
+    return target
+
+
 def build_shard_partition(force=False):
     """g++ build of csrc/shard_partition.h behind a C entry point (CPU test vehicle, tests/test_shard_partition.py)."""
     os.makedirs(LIBDIR, exist_ok=True)

@@ -840,10 +840,13 @@ int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint6
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
-  // h = (ax*bx - cx) / Z straight from the witness (no px): the shape the reference supports has Z = prod_{i<=n}(x - i)
-  // (m = n + 2, SURVEY H5) — checked; anything else goes through px and the division.
-  if (r1->n >= 2 && pk->Z.nb == r1->n + 1) {
-    if ((rc = qap_h_enqueue(r1, *ws, *pk->pctx().poly, d_w, err, sq))) return rc;
+  // h = (ax*bx - cx) / Z straight from the witness (no px): the shapes whose proofs can verify have Z = prod_{i<=n}(x - i)
+  // (m = n + 2, SURVEY H5) or Z = prod_{i<n}(x - i) (m = n + 1: h = (x - n) q + kappa, qap_sparse.cuh) — checked; anything
+  // else goes through px and the division.
+  if (r1->n >= 2 && (pk->Z.nb == r1->n + 1 || pk->Z.nb == r1->n)) {
+    if (pk->Z.nb == r1->n + 1) rc = qap_h_enqueue(r1, *ws, *pk->pctx().poly, d_w, err, sq);
+    else rc = qap_h_short_enqueue(r1, *ws, *pk->pctx().poly, d_w, err, sq);
+    if (rc) return rc;
     return groth16_enqueue(pk, d_w, pk->m, nullptr, npx, r, s, d_out, st, err, 0, ws->h_std.as<Fr>());
   }
   if ((rc = qap_px_enqueue(r1, *ws, *pk->pctx().poly, d_w, nullptr, nullptr, err, sq))) return rc;
@@ -869,8 +872,9 @@ int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t
 
 // ---- batches: k witness-fed proofs under one key (b200_groth16_prove_witness_batch) ---------------------------------
 // Proof p is the proof of groth16_witness_enqueue for (w_p, r_p, s_p).  The four MSMs run as batched MSMs over k scalar
-// vectors (W_p = w_p ++ [1, r_p, s_p] for A, B1, B2 with one shared sort; C||PTD_p), the h-direct quotients as one batched
-// front end (qap_h_batch_enqueue), the blinding products with one warp per proof: the launches of one proof, whatever k.
+// vectors (W_p = w_p ++ [1, r_p, s_p] for A, B1, B2 with one shared sort; C||PTD_p), the quotients as one batched front
+// end (len(Z) = n + 1: qap_h_batch_enqueue; len(Z) = n: qap_h_short_batch_enqueue), the blinding products with one warp
+// per proof: the launches of one proof, whatever k.
 // On a key shard every vector is the rank's part of it (G16Slices), and the batch ends in k partial records.
 
 // Everything that is refused before anything is allocated or enqueued.  On a key shard every refusal is decided on
@@ -941,6 +945,7 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
                         Fq* d_proofs, uint8_t* d_recs, cudaStream_t st, int* err, R1csBatch** fb_used) {
   const size_t m = pk->m, l1 = pk->npublic + 1, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
   const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as groth16_witness_enqueue
+  const bool short_z = r1->n >= 2 && pk->Z.nb == r1->n;        // m = n + 1: the same front end, h = (x - n) q + kappa
   const G16Slices sl = g16_slices(pk, pk->rank);
   size_t woff[3];
   g16_w_layout(pk, sl, woff);
@@ -966,7 +971,8 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
   int rc;
   if (quotient) {
     if ((rc = r1cs_work(r1, pk->ctx, &ws))) return rc;
-    if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+    if ((h_direct || short_z) && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+    if (short_z && (rc = r1cs_short_u(r1))) return rc;
   }
   *fb_used = fb;
   if ((rc = groth16_batch_scratch(pk, k, false))) return rc;
@@ -1025,6 +1031,9 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
       if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
       k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)n_p,
                                                           tail, 4, qtotal, chq, (uint32_t)nch, (uint32_t)sl.p_lo);
+      g_launches += 1;
+    } else if (short_z) {   // the store is part of it
+      if ((rc = qap_h_short_batch_enqueue(r1, *fb, pc, d_w, k, err, s3, chq, nch, n_p, sl.p_lo, tail))) return rc;
     } else {   // not batched: the single-witness px and division of each witness, into its vector (a shard: its slice)
       const bool direct = sl.p_lo == 0 && nq <= n_p;
       const size_t have = nq > sl.p_lo ? std::min(nq - sl.p_lo, n_p) : 0;   // quotient coefficients inside the slice
@@ -1036,8 +1045,8 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
       }
       k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)n_p, tail, 4, qtotal, chq,
                                                           (uint32_t)nch, (uint32_t)sl.p_lo);
+      g_launches += 1;
     }
-    g_launches += 1;
   }
   MsmShape sh;
   if (Bases* gch = pk->g[3].get()) {
@@ -1177,8 +1186,10 @@ int pinocchio_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, Fq* d_out
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
   PolyCtx& pc = *pk->pctx().poly;
-  if (r1->n >= 2 && pk->Z.nb == r1->n + 1) {   // h-direct, as groth16_witness_enqueue
-    if ((rc = qap_h_enqueue(r1, *ws, pc, d_w, err, sq))) return rc;
+  if (r1->n >= 2 && (pk->Z.nb == r1->n + 1 || pk->Z.nb == r1->n)) {   // h-direct, as groth16_witness_enqueue
+    if (pk->Z.nb == r1->n + 1) rc = qap_h_enqueue(r1, *ws, pc, d_w, err, sq);
+    else rc = qap_h_short_enqueue(r1, *ws, pc, d_w, err, sq);
+    if (rc) return rc;
     return pinocchio_enqueue(pk, d_w, nullptr, npx, 0, ws->h_std.as<Fr>(), d_out, record, st, err);
   }
   if ((rc = qap_px_enqueue(r1, *ws, pc, d_w, nullptr, nullptr, err, sq))) return rc;
@@ -1265,6 +1276,7 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
                           int* err, R1csBatch** fb_used) {
   const size_t m = pk->m, l1 = pk->npublic + 1, ng = pk->n_h_bases, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
   const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as pinocchio_witness_enqueue
+  const bool short_z = r1->n >= 2 && pk->Z.nb == r1->n;
   const size_t terms[8] = {m - l1, m - l1, m, m, m, m, m, ng};
   // the set that sorts for set j: the first set of j's group (kPinSortSrc) this key holds
   int src[8];
@@ -1279,7 +1291,8 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
   int rc;
   if (pk->g[7]) {
     if ((rc = r1cs_work(r1, pk->ctx, &ws))) return rc;
-    if (h_direct && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+    if ((h_direct || short_z) && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
+    if (short_z && (rc = r1cs_short_u(r1))) return rc;
   }
   *fb_used = fb;
   if ((rc = pinocchio_batch_scratch(pk, k, false))) return rc;
@@ -1334,14 +1347,17 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
       if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
       k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)ng,
                                                           nullptr, 0, qtotal, H, (uint32_t)ng);
+      g_launches += 1;
+    } else if (short_z) {   // the store is part of it
+      if ((rc = qap_h_short_batch_enqueue(r1, *fb, pc, d_w, k, err, s3, H, ng, ng, 0, nullptr))) return rc;
     } else {   // not batched: the single-witness px and division of each witness, straight into its vector
       for (size_t p = 0; p < k; p++) {
         if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
         CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, H + p * ng, nullptr, err, s3));
       }
       k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)ng, nullptr, 0, qtotal, H, (uint32_t)ng);
+      g_launches += 1;
     }
-    g_launches += 1;
     if ((rc = sort_of(7, H, ng, s3))) return rc;
     if ((rc = buckets_of(7, s3))) return rc;
   }

@@ -576,6 +576,87 @@ inline cudaError_t qap_h_batch(PolyCtx& pc, const QapDomain& dom, QapWork& wk, Q
   return qap_h_from_newton(pc, hd, d, dom.N, st, ws, k);
 }
 
+// ---- the quotient by Z_n = prod_{i=1..n-1}(x - i): circuits with m = n + 1 signals (len(Z) = n) --------------------------
+// The branch above gives q = quotient(a b - c', Z_{n+1}), n - 1 coefficients, with a b - c' = Z_{n+1} q exactly.  Since
+// Z_{n+1} = Z_n (x - n) and c' - c has degree <= n - 1 = deg Z_n, DivisorPolynomial(a b - c, Z_n) is, for ANY witness,
+//     h = (x - n) q + kappa,    kappa = sum_j (a_j b_j - c_j) lambda_j,    lambda_j = (-1)^(n-1-j) / (j! (n-1-j)!)
+// (j = 0 .. n-1 for the point j + 1): kappa is the x^(n-1) coefficient of the interpolant of c' - c, its top divided
+// difference.  sum_j a_j b_j lambda_j is the top Newton coefficient d_{n-1} of the products block, which newton_coeffs
+// already computes; sum_j c_j lambda_j = w . u with u = C^T lambda, one m-vector per R1CS, so C w is still never formed.
+// What the branch adds per call: one dot product per witness (k_short_z_dot, per-block partials summed by the thread of
+// the store that writes h[0]) and the shifted store in place of k_quotient_store / k_poly_store.  Field addition is
+// exact, so the order of the sums does not change a bit of h.
+constexpr uint32_t kShortZDotThreads = 256;
+constexpr uint32_t kShortZDotBlocks = 32;   // partial sums per witness, at most
+inline uint32_t short_z_dot_blocks(size_t m) {
+  const size_t b = (m + kShortZDotThreads - 1) / kShortZDotThreads;
+  return b < kShortZDotBlocks ? (uint32_t)b : kShortZDotBlocks;
+}
+// lam[j] = (-1)^(n-1-j) / (j! (n-1-j)!), j < n: the weights of the top divided difference over {1..n}
+__global__ void k_short_z_lambda(const Fr* __restrict__ invfact, uint32_t n, Fr* __restrict__ lam) {
+  uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  Fr v = invfact[j] * invfact[n - 1 - j];
+  lam[j] = ((n - 1 - j) & 1) ? v.neg() : v;
+}
+// Block b of witness p (blockIdx.x = p * nb + b; one-dimensional, so any k fits): the partial sum over the signals
+// i = b * blockDim + t (mod nb * blockDim) of u_i * w_p,i, w signal-major (w_p,i at w[i * k + p], Montgomery: what
+// k_witness_load_batch writes; k = 1: one witness vector) -> partial[p * nb + b].
+__global__ void __launch_bounds__(kShortZDotThreads) k_short_z_dot(const Fr* __restrict__ u, const Fr* __restrict__ w, uint32_t m,
+                                                                   uint32_t k, uint32_t nb, Fr* __restrict__ partial) {
+  __shared__ Fr red[kShortZDotThreads];
+  const uint32_t p = blockIdx.x / nb, b = blockIdx.x - p * nb, t = threadIdx.x;
+  Fr acc = Fr::zero();
+  for (uint32_t i = b * blockDim.x + t; i < m; i += nb * blockDim.x) acc = acc + u[i] * w[(size_t)i * k + p];
+  red[t] = acc;
+  __syncthreads();
+  for (uint32_t h = blockDim.x / 2; h; h >>= 1) {
+    if (t < h) red[t] = red[t] + red[t + h];
+    __syncthreads();
+  }
+  if (t == 0) partial[blockIdx.x] = red[0];
+}
+// As k_quotient_store, for h = (x - n) q + kappa (nh = n coefficients): slot i of vector p holds h_p[off + i] in standard
+// form, h[g] = q[g-1] - n q[g] (q[-1] = q[n-1] = 0; q_p at coef + p * cstride, Montgomery; nm = n, Montgomery) and at
+// g = 0 also kappa_p = top[p * top_stride] - sum of the nb partials at partial + p * nb; zeros for g >= nh; then the tail.
+// off > 0: a key shard whose PowersTauDelta slice starts at index off (only global index 0 takes kappa).
+__global__ void k_quotient_store_shifted(const Fr* __restrict__ coef, uint32_t cstride, uint32_t nh, Fr nm,
+                                         const Fr* __restrict__ top, uint32_t top_stride, const Fr* __restrict__ partial,
+                                         uint32_t nb, uint32_t n_ptd, const Fr* __restrict__ tail, uint32_t tstride,
+                                         uint32_t total, Fr* __restrict__ ch, uint32_t stride, uint32_t off) {
+  uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  uint32_t p = e / (n_ptd + 1), i = e - p * (n_ptd + 1);
+  Fr* d = ch + (size_t)p * stride + i;
+  if (i < n_ptd) {
+    const size_t g = (size_t)off + i;
+    if (g >= nh) {
+      *d = Fr::zero();
+      return;
+    }
+    const Fr* q = coef + (size_t)p * cstride;
+    Fr v = g + 1 < nh ? (q[g] * nm).neg() : Fr::zero();
+    if (g) {
+      v = v + q[g - 1];
+    } else {
+      Fr s = Fr::zero();
+      for (uint32_t b = 0; b < nb; b++) s = s + partial[(size_t)p * nb + b];
+      v = v + (top[(size_t)p * top_stride] - s);
+    }
+    *d = v.from_mont();
+  } else if (tail) {
+    *d = tail[(size_t)p * tstride];
+  }
+}
+// The dot products of k witnesses (wt: [m][k], Montgomery) against u: short_z_dot_blocks(m) partials per witness at
+// partial + p * nb.  One launch, whatever k.
+inline cudaError_t short_z_dot(PolyCtx& pc, const Fr* u, const Fr* wt, size_t m, int k, Fr* partial, cudaStream_t st) {
+  const uint32_t nb = short_z_dot_blocks(m);
+  B200_LAUNCH_CTA(k_short_z_dot, nb * (uint32_t)k, kShortZDotThreads, st, u, wt, (uint32_t)m, (uint32_t)k, nb, partial);
+  pc.note(1);
+  return cudaGetLastError();
+}
+
 // ---- a sparse R1CS resident on the device ------------------------------------------------------------------
 struct SparseMat {
   DevBuf rowptr, col, val;      // CSR (n rows)
@@ -586,6 +667,7 @@ struct SparseMat {
 struct R1csBatchWork {
   size_t k = 0;
   DevBuf wt, vals, coef;            // witnesses [m][k]; A w_p | B w_p | products (3k x n); Newton coefficients (3k x N)
+  DevBuf part;                      // len(Z) = n: the k_short_z_dot partials (k x short_z_dot_blocks(m))
   QapWork work;
   QapHWork hw;
   virtual ~R1csBatchWork() = default;
@@ -596,7 +678,8 @@ struct R1csWork {
   DevBuf w_mont, vals, coef;        // witness (m), A w | B w | C w (3 x n; the quotient path: A w | B w | their products),
                                     // coefficients (3 x N), all Montgomery
   DevBuf px_mont;                   // 2n - 1
-  DevBuf h_std;                     // h = px / Z, n - 1 coefficients, standard form (h-direct branch)
+  DevBuf h_std;                     // h = px / Z, standard form: n - 1 coefficients (h-direct branch), n (len(Z) = n)
+  DevBuf part;                      // len(Z) = n: the k_short_z_dot partials of one witness
   QapWork work;
   QapHWork hw;
   std::unique_ptr<R1csBatchWork> batch;   // batches of witnesses (allocated on the first batch)
@@ -606,6 +689,7 @@ struct R1cs {
   SparseMat M[3];
   DevBuf lag;                       // Lagrange basis at tau (n): the trusted setup
   std::unique_ptr<QapHDomain> hd;   // witness -> h directly (b200_groth16_prove_witness), built on first use
+  std::unique_ptr<DevBuf> short_u;  // u = C^T lambda (m, Montgomery): the quotient by len(Z) = n, built on first use
   std::unique_ptr<R1csWork> ws[2];  // per prove context, allocated on first use
 };
 

@@ -102,6 +102,7 @@ int r1cs_work(R1cs* r, int ctx, R1csWork** out) {
     CU(w->coef.alloc(3 * N * sizeof(Fr)));
     CU(w->px_mont.alloc((2 * n) * sizeof(Fr)));
     CU(w->h_std.alloc(n * sizeof(Fr)));
+    CU(w->part.alloc(kShortZDotBlocks * sizeof(Fr)));
     ws = std::move(w);
   }
   *out = ws.get();
@@ -160,9 +161,10 @@ int r1cs_hdomain(R1cs* r, QapDomain** dom) {
 // coefficients of h = DivisorPolynomial(ax*bx - cx, Z) in ws.h_std (standard form), without forming px (qap_sparse.cuh:
 // QapHDomain).  The quotient does not depend on cx, so C w is not computed.  Requires n >= 2.  The domains are shared by
 // every context: built on g_ctx[0].main and waited for on the first call.
-int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
+// The witness load and the quotient q by Z_{n+1} (Montgomery, ws.hw.coef), from the Newton coefficients of a | b | a*b that
+// it leaves in ws.coef (N-strided) and the witness (Montgomery) in ws.w_mont.  Requires n >= 2.
+int qap_q_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
   const size_t n = r->n, m = r->m;
-  if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
   QapDomain* dom;
   int rc = r1cs_hdomain(r, &dom);
   if (rc) return rc;
@@ -175,6 +177,14 @@ int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* er
   g_launches += 3;
   Fr* coef = ws.coef.as<Fr>();   // here: the Newton coefficients of a | b | a*b (N-strided)
   CU(qap_h_from_values(pc, *dom, ws.work, *r->hd, vals, coef, st, &ws.hw));
+  return B200_OK;
+}
+
+int qap_h_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
+  const size_t n = r->n;
+  if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
+  int rc = qap_q_enqueue(r, ws, pc, d_w_std, err, st);
+  if (rc) return rc;
   k_poly_store<<<nblk(n - 1, 256), 256, 0, st>>>(ws.hw.coef.as<Fr>(), (uint32_t)(n - 1), 0, 1, ws.h_std.as<Fr>());
   g_launches += 1;
   CU(cudaGetLastError());
@@ -187,7 +197,7 @@ struct R1csBatch : R1csBatchWork {
   ~R1csBatch() override { if (done) cudaEventDestroy(done); }
 };
 
-// Before a batch of k witnesses on the h-direct branch: builds the domains (first use) and grows the workspace's batch
+// Before a batch of k witnesses on the h-direct branch or the len(Z) = n one: builds the domains (first use) and grows the workspace's batch
 // scratch to k witnesses, every buffer the batch touches included, so that enqueueing it allocates nothing.  A regrowth
 // first waits for the last batch that used the scratch, not for the device.
 int qap_batch_prepare(R1cs* r, R1csWork& ws, size_t k, R1csBatch** out) {
@@ -206,6 +216,7 @@ int qap_batch_prepare(R1cs* r, R1csWork& ws, size_t k, R1csBatch** out) {
     CU(b->wt.alloc(m * k * F));
     CU(b->vals.alloc(3 * k * n * F));
     CU(b->coef.alloc(3 * k * N * F));
+    CU(b->part.alloc(k * kShortZDotBlocks * F));
     CU(b->work.U.alloc(3 * k * 2 * N * F));
     CU(b->hw.V.alloc(3 * k * M * F));
     CU(b->hw.hv.alloc(k * n * F));
@@ -321,6 +332,68 @@ __global__ void k_spmv_t(const uint32_t* __restrict__ cptr, const uint32_t* __re
   for (uint32_t k = cptr[i], e = cptr[i + 1]; k < e; k++) acc = acc + cval[k] * l[crow[k]];
   out[i] = acc;
 }
+
+// ---- the quotient by len(Z) = n (m = n + 1 signals): h = (x - n) q + kappa (qap_sparse.cuh) -----------------------------
+// u = C^T lambda of r, built on g_ctx[0].main and waited for on first use; shared by both prove contexts.
+int r1cs_short_u(R1cs* r) {
+  if (r->short_u) return B200_OK;
+  const size_t n = r->n, m = r->m;
+  QapDomain* dom;
+  int rc = get_domain(pow2_at_least(n), &dom);
+  if (rc) return rc;
+  cudaStream_t st = g_ctx[0].main;
+  auto u = std::make_unique<DevBuf>();
+  DevBuf lam;
+  CU(lam.alloc(n * sizeof(Fr)));
+  CU(u->alloc(m * sizeof(Fr)));
+  k_short_z_lambda<<<nblk(n, 256), 256, 0, st>>>(dom->invfact.as<Fr>(), (uint32_t)n, lam.as<Fr>());
+  k_spmv_t<<<nblk(m, 128), 128, 0, st>>>(r->M[2].cptr.as<uint32_t>(), r->M[2].crow.as<uint32_t>(), r->M[2].cval.as<Fr>(),
+                                          lam.as<Fr>(), (uint32_t)m, u->as<Fr>());
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));   // lam is freed on return
+  r->short_u = std::move(u);
+  return B200_OK;
+}
+
+// h_p[off + i] (i < n_ptd) of k quotients into the vectors at vec + p * stride, standard form, zeros beyond len(h) = n,
+// then tail[4p] when given (k_quotient_store_shifted).  q: quotient p at q + p * qstride; d: the Newton coefficients of
+// a | b | a*b of witness p at d + 3p * N; part: the k_short_z_dot partials.
+int qap_short_store(R1cs* r, const Fr* q, size_t qstride, const Fr* d, const Fr* part, size_t k, Fr* vec, size_t stride,
+                    size_t n_ptd, size_t off, const Fr* tail, cudaStream_t st) {
+  const size_t n = r->n, N = pow2_at_least(n);
+  const uint32_t total = (uint32_t)(k * (n_ptd + 1));
+  k_quotient_store_shifted<<<nblk(total, 256), 256, 0, st>>>(q, (uint32_t)qstride, (uint32_t)n, fr_from_u64(n), d + 2 * N + (n - 1),
+                                                             (uint32_t)(3 * N), part, short_z_dot_blocks(r->m), (uint32_t)n_ptd, tail, 4,
+                                                             total, vec, (uint32_t)stride, (uint32_t)off);
+  g_launches += 1;
+  CU(cudaGetLastError());
+  return B200_OK;
+}
+
+// qap_h_enqueue for len(Z) = n: the n coefficients of h = DivisorPolynomial(ax*bx - cx, Z_n) in ws.h_std (standard form),
+// from the same front end plus one dot product; C w is not computed.  Requires n >= 2.
+int qap_h_short_enqueue(R1cs* r, R1csWork& ws, PolyCtx& pc, const Fr* d_w_std, int* err, cudaStream_t st) {
+  const size_t n = r->n;
+  if (n < 2) return fail(B200_EINVAL, "qap_h: needs at least 2 constraints");
+  int rc = r1cs_short_u(r);
+  if (rc) return rc;
+  if ((rc = qap_q_enqueue(r, ws, pc, d_w_std, err, st))) return rc;
+  CU(short_z_dot(pc, r->short_u->as<Fr>(), ws.w_mont.as<Fr>(), r->m, 1, ws.part.as<Fr>(), st));
+  return qap_short_store(r, ws.hw.coef.as<Fr>(), 0, ws.coef.as<Fr>(), ws.part.as<Fr>(), 1, ws.h_std.as<Fr>(), n, n, 0, nullptr, st);
+}
+
+// qap_h_batch_enqueue for len(Z) = n, quotients included: h_p[off + i] (i < n_ptd) into vec + p * stride (standard form,
+// zeros beyond len(h) = n), then tail[4p] when given.  After qap_batch_prepare for >= k.  The launches of
+// qap_h_batch_enqueue plus k_short_z_dot, whatever k; the store takes the place of k_quotient_store.
+int qap_h_short_batch_enqueue(R1cs* r, R1csBatch& b, PolyCtx& pc, const Fr* d_w, size_t k, int* err, cudaStream_t st, Fr* vec,
+                              size_t stride, size_t n_ptd, size_t off, const Fr* tail) {
+  int rc = r1cs_short_u(r);
+  if (rc) return rc;
+  if ((rc = qap_h_batch_enqueue(r, b, pc, d_w, k, err, st))) return rc;
+  CU(short_z_dot(pc, r->short_u->as<Fr>(), b.wt.as<Fr>(), r->m, (int)k, b.part.as<Fr>(), st));
+  return qap_short_store(r, b.hw.coef.as<Fr>(), r->hd->tree.N, b.coef.as<Fr>(), b.part.as<Fr>(), k, vec, stride, n_ptd, off, tail, st);
+}
+
 // Enqueues at | bt | ct (Montgomery, m each) into d_out on `st`; *zt = prod_{i=1..nz}(tau - i) (Montgomery).  t: tau in
 // Montgomery form.  tau in 1..n sets bit 4 of g_d_err.
 int qap_eval_at_enqueue(R1cs* r, Fr t, size_t nz, Fr* d_out, Fr* zt, cudaStream_t st) {

@@ -79,7 +79,7 @@ class SyntheticGroth16:
         h = _lib._h(0)
         check(lib().b200_groth16_pk_load_shard(
             ptr(self.at), ptr(self.b1), ptr(self.b2), ptr(self.cd), self.m, ptr(self.ptd), self.n_ptd,
-            ptr(self.z), self.n + 1, ptr(self.alpha1), ptr(self.beta1), ptr(self.delta1), ptr(self.beta2),
+            ptr(self.z), self.z.shape[0], ptr(self.alpha1), ptr(self.beta1), ptr(self.delta1), ptr(self.beta2),
             ptr(self.delta2), self.npublic, window_bits, rank, world, h))
         return h.value
 
@@ -121,10 +121,17 @@ class SyntheticCircuit:
         (x_0 + 5) * x_0 = x_1;     x_k * x_{k-1} = x_{k+1}  (k = 1 .. n-2);     x_{n-1} * x_{n-2} = pub
 
     1-2 non-zeros per row of A, one in B, one in C (coefficients 1 and the 5 of README.md:174).  CSR arrays are numpy;
-    the witness is the chain evaluated mod r from a seeded x_0 (NPublic = 1: the last product)."""
+    the witness is the chain evaluated mod r from a seeded x_0 (NPublic = 1: the last product).
 
-    def __init__(self, n, seed=SEED_WITNESS):
+    ``short_z=True``: the m = n + 1 variant, n constraints over [one, pub, c_0 .. c_{n-2}] — the linear row c_0 * one = c_0,
+    then the n - 1 products of the same chain (c_0 + 5) * c_0 = c_1, c_k * c_{k-1} = c_{k+1}, the last one into pub.  Its
+    Z has length m - 1 = n."""
+
+    def __init__(self, n, seed=SEED_WITNESS, short_z=False):
         assert n >= 2
+        if short_z:
+            self._init_short(n, seed)
+            return
         self.n, self.m, self.npublic = n, n + 2, 1
         j = np.arange(n, dtype=np.uint32)
         # A: row 0 = {x_0: 1, one: 5}, row j = {x_j: 1}
@@ -147,6 +154,29 @@ class SyntheticCircuit:
         self.witness = [1, pub] + xs[:n]
         self.public_signals = [pub]
 
+    def _init_short(self, n, seed):
+        self.n, self.m, self.npublic = n, n + 1, 1
+        j = np.arange(2, n, dtype=np.uint32)                                   # product rows 2 .. n-1
+        rowptr1 = np.arange(n + 1, dtype=np.uint32)
+        # A: row 0 = {c_0}, row 1 = {one: 5, c_0}, row j = {c_{j-1}};  B: row 0 = {one}, row 1 = {c_0}, row j = {c_{j-2}}
+        a_rowptr = np.concatenate(([0, 1], 3 + np.arange(n - 1, dtype=np.uint32))).astype(np.uint32)
+        a_col = np.concatenate(([2, 0, 2], j + 1)).astype(np.uint32)
+        a_val = np.zeros((n + 1, 4), dtype=np.uint64)
+        a_val[:, 0] = 1
+        a_val[1, 0] = 5
+        b_col = np.concatenate(([0, 2], j)).astype(np.uint32)
+        # C: row 0 = {c_0}, row j = {c_j} (j < n-1), row n-1 = {pub}
+        c_col = np.concatenate(([2], 2 + np.arange(1, n - 1, dtype=np.uint32), [1])).astype(np.uint32)
+        ones = np.zeros((n, 4), dtype=np.uint64)
+        ones[:, 0] = 1
+        self.csr = [(a_rowptr, a_col, a_val), (rowptr1, b_col, ones), (rowptr1.copy(), c_col, ones.copy())]
+        c0 = limbs_to_ints(rand_limbs(1, seed))[0] % R
+        cs = [c0, (c0 + 5) * c0 % R]
+        for k in range(1, n - 1):
+            cs.append(cs[k] * cs[k - 1] % R)
+        self.witness = [1, cs[n - 1]] + cs[:n - 1]
+        self.public_signals = [cs[n - 1]]
+
     def dense(self):
         """The same R1CS as dense n x m matrices (small n only): the reference's a, b, c."""
         out = []
@@ -164,20 +194,23 @@ class CircuitQAP:
     """What a real trusted setup of SyntheticCircuit(n) starts from, shared by CircuitGroth16 and CircuitPinocchio: the R1CS
     resident on the device, the satisfying witness (limbs in ``w``), Z = prod_{i=1..n}(x - i) (groth16.go:122-132,
     snark.go:210-221), and the QAP evaluated at the toxic T for every signal — at_s / bt_s / ct_s = Eval(alphas[i], T) etc.
-    through the sparse A^T l(T) of b200_qap_eval_at, and zt = Z(T) — as Python ints.  Any n >= 2."""
+    through the sparse A^T l(T) of b200_qap_eval_at, and zt = Z(T) — as Python ints.  Any n >= 2.  ``short_z``: the
+    m = n + 1 variant of SyntheticCircuit, whose Z = prod_{i=1..n-1}(x - i) has length m - 1 = n."""
 
-    def __init__(self, n, t):
+    def __init__(self, n, t, short_z=False):
         from .r1csqap import SparseR1CS
         assert n >= 2
-        self.n, self.m, self.npublic = n, n + 2, 1
+        self.circuit = SyntheticCircuit(n, short_z=short_z)
+        self.n, self.m, self.npublic = n, self.circuit.m, 1
+        self.short_z = short_z
         self.logn = n.bit_length() - 1 if n & (n - 1) == 0 else None
-        self.circuit = SyntheticCircuit(n)
         self.r1cs = SparseR1CS(n, self.m, self.circuit.csr)
-        at_l, bt_l, ct_l, self.zt = self.r1cs.EvalAt(t)
+        at_l, bt_l, ct_l, self.zt = self.r1cs.EvalAt(t)                      # zt = Z(T), Z of m - 2 roots
         self.at_s, self.bt_s, self.ct_s = limbs_to_ints(at_l), limbs_to_ints(bt_l), limbs_to_ints(ct_l)
         self.w = ints_to_limbs(self.circuit.witness)
-        self.z = np.zeros((n + 1, 4), dtype=np.uint64)
-        check(lib().b200_zero_poly(n, ptr(self.z)))
+        nz = self.m - 2
+        self.z = np.zeros((nz + 1, 4), dtype=np.uint64)
+        check(lib().b200_zero_poly(nz, ptr(self.z)))
 
     def px_of(self, w_limbs):
         """px = A(x) B(x) - C(x) of a witness of this R1CS (r1csqap.go:191-210), from the sparse front end (b200_qap_px)."""
@@ -195,13 +228,14 @@ class CircuitGroth16(CircuitQAP, SyntheticGroth16):
     k*G with a known k (k = Eval(alphas[i], tau) etc., see CircuitQAP), so
     the known-discrete-log parity check of SyntheticGroth16 keeps working AND the proof verifies under the real Vk.
     px comes from the sparse QAP front end (b200_qap_px); the expected proof is computed in the exponent from the QAP
-    identity  h(tau) Z(tau) = A(tau) B(tau) - C(tau)  — independently of the GPU's px and h.  Sized by 2^logn or by n."""
+    identity  h(tau) Z(tau) = A(tau) B(tau) - C(tau)  — independently of the GPU's px and h.  Sized by 2^logn or by n;
+    ``short_z``: the m = n + 1 circuit (len(Z) = n)."""
 
-    def __init__(self, logn=None, mint=True, n=None):
+    def __init__(self, logn=None, mint=True, n=None, short_z=False):
         tox = [x % R for x in limbs_to_ints(rand_limbs(5, SEED_TOXIC))]
         self.toxic = dict(zip(("T", "Kalpha", "Kbeta", "Kgamma", "Kdelta"), tox))
         t, ka, kb, kg, kd = tox
-        super().__init__(_size(logn, n), t)
+        super().__init__(_size(logn, n), t, short_z)
         m = self.m
         self.n_ptd = m - 1
         at, bt, ct, zt = self.at_s, self.bt_s, self.ct_s, self.zt
@@ -308,11 +342,12 @@ class CircuitPinocchio(CircuitQAP):
     """A REAL Pinocchio instance at benchmark sizes (any n >= 2): SyntheticCircuit's R1CS and witness, and the key and Vk
     that snark.GenerateTrustedSetup (snark.go:98-251) yields for seeded toxic values.  Every point is k*G with k from
     pinocchio_key_dlogs, minted on the GPU; the expected proof comes from pinocchio_proof_dlogs.  Key arrays are Jacobian
-    limbs in ``pk`` (A, Ap, B (G2), Bp, C, Cp, Kp, G1T), the Vk is a snark.VerifyProof dict of points in ``vk``."""
+    limbs in ``pk`` (A, Ap, B (G2), Bp, C, Cp, Kp, G1T), the Vk is a snark.VerifyProof dict of points in ``vk``.
+    ``short_z``: the m = n + 1 circuit (len(Z) = len(G1T) = n)."""
 
-    def __init__(self, n, mint=True):
+    def __init__(self, n, mint=True, short_z=False):
         self.toxic = pinocchio_toxic()
-        super().__init__(n, self.toxic["T"])
+        super().__init__(n, self.toxic["T"], short_z)
         self.k = pinocchio_key_dlogs(self.at_s, self.bt_s, self.ct_s, self.zt, self.toxic, self.npublic)
         if mint:
             self.mint()
@@ -333,7 +368,7 @@ class CircuitPinocchio(CircuitQAP):
         h = _lib._h(0)
         check(lib().b200_pinocchio_pk_load_shard(
             ptr(p["A"]), ptr(p["Ap"]), ptr(p["B"]), ptr(p["Bp"]), ptr(p["C"]), ptr(p["Cp"]), ptr(p["Kp"]), self.m,
-            ptr(p["G1T"]), p["G1T"].shape[0], ptr(self.z), self.n + 1, self.npublic, window_bits, rank, world, h))
+            ptr(p["G1T"]), p["G1T"].shape[0], ptr(self.z), self.z.shape[0], self.npublic, window_bits, rank, world, h))
         return h.value
 
     def expected_dlogs(self, witness=None):

@@ -381,8 +381,9 @@ int b200_pinocchio_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs);
 /* groth16.GenerateProofs fed from the witness: px is computed on the device from the resident R1CS (b200_qap_px) and
  * never leaves HBM; otherwise identical to b200_groth16_prove (groth16/groth16.go:225-278 after the caller's
- * CombinePolynomials step, cli/main.go:339-349).  When len(Z) = n + 1 the quotient h = DivisorPolynomial(px, Z) is
- * computed without forming px (C w is not needed: deg cx < deg Z); like the reference, it drops the remainder, so a
+ * CombinePolynomials step, cli/main.go:339-349).  When len(Z) = n + 1 or len(Z) = n (n >= 2: m = n + 2 or n + 1 signals)
+ * the quotient h = DivisorPolynomial(px, Z) is computed without forming px or C w (for len(Z) = n, h = (x - n) q + kappa
+ * with one dot product of the witness against a per-R1CS vector); like the reference, it drops the remainder, so a
  * witness that does not satisfy the R1CS gets the same proof as from b200_groth16_prove with its px (which does not
  * verify).  nw must equal the key's m and the R1CS's m.  Like b200_groth16_prove
  * it runs on the key's prove context (B200_CFG_PK_CONTEXT) and waits with the library mutex released, so two host
@@ -414,11 +415,13 @@ int b200_groth16_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const void
  *   - One batched sort serves the A, B1 and B2 MSMs of all k proofs (scalar vectors w_p ++ [1, r_p, s_p]); C||PTD has
  *     its own.  Each set runs one batched bucket phase (b200_msm_device_batch), the blinding products take one warp per
  *     proof and one kernel combines the k proofs.
- *   - len(Z) = n + 1, n >= 2 (the h-direct shape): the k quotients come from one batched front end (witness load, one
- *     sparse product of A and B over all k witnesses, Newton coefficients, shift products, interpolation), so a batch
- *     issues the launches of a batch of one, plus the documented extras of b200_msm_device_batch (one more launch when
+ *   - len(Z) = n + 1 or n, n >= 2 (the shapes whose proofs can verify: m = n + 2 or n + 1): the k quotients come from
+ *     one batched front end (witness load, one sparse product of A and B over all k witnesses, Newton coefficients,
+ *     shift products, interpolation; for len(Z) = n one more launch, the k dot products), so a batch issues the
+ *     launches of a batch of one, plus the documented extras of b200_msm_device_batch (one more launch when
  *     k*G*2^(c-1) bucket counters of a set exceed 64 Ki, one or two per further 65535 tail rows).  Any other len(Z)
- *     takes px and the division like the single entry, once per witness: correct, but not batched.
+ *     (m > n + 2, or n = 1) takes px and the division like the single entry, once per witness: correct, but not
+ *     batched.
  *   - Runs on the key's prove context; calls on keys of one context must be ordered.  Batches on keys of contexts 0 and
  *     1 may be in flight together, also on one R1CS handle.  Waits with the library mutex released.
  *   - Scratch: about k times one proof's sort, bucket and front-end scratch.  The key's (counted by
@@ -496,8 +499,8 @@ int b200_pinocchio_prove_device(b200_pk_t pk, const void* d_w, size_t nw, const 
                                 void* stream);
 /* snark.GenerateProofs fed from the witness: the quotient is computed on the device from the resident R1CS and never
  * leaves HBM; otherwise identical to b200_pinocchio_prove with px = CombinePolynomials(w, R1CSToQAP(a, b, c)).  When
- * len(Z) = n + 1 and n >= 2 the quotient h = DivisorPolynomial(px, Z) is computed without forming px (C w is not needed);
- * any other len(Z) takes px (b200_qap_px) and the key's division.  Like the reference it drops the remainder, so a witness
+ * len(Z) = n + 1 or n and n >= 2 the quotient h = DivisorPolynomial(px, Z) is computed without forming px or C w; any
+ * other len(Z) takes px (b200_qap_px) and the key's division.  Like the reference it drops the remainder, so a witness
  * that does not satisfy the R1CS gets the proof b200_pinocchio_prove gives for that witness and its px (which does not
  * verify).  The front end runs on the stream the G1T MSM runs on, beside the seven witness MSMs.  nw must equal the key's
  * m and the R1CS's m.  Unlike b200_pinocchio_prove it waits with the library mutex released, so two host threads proving
@@ -526,9 +529,10 @@ int b200_pinocchio_prove_witness_device(b200_pk_t pk, b200_r1cs_t r1cs, const vo
  *   - Three batched sorts, eight batched bucket phases (b200_msm_device_batch), whatever k.  The scalar vectors of the
  *     seven witness MSMs are the witnesses where they lie: one sort of w_p (stride nw) serves B, Bp, C, Cp, Kp, one of
  *     w_p[NPublic+1..) serves A, Ap, one of the k quotient vectors serves G1T; one kernel writes the k proofs.
- *   - len(Z) = n + 1, n >= 2 (the h-direct shape): the k quotients come from one batched front end, so a batch issues the
- *     launches of a batch of one, plus the documented extras of b200_msm_device_batch.  Any other len(Z) takes px and the
- *     division like the single entry, once per witness: correct, but not batched.
+ *   - len(Z) = n + 1 or n, n >= 2 (m = n + 2 or n + 1): the k quotients come from one batched front end (for len(Z) = n
+ *     one more launch, the k dot products), so a batch issues the launches of a batch of one, plus the documented extras
+ *     of b200_msm_device_batch.  Any other len(Z) takes px and the division like the single entry, once per witness:
+ *     correct, but not batched.
  *   - Waits with the library mutex released; batches on keys of contexts 0 and 1 may be in flight together, also on one
  *     R1CS handle.
  *   - Scratch: about k times one proof's sort, bucket and front-end scratch.  The key's (counted by b200_pk_device_bytes:
