@@ -188,6 +188,18 @@ def build_host_short_z(force=False):
     return target
 
 
+def build_host_setup_key(force=False):
+    """g++ build of the setup into a resident key (the generator table, minting into a base set's row 0, the window rows
+    from it, and the per-rank set plans) over csrc/host_stub (CPU test vehicle, tests/test_host_setup_key.py)."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    target = os.path.join(LIBDIR, "libb200_host_setup_key.so")
+    if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):
+        return target
+    _run(["g++", "-O2", "-std=c++17", "-x", "c++", "-shared", "-fPIC", "-Wno-psabi", "-I", os.path.join(HOSTTEST, "host_stub"),
+          "-I", HOSTTEST, "-I", CSRC, "-o", target, os.path.join(HOSTTEST, "setup_key_test.cpp")])
+    return target
+
+
 def build_shard_partition(force=False):
     """g++ build of csrc/shard_partition.h behind a C entry point (CPU test vehicle, tests/test_shard_partition.py)."""
     os.makedirs(LIBDIR, exist_ok=True)

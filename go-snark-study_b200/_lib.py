@@ -97,6 +97,8 @@ _SIGNATURES = {
     "b200_interpolate": [_vp, _sz, _vp],
     "b200_groth16_setup": [_h, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "b200_pinocchio_setup": [_h, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "b200_groth16_setup_pk": [_h, _sz, _vp, _int, _int, _int, ctypes.POINTER(_h), _vp, _vp, _vp, _vp, _vp],
+    "b200_pinocchio_setup_pk": [_h, _sz, _vp, _int, _int, _int, ctypes.POINTER(_h), _vp, _vp, _vp],
     "b200_groth16_prove_witness": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp, _vp],
     "b200_groth16_prove_witness_device": [_h, _h, _vp, _sz, _vp, _vp, _vp, _vp],
     "b200_groth16_prove_witness_batch": [_h, _h, _vp, _sz, _sz, _vp, _vp, _vp, _vp, _vp],

@@ -335,9 +335,12 @@ MsmShape msm_shape(size_t n, int c, int t) {
 // populated enough to amortise its per-round launches; since the per-round inversion became a binary-Euclid warp
 // it also wins for a stand-alone MSM.  A proving-key
 // shard that leaves a rank only a small MSM passes false (prove_host.cuh); B200_ACC_MODE=xyzz|affine forces either.
+// The points: n standard-form Jacobian points `pts` on the host, or, with `gen`, d_scalars[i] * G minted on the device
+// straight into the table's row 0 (n standard-form scalars < r, device memory): the same table words either way.
 template <class F>
-int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_ptr<Bases>& out_b, bool prefer_affine = true) {
-  if (!pts || n == 0 || n > (1u << 26)) return fail(B200_EINVAL, "bases_load: bad arguments");
+int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_ptr<Bases>& out_b, bool prefer_affine = true,
+                 const FixedBaseTable<F>* gen = nullptr, const Fr* d_scalars = nullptr) {
+  if ((!pts && !gen) || n == 0 || n > (1u << 26)) return fail(B200_EINVAL, "bases_load: bad arguments");
   if (c == 0) c = pick_window_bits(n);
   if (c < 2 || c > 24) return fail(B200_EINVAL, "window_bits must be in [2,24]");
   auto b = std::make_unique<Bases>();
@@ -376,11 +379,15 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   CU(b->d_err.alloc(sizeof(int)));
   CU(cudaMemset(b->d_err.p, 0, sizeof(int)));
 
-  // upload + normalise + window precompute
+  // upload + normalise (or mint row 0) + window precompute
   DevBuf staging, state;
-  CU(staging.alloc(n * 3 * sizeof(F)));
   CU(state.alloc(n * sizeof(XYZZ<F>)));
-  CU(cudaMemcpyAsync(staging.p, pts, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
+  if (gen) {
+    fixed_base_row_enqueue<F>(*gen, d_scalars, n, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_ctx[0].main);
+  } else {
+    CU(staging.alloc(n * 3 * sizeof(F)));
+    CU(cudaMemcpyAsync(staging.p, pts, n * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
+  }
   window_table_enqueue<F>(staging.as<F>(), n, sh.rows, c, b->table.as<Affine<F>>(), state.as<XYZZ<F>>(), g_d_err, g_ctx[0].main);
   CU(cudaGetLastError());
   int rc = check_err_flag("bases_load", g_d_err);
@@ -781,12 +788,16 @@ int poly_mul_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, ui
   return check_err_flag("poly_mul", g_d_err);
 }
 
-int divisor_init(Divisor& dv, const uint64_t* b, size_t nb) {
+// The divisor b (nb standard-form coefficients) from device memory (d_b) or, with d_b null, from the host (b).
+int divisor_init(Divisor& dv, const uint64_t* b, size_t nb, const Fr* d_b = nullptr) {
   DevBuf tmp;
-  CU(tmp.alloc(nb * sizeof(Fr)));
+  if (!d_b) {
+    CU(tmp.alloc(nb * sizeof(Fr)));
+    CU(cudaMemcpyAsync(tmp.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+    d_b = tmp.as<Fr>();
+  }
   CU(dv.b_mont.alloc(nb * sizeof(Fr)));
-  CU(cudaMemcpyAsync(tmp.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
-  k_poly_load<<<nblk(nb, 256), 256, 0, g_ctx[0].main>>>(tmp.as<Fr>(), (uint32_t)nb, (uint32_t)nb, 0, 0, dv.b_mont.as<Fr>(),
+  k_poly_load<<<nblk(nb, 256), 256, 0, g_ctx[0].main>>>(d_b, (uint32_t)nb, (uint32_t)nb, 0, 0, dv.b_mont.as<Fr>(),
                                                     (uint32_t)nb, g_d_err);
   CU(cudaStreamSynchronize(g_ctx[0].main));
   dv.nb = nb;
@@ -1570,9 +1581,10 @@ int poly_eval_batch_host(const uint64_t* polys, size_t m, size_t n, const uint64
   return check_err_flag("poly_eval_batch", g_d_err);
 }
 
-int zero_poly_host(size_t n, uint64_t* out) {   // coefficients of prod_{i=1..n} (x - i), n + 1 of them
-  if (!out || n > ((size_t)1 << 26)) return fail(B200_EINVAL, "zero_poly: bad arguments (n <= 2^26)");
-  DevBuf zn, zz;
+// zz = the n + 1 standard-form coefficients of prod_{i=1..n} (x - i), on the device, enqueued on context 0's main stream
+int zero_poly_enqueue(size_t n, DevBuf& zz) {
+  if (n > ((size_t)1 << 26)) return fail(B200_EINVAL, "zero_poly: bad arguments (n <= 2^26)");
+  DevBuf zn;
   CU(zz.alloc((n + 1) * sizeof(Fr)));
   if (n <= 2048) {   // one-block schoolbook; above: Newton basis element n through the subproduct tree (qap_sparse.cuh)
     CU(zn.alloc((n + 1) * sizeof(Fr)));
@@ -1583,6 +1595,14 @@ int zero_poly_host(size_t n, uint64_t* out) {   // coefficients of prod_{i=1..n}
   }
   k_poly_store<<<nblk(n + 1, 256), 256, 0, g_ctx[0].main>>>(zn.as<Fr>(), (uint32_t)(n + 1), 0, 1, zz.as<Fr>());
   CU(cudaGetLastError());
+  return B200_OK;
+}
+
+int zero_poly_host(size_t n, uint64_t* out) {   // coefficients of prod_{i=1..n} (x - i), n + 1 of them
+  if (!out) return fail(B200_EINVAL, "zero_poly: bad arguments (n <= 2^26)");
+  DevBuf zz;
+  int rc = zero_poly_enqueue(n, zz);
+  if (rc) return rc;
   CU(cudaMemcpyAsync(out, zz.p, (n + 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
   return check_err_flag("zero_poly", g_d_err);
 }
@@ -2077,6 +2097,15 @@ int b200_pinocchio_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[
                          uint64_t* bp, uint64_t* c, uint64_t* cp, uint64_t* kp, uint64_t* g1t, uint64_t* z, uint64_t vk_g1[24],
                          uint64_t vk_g2[120]) {
   B200_API_BODY(pinocchio_setup_host(r1cs, npublic, toxic, a, ap, b2, bp, c, cp, kp, g1t, z, vk_g1, vk_g2))
+}
+int b200_groth16_setup_pk(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[20], int window_bits, int rank, int world,
+                          b200_pk_t* out, uint64_t alpha1[12], uint64_t beta2[24], uint64_t gamma2[24], uint64_t delta2[24],
+                          uint64_t* ic) {
+  B200_API_BODY(groth16_setup_pk(r1cs, npublic, toxic, window_bits, rank, world, out, alpha1, beta2, gamma2, delta2, ic))
+}
+int b200_pinocchio_setup_pk(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[32], int window_bits, int rank, int world,
+                            b200_pk_t* out, uint64_t vk_g1[24], uint64_t vk_g2[120], uint64_t* ic) {
+  B200_API_BODY(pinocchio_setup_pk(r1cs, npublic, toxic, window_bits, rank, world, out, vk_g1, vk_g2, ic))
 }
 int b200_groth16_prove_witness(b200_pk_t pk, b200_r1cs_t r1cs, const uint64_t* w, size_t nw, const uint64_t r[4],
                                const uint64_t s[4], uint64_t pi_a[12], uint64_t pi_b[24], uint64_t pi_c[12]) {

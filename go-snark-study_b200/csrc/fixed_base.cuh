@@ -36,13 +36,14 @@ inline const uint64_t kG2GenJacStd[24] = {
     0x55acdadcd122975bull, 0xbc4b313370b38ef3ull, 0xec9e99ad690c3395ull, 0x090689d0585ff075ull,
     1, 0, 0, 0, 0, 0, 0, 0};
 
-// table[w][i] = 2^(c*w) * P_i (Montgomery affine) for w < nwin, from n standard-form Jacobian points on the device.
-// state: n XYZZ records of scratch.  err |= 1 when a coordinate is >= q.  (The window precompute of an MSM base set.)
+// table[w][i] = 2^(c*w) * P_i (Montgomery affine) for w < nwin, from n standard-form Jacobian points on the device, or,
+// with jac_std null, from the points already in row 0 (minted there by fixed_base_row_enqueue).  state: n XYZZ records of
+// scratch.  err |= 1 when a coordinate is >= q.  (The window precompute of an MSM base set.)
 template <class F>
 void window_table_enqueue(const F* jac_std, size_t n, uint32_t nwin, int c, Affine<F>* table, XYZZ<F>* state, int* err,
                           cudaStream_t st) {
   auto* to_affine = &k_batch_to_affine<F, 8>;
-  B200_LAUNCH(k_load_bases<F>, nblk(n, 128), 128, st, jac_std, n, table, err);
+  if (jac_std) B200_LAUNCH(k_load_bases<F>, nblk(n, 128), 128, st, jac_std, n, table, err);
   B200_LAUNCH(k_affine_to_xyzz<F>, nblk(n, 128), 128, st, table, state, n);
   for (uint32_t w = 1; w < nwin; w++) {
     B200_LAUNCH(k_window_step<F>, nblk(n, 128), 128, st, state, n, c);
@@ -88,37 +89,70 @@ __global__ void k_affine_store_std(const Affine<F>* __restrict__ in, size_t n, F
   o[2] = one;
 }
 
-// out_jac_std[i] = scalars[i] * G (G the generator of F's group) for n standard-form scalars < r on the device; affine
-// (x, y, 1) in standard form, infinity all zero.  Builds the generator table, runs the kernel and normalises; returns
-// after synchronising `st`.  err |= 1 if a table coordinate were >= q (never, for the generators).
+// The generator table of k_fixed_base for F's group: kFixedBaseWin x kFixedBaseRow affine points (2.75 MiB in G1,
+// 5.5 MiB in G2), built once per call and shared by every set that call mints.
 template <class F>
-cudaError_t fixed_base_mul(const Fr* d_scalars_std, size_t n, F* d_out_jac_std, int* err, cudaStream_t st) {
-  if (n == 0) return cudaSuccess;
-  constexpr size_t H = kFixedBaseRow;
-  const uint64_t* gen = sizeof(F) == sizeof(Fq) ? kG1GenJacStd : kG2GenJacStd;
-  std::vector<Fr> ks(H);
-  for (size_t d = 0; d < H; d++) {
-    ks[d] = Fr::zero();
-    ks[d].l[0] = (uint32_t)(d + 1);
+struct FixedBaseTable {
+  DevBuf table;
+  // the base set {1*G, .., 2^(c-1)*G}, then its window table.  err |= 1 if a coordinate were >= q (never, for the generators)
+  cudaError_t build(int* err, cudaStream_t st) {
+    constexpr size_t H = kFixedBaseRow;
+    const uint64_t* gen = sizeof(F) == sizeof(Fq) ? kG1GenJacStd : kG2GenJacStd;
+    std::vector<Fr> ks(H);
+    for (size_t d = 0; d < H; d++) {
+      ks[d] = Fr::zero();
+      ks[d].l[0] = (uint32_t)(d + 1);
+    }
+    DevBuf dgen, dks, base, state;
+    PCU(dgen.alloc(3 * sizeof(F)));
+    PCU(dks.alloc(H * sizeof(Fr)));
+    PCU(base.alloc(3 * H * sizeof(F)));
+    PCU(state.alloc(H * sizeof(XYZZ<F>)));
+    PCU(table.alloc((size_t)kFixedBaseWin * H * sizeof(Affine<F>)));
+    PCU(cudaMemcpyAsync(dgen.p, gen, 3 * sizeof(F), cudaMemcpyHostToDevice, st));
+    PCU(cudaMemcpyAsync(dks.p, ks.data(), H * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    B200_LAUNCH(k_mul_batch_ref<F>, nblk(H, 128), 128, st, dgen.as<F>(), 1, dks.as<Fr>(), H, base.as<F>(), err);
+    window_table_enqueue<F>(base.as<F>(), H, kFixedBaseWin, kFixedBaseC, table.as<Affine<F>>(), state.as<XYZZ<F>>(), err, st);
+    PCU(cudaGetLastError());
+    return cudaStreamSynchronize(st);   // the temporaries above are freed on return
   }
-  DevBuf dgen, dks, base, table, state, aff;
-  PCU(dgen.alloc(3 * sizeof(F)));
-  PCU(dks.alloc(H * sizeof(Fr)));
-  PCU(base.alloc(3 * H * sizeof(F)));
-  PCU(table.alloc((size_t)kFixedBaseWin * H * sizeof(Affine<F>)));
-  PCU(state.alloc((n > H ? n : H) * sizeof(XYZZ<F>)));
-  PCU(aff.alloc(n * sizeof(Affine<F>)));
-  PCU(cudaMemcpyAsync(dgen.p, gen, 3 * sizeof(F), cudaMemcpyHostToDevice, st));
-  PCU(cudaMemcpyAsync(dks.p, ks.data(), H * sizeof(Fr), cudaMemcpyHostToDevice, st));
-  // the base set {1*G, .., 2^(c-1)*G}, then its window table
-  B200_LAUNCH(k_mul_batch_ref<F>, nblk(H, 128), 128, st, dgen.as<F>(), 1, dks.as<Fr>(), H, base.as<F>(), err);
-  window_table_enqueue<F>(base.as<F>(), H, kFixedBaseWin, kFixedBaseC, table.as<Affine<F>>(), state.as<XYZZ<F>>(), err, st);
+};
+
+// row0[i] = scalars[i] * G as Montgomery affine points, infinity as Affine::inf() (the words k_load_bases writes for the
+// same points), for n standard-form scalars < r on the device.  state: n XYZZ records of scratch.  row0 is row 0 of a
+// base set's table (setup into a resident key) or a plain buffer (fixed_base_mul).
+template <class F>
+void fixed_base_row_enqueue(const FixedBaseTable<F>& gen, const Fr* d_scalars_std, size_t n, Affine<F>* row0,
+                            XYZZ<F>* state, cudaStream_t st) {
+  if (n == 0) return;
   auto* to_affine = &k_batch_to_affine<F, 8>;
-  B200_LAUNCH(k_fixed_base<F>, nblk(n, 128), 128, st, table.as<Affine<F>>(), d_scalars_std, n, state.as<XYZZ<F>>());
-  B200_LAUNCH(to_affine, nblk((n + 7) / 8, 128), 128, st, state.as<XYZZ<F>>(), aff.as<Affine<F>>(), n);
+  B200_LAUNCH(k_fixed_base<F>, nblk(n, 128), 128, st, gen.table.template as<Affine<F>>(), d_scalars_std, n, state);
+  B200_LAUNCH(to_affine, nblk((n + 7) / 8, 128), 128, st, state, row0, n);
+}
+
+// out_jac_std[i] = scalars[i] * G under a built generator table: affine (x, y, 1) in standard form, infinity all zero,
+// stored from the minted row.  Returns after synchronising `st`.
+template <class F>
+cudaError_t fixed_base_std(const FixedBaseTable<F>& gen, const Fr* d_scalars_std, size_t n, F* d_out_jac_std, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  DevBuf state, aff;
+  PCU(state.alloc(n * sizeof(XYZZ<F>)));
+  PCU(aff.alloc(n * sizeof(Affine<F>)));
+  fixed_base_row_enqueue<F>(gen, d_scalars_std, n, aff.as<Affine<F>>(), state.as<XYZZ<F>>(), st);
   B200_LAUNCH(k_affine_store_std<F>, nblk(n, 128), 128, st, aff.as<Affine<F>>(), n, d_out_jac_std);
   PCU(cudaGetLastError());
   return cudaStreamSynchronize(st);
+}
+
+// out_jac_std[i] = scalars[i] * G (G the generator of F's group) for n standard-form scalars < r on the device; affine
+// (x, y, 1) in standard form, infinity all zero.  Builds the generator table, mints and stores; returns after
+// synchronising `st`.  err |= 1 if a table coordinate were >= q (never, for the generators).
+template <class F>
+cudaError_t fixed_base_mul(const Fr* d_scalars_std, size_t n, F* d_out_jac_std, int* err, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  FixedBaseTable<F> gen;
+  PCU(gen.build(err, st));
+  return fixed_base_std<F>(gen, d_scalars_std, n, d_out_jac_std, st);
 }
 
 }  // namespace b200

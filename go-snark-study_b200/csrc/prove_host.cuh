@@ -164,10 +164,37 @@ struct PointCat {
   size_t count() const { return v.size() / words; }
 };
 
-int pk_common_init(ProvingKey& pk, const uint64_t* z, size_t nz, size_t m) {
-  if (!z || nz == 0) return fail(B200_EINVAL, "pk_load: missing Z");
+// Where the points of a key's base sets come from when they are minted on the device (setup into a resident key) instead
+// of read from the host arrays of b200_*_pk_load: the standard-form scalars of k_groth16_setup_scalars /
+// k_pinocchio_setup_scalars in their layouts (setup_host.cuh), each set's slice being a contiguous range there, the
+// generator tables (built once per call), the Groth16 tail scalars Kalpha, Kbeta, Kdelta (standard form), and Z.
+struct MintSource {
+  const Fr* g1 = nullptr;
+  const Fr* g2 = nullptr;
+  const FixedBaseTable<Fq>* gen1 = nullptr;
+  const FixedBaseTable<Fq2>* gen2 = nullptr;
+  Fr alpha{}, beta{}, delta{};
+  const Fr* d_z = nullptr;   // standard-form coefficients on the device
+};
+
+// A base set of cnt scalars src[0..cnt) (device) ++ `tail` (host; only when with_tail) minted into its table's row 0.
+// Transient device memory: the n scalars here and bases_create's XYZZ state, freed before the next set.
+template <class F>
+int mint_set(const FixedBaseTable<F>& gen, const Fr* src, size_t cnt, bool with_tail, std::initializer_list<Fr> tail, int c,
+             int group, std::unique_ptr<Bases>& out, bool prefer_affine) {
+  const size_t nt = with_tail ? tail.size() : 0, n = cnt + nt;
+  if (n == 0) return fail(B200_EINVAL, "bases_load: bad arguments");
+  DevBuf sc;
+  CU(sc.alloc(n * sizeof(Fr)));
+  if (cnt) CU(cudaMemcpyAsync(sc.p, src, cnt * sizeof(Fr), cudaMemcpyDeviceToDevice, g_ctx[0].main));
+  if (nt) CU(cudaMemcpyAsync(sc.as<Fr>() + cnt, tail.begin(), nt * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  return bases_create<F>(nullptr, n, c, group, out, prefer_affine, &gen, sc.as<Fr>());
+}
+
+int pk_common_init(ProvingKey& pk, const uint64_t* z, size_t nz, size_t m, const Fr* d_z = nullptr) {
+  if ((!z && !d_z) || nz == 0) return fail(B200_EINVAL, "pk_load: missing Z");
   pk.ctx = g_pk_ctx;
-  int rc = divisor_init(pk.Z, z, nz);
+  int rc = divisor_init(pk.Z, z, nz, d_z);
   if (rc) return rc;
   CU(pk.s1.alloc((m + 4) * sizeof(Fr)));
   CU(pk.s2.alloc((m + 4) * sizeof(Fr)));
@@ -186,8 +213,8 @@ int pk_common_init(ProvingKey& pk, const uint64_t* z, size_t nz, size_t m) {
 int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, const uint64_t* bacdelta, size_t m,
                     const uint64_t* ptd, size_t n_ptd, const uint64_t* z, size_t nz, const uint64_t* alpha1,
                     const uint64_t* beta1, const uint64_t* delta1, const uint64_t* beta2, const uint64_t* delta2,
-                    size_t npublic, int c, int rank, int world, b200_pk_t* out) {
-  if (!at || !b1 || !b2 || !bacdelta || !ptd || !alpha1 || !beta1 || !delta1 || !beta2 || !delta2 || !out)
+                    size_t npublic, int c, int rank, int world, b200_pk_t* out, const MintSource* mint = nullptr) {
+  if ((!mint && (!at || !b1 || !b2 || !bacdelta || !ptd || !alpha1 || !beta1 || !delta1 || !beta2 || !delta2)) || !out)
     return fail(B200_EINVAL, "groth16_pk_load: null pointer");
   if (m == 0 || npublic + 1 > m || n_ptd == 0) return fail(B200_EINVAL, "groth16_pk_load: bad sizes");
   if (world < 1 || rank < 0 || rank >= world) return fail(B200_EINVAL, "groth16_pk_load: bad shard %d/%d", rank, world);
@@ -196,28 +223,26 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   pk->m = m;
   pk->npublic = npublic;
   pk->n_h_bases = n_ptd;
-  int rc = pk_common_init(*pk, z, nz, m);
+  int rc = pk_common_init(*pk, z, nz, m, mint ? mint->d_z : nullptr);
   if (rc) return rc;
   pk->rank = rank;
   pk->world = world;
   const size_t l1 = npublic + 1;
   const size_t n_c_full = pk->n_c_full = m - l1;
-  const size_t len[4] = {m, m, m, n_c_full + n_ptd};
   // Cost weights of the line partition, in G1 terms of the C||PTD set: a G2 term (B2), and a term of A / B1 — whose ranks
   // also pay the two GLV products s*A_part + r*B1_part (single-warp latency) on their critical path when sharded.
   const double w_ab = world > 1 ? g_w_ab / 100.0 : 1.0;
   const double wgt[4] = {w_ab, w_ab, g_w_g2 / 100.0, 1.0};
-  std::vector<ShardCut> cuts((size_t)world);
-  shard_partition(len, wgt, world, cuts.data());   // equal pieces of the weighted line (shard_partition.h)
-  for (int k = 0; k < 4; k++) pk->len[k] = len[k];
+  G16Plan plan = groth16_set_plan(m, npublic, n_ptd, wgt, rank, world);   // equal pieces of the weighted line
   pk->window_bits = c;
   pk->table_windows = g_table_windows;
   for (int k = 0; k < 4; k++) {
-    pk->lo[k] = cuts[(size_t)rank].lo[k];
-    pk->hi[k] = cuts[(size_t)rank].hi[k];
-    pk->tail[k] = pk->hi[k] == len[k] && (pk->lo[k] < pk->hi[k] || (rank == world - 1 && len[k] == 0));
+    pk->len[k] = plan.len[k];
+    pk->lo[k] = plan.cuts[(size_t)rank].lo[k];
+    pk->hi[k] = plan.cuts[(size_t)rank].hi[k];
+    pk->tail[k] = plan.tail[k];
   }
-  // a set whose end falls exactly on a cut: the rank holding its last element owns the tail (checked above);
+  // a set whose end falls exactly on a cut: the rank holding its last element owns the tail (shard_holds_tail);
   // if no rank holds elements of it (len == 0) the last rank does.
   // Accumulation kernel per SET of this rank.  The batched-affine tree pays off once a set is large enough to amortise its
   // per-round launches (G2 sets earlier than G1 sets); below g_aff_min_g1 / g_aff_min_g2 terms a shard takes the XYZZ
@@ -225,35 +250,59 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   // MSMs cover each other's gaps.
   auto set_terms = [&](int k) { return (double)(pk->hi[k] - pk->lo[k]); };
   auto affine_for = [&](int k) { return world == 1 || set_terms(k) >= (double)(k == 2 ? g_aff_min_g2 : g_aff_min_g1); };
+  // Each set from the host arrays, or minted: its slice of the setup's scalars (C||PTD: BACDelta[l1..m) ++ PTD is one
+  // range there), then the scalars of its tail (0 for an infinity).
   static const uint64_t inf1[12] = {0}, inf2[24] = {0};
   auto has = [&](int k) { return pk->lo[k] < pk->hi[k] || pk->tail[k]; };
+  const Fr o = Fr::zero();
+  auto cnt = [&](int k) { return pk->hi[k] - pk->lo[k]; };
   if (has(0)) {
-    PointCat cat(12);
-    cat.add(at + 12 * pk->lo[0], pk->hi[0] - pk->lo[0]);
-    if (pk->tail[0]) { cat.add(alpha1, 1); cat.add(delta1, 1); cat.add(inf1, 1); }
-    if ((rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[0], affine_for(0)))) return rc;
+    if (mint) {
+      rc = mint_set<Fq>(*mint->gen1, mint->g1 + pk->lo[0], cnt(0), pk->tail[0], {mint->alpha, mint->delta, o}, c, 1, pk->g[0], affine_for(0));
+    } else {
+      PointCat cat(12);
+      cat.add(at + 12 * pk->lo[0], cnt(0));
+      if (pk->tail[0]) { cat.add(alpha1, 1); cat.add(delta1, 1); cat.add(inf1, 1); }
+      rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[0], affine_for(0));
+    }
+    if (rc) return rc;
   }
   if (has(1)) {
-    PointCat cat(12);
-    cat.add(b1 + 12 * pk->lo[1], pk->hi[1] - pk->lo[1]);
-    if (pk->tail[1]) { cat.add(beta1, 1); cat.add(inf1, 1); cat.add(delta1, 1); }
-    if ((rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[1], affine_for(1)))) return rc;
+    if (mint) {
+      rc = mint_set<Fq>(*mint->gen1, mint->g1 + m + pk->lo[1], cnt(1), pk->tail[1], {mint->beta, o, mint->delta}, c, 1, pk->g[1], affine_for(1));
+    } else {
+      PointCat cat(12);
+      cat.add(b1 + 12 * pk->lo[1], cnt(1));
+      if (pk->tail[1]) { cat.add(beta1, 1); cat.add(inf1, 1); cat.add(delta1, 1); }
+      rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[1], affine_for(1));
+    }
+    if (rc) return rc;
   }
   if (has(2)) {
-    PointCat cat(24);
-    cat.add(b2 + 24 * pk->lo[2], pk->hi[2] - pk->lo[2]);
-    if (pk->tail[2]) { cat.add(beta2, 1); cat.add(inf2, 1); cat.add(delta2, 1); }
-    if ((rc = bases_create<Fq2>(cat.v.data(), cat.count(), c, 2, pk->g[2], affine_for(2)))) return rc;
+    if (mint) {
+      rc = mint_set<Fq2>(*mint->gen2, mint->g2 + pk->lo[2], cnt(2), pk->tail[2], {mint->beta, o, mint->delta}, c, 2, pk->g[2], affine_for(2));
+    } else {
+      PointCat cat(24);
+      cat.add(b2 + 24 * pk->lo[2], cnt(2));
+      if (pk->tail[2]) { cat.add(beta2, 1); cat.add(inf2, 1); cat.add(delta2, 1); }
+      rc = bases_create<Fq2>(cat.v.data(), cat.count(), c, 2, pk->g[2], affine_for(2));
+    }
+    if (rc) return rc;
   }
   if (has(3)) {
-    PointCat cat(12);
-    size_t lo3 = pk->lo[3], hi3 = pk->hi[3];
-    size_t c_lo = lo3 < n_c_full ? lo3 : n_c_full, c_hi = hi3 < n_c_full ? hi3 : n_c_full;
-    size_t p_lo = lo3 > n_c_full ? lo3 - n_c_full : 0, p_hi = hi3 > n_c_full ? hi3 - n_c_full : 0;
-    cat.add(bacdelta + 12 * (l1 + c_lo), c_hi - c_lo);
-    cat.add(ptd + 12 * p_lo, p_hi - p_lo);
-    if (pk->tail[3]) cat.add(delta1, 1);
-    if ((rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[3], affine_for(3)))) return rc;
+    if (mint) {
+      rc = mint_set<Fq>(*mint->gen1, mint->g1 + 2 * m + l1 + pk->lo[3], cnt(3), pk->tail[3], {mint->delta}, c, 1, pk->g[3], affine_for(3));
+    } else {
+      PointCat cat(12);
+      size_t lo3 = pk->lo[3], hi3 = pk->hi[3];
+      size_t c_lo = lo3 < n_c_full ? lo3 : n_c_full, c_hi = hi3 < n_c_full ? hi3 : n_c_full;
+      size_t p_lo = lo3 > n_c_full ? lo3 - n_c_full : 0, p_hi = hi3 > n_c_full ? hi3 - n_c_full : 0;
+      cat.add(bacdelta + 12 * (l1 + c_lo), c_hi - c_lo);
+      cat.add(ptd + 12 * p_lo, p_hi - p_lo);
+      if (pk->tail[3]) cat.add(delta1, 1);
+      rc = bases_create<Fq>(cat.v.data(), cat.count(), c, 1, pk->g[3], affine_for(3));
+    }
+    if (rc) return rc;
   }
   // sets that consume identical scalar slices into the same table rows share one digit sort
   for (int k = 1; k < 3; k++)
@@ -264,7 +313,7 @@ int groth16_pk_load(const uint64_t* at, const uint64_t* b1, const uint64_t* b2, 
   CU(pk->s3.alloc((m + n_ptd + 4) * sizeof(Fr)));
   CU(pk->s4.alloc((m + 4) * sizeof(Fr)));
   if (world > 1) CU(pk->h_full.alloc((m + n_ptd + 4) * sizeof(Fr)));
-  pk->cuts = std::move(cuts);
+  pk->cuts = std::move(plan.cuts);
   uint64_t h = g_next_pk++;
   g_pks[h] = std::move(pk);
   *out = h;
@@ -292,7 +341,7 @@ G16Slices g16_slices(const ProvingKey* pk, int rank) {
   for (int j = 0; j < 4; j++) {
     sl.lo[j] = ct.lo[j];
     sl.hi[j] = ct.hi[j];
-    sl.tail[j] = sl.hi[j] == pk->len[j] && (sl.lo[j] < sl.hi[j] || (rank == pk->world - 1 && pk->len[j] == 0));
+    sl.tail[j] = shard_holds_tail(sl.lo[j], sl.hi[j], pk->len[j], rank, pk->world);
     sl.terms[j] = sl.hi[j] - sl.lo[j] + (sl.tail[j] ? (j < 3 ? 3 : 1) : 0);
   }
   const size_t ncf = pk->n_c_full;
@@ -659,30 +708,16 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
 // Base sets g[k]: 0 A, 1 Ap, 2 B (G2), 3 Bp, 4 C, 5 Cp, 6 Kp, 7 G1T.
 constexpr int kPinSlot[8] = {0, 1, 7, 2, 3, 4, 6, 5};
 
-// Sharded mode (world > 1): the eight MSMs are independent objects, so whole MSMs are dealt to the ranks — greedy
-// longest-first onto the least loaded rank by term count (a G2 term ~2.8 G1 terms) — and no MSM is split.  `owner[k]` is the
-// same on every rank.  (Eight objects: more than 8 ranks leave the rest idle.)
-void pinocchio_owners(size_t m, size_t l1, size_t n_g1t, int world, int owner[8]) {
-  double cost[8] = {(double)(m - l1), (double)(m - l1), 2.8 * (double)m, (double)m, (double)m, (double)m, (double)m, (double)n_g1t};
-  int order[8] = {0, 1, 2, 3, 4, 5, 6, 7};
-  std::stable_sort(order, order + 8, [&](int x, int y) { return cost[x] > cost[y]; });
-  std::vector<double> load((size_t)world, 0.0);
-  for (int q = 0; q < 8; q++) {
-    int k = order[q], best = 0;
-    for (int g = 1; g < world; g++)
-      if (load[g] < load[best]) best = g;
-    owner[k] = best;
-    load[best] += cost[k];
-  }
-}
+// Sharded mode (world > 1): whole MSMs are dealt to the ranks by pinocchio_owners (shard_partition.h).
 
 // The world records of one proof are summed slot by slot by k_pinocchio_gather_finalize_batch (pinocchio_batch.cuh) with
 // k = 1: every slot is non-infinity on exactly one rank.
 
 int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2, const uint64_t* bp,
                       const uint64_t* c, const uint64_t* cp, const uint64_t* kp, size_t m, const uint64_t* g1t,
-                      size_t n_g1t, const uint64_t* z, size_t nz, size_t npublic, int wb, int rank, int world, b200_pk_t* out) {
-  if (!a || !ap || !b2 || !bp || !c || !cp || !kp || !g1t || !out)
+                      size_t n_g1t, const uint64_t* z, size_t nz, size_t npublic, int wb, int rank, int world, b200_pk_t* out,
+                      const MintSource* mint = nullptr) {
+  if ((!mint && (!a || !ap || !b2 || !bp || !c || !cp || !kp || !g1t)) || !out)
     return fail(B200_EINVAL, "pinocchio_pk_load: null pointer");
   if (m == 0 || npublic + 1 > m || n_g1t == 0) return fail(B200_EINVAL, "pinocchio_pk_load: bad sizes");
   if (world < 1 || rank < 0 || rank >= world) return fail(B200_EINVAL, "pinocchio_pk_load: bad shard %d/%d", rank, world);
@@ -691,7 +726,7 @@ int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2,
   pk->m = m;
   pk->npublic = npublic;
   pk->n_h_bases = n_g1t;
-  int rc = pk_common_init(*pk, z, nz, m);
+  int rc = pk_common_init(*pk, z, nz, m, mint ? mint->d_z : nullptr);
   if (rc) return rc;
   size_t l1 = npublic + 1;
   pk->rank = rank;
@@ -701,17 +736,27 @@ int pinocchio_pk_load(const uint64_t* a, const uint64_t* ap, const uint64_t* b2,
   int owner[8];
   pinocchio_owners(m, l1, n_g1t, world, owner);
   auto mine = [&](int k) { return owner[k] == rank; };
+  // Set k: `cnt` points from index `first` of its host array, or minted from offset `off` of the setup's G1 / G2 scalars
+  // (layout of k_pinocchio_setup_scalars).
+  auto set = [&](int k, const uint64_t* pts, size_t first, size_t off, size_t cnt) {
+    if (!mine(k)) return (int)B200_OK;
+    if (k == 2)
+      return mint ? mint_set<Fq2>(*mint->gen2, mint->g2 + off, cnt, false, {}, wb, 2, pk->g[k], true)
+                  : bases_create<Fq2>(pts + 24 * first, cnt, wb, 2, pk->g[k], true);
+    return mint ? mint_set<Fq>(*mint->gen1, mint->g1 + off, cnt, false, {}, wb, 1, pk->g[k], true)
+                : bases_create<Fq>(pts + 12 * first, cnt, wb, 1, pk->g[k], true);
+  };
   // snark.go:265-268: PiA, PiAp run over i in [NPublic+1, NVars)
   if (m > l1) {
-    if (mine(0) && (rc = bases_create<Fq>(a + 12 * l1, m - l1, wb, 1, pk->g[0], true))) return rc;
-    if (mine(1) && (rc = bases_create<Fq>(ap + 12 * l1, m - l1, wb, 1, pk->g[1], true))) return rc;
+    if ((rc = set(0, a, l1, l1, m - l1))) return rc;
+    if ((rc = set(1, ap, l1, m + l1, m - l1))) return rc;
   }
-  if (mine(2) && (rc = bases_create<Fq2>(b2, m, wb, 2, pk->g[2], true))) return rc;
-  if (mine(3) && (rc = bases_create<Fq>(bp, m, wb, 1, pk->g[3], true))) return rc;
-  if (mine(4) && (rc = bases_create<Fq>(c, m, wb, 1, pk->g[4], true))) return rc;
-  if (mine(5) && (rc = bases_create<Fq>(cp, m, wb, 1, pk->g[5], true))) return rc;
-  if (mine(6) && (rc = bases_create<Fq>(kp, m, wb, 1, pk->g[6], true))) return rc;
-  if (mine(7) && (rc = bases_create<Fq>(g1t, n_g1t, wb, 1, pk->g[7], true))) return rc;
+  if ((rc = set(2, b2, 0, 0, m))) return rc;
+  if ((rc = set(3, bp, 0, 2 * m, m))) return rc;
+  if ((rc = set(4, c, 0, 3 * m, m))) return rc;
+  if ((rc = set(5, cp, 0, 4 * m, m))) return rc;
+  if ((rc = set(6, kp, 0, 5 * m, m))) return rc;
+  if ((rc = set(7, g1t, 0, 6 * m, n_g1t))) return rc;
   CU(pk->s3.alloc((n_g1t + 4) * sizeof(Fr)));
   uint64_t h = g_next_pk++;
   g_pks[h] = std::move(pk);

@@ -84,6 +84,41 @@ int copy_points(uint64_t* dst, const F* d_pts, size_t first, size_t count, cudaS
   return B200_OK;
 }
 
+// Steps 1-2 of the Groth16 setup on context 0's main stream: s1 / s2 = the standard-form scalars of every G1 / G2 point in
+// the layouts of k_groth16_setup_scalars, with Alpha, Beta, Delta (G1) and Beta, Gamma, Delta (G2) appended; n1 / n2
+// scalars.  tx: T, Kalpha, Kbeta, Kgamma, Kdelta (Montgomery).
+int groth16_scalars(R1cs* r, size_t npublic, const Fr* tx, DevBuf& s1, DevBuf& s2, size_t* n1, size_t* n2) {
+  const size_t m = r->m, l1 = npublic + 1;
+  cudaStream_t st = g_ctx[0].main;
+  *n1 = 4 * m - 1 + l1 + 3;
+  *n2 = m + 3;
+  DevBuf ev;
+  CU(ev.alloc(3 * m * sizeof(Fr)));
+  CU(s1.alloc(*n1 * sizeof(Fr)));
+  CU(s2.alloc(*n2 * sizeof(Fr)));
+  Fr zt;
+  int rc = qap_eval_at_enqueue(r, tx[0], m - 2, ev.as<Fr>(), &zt, st);
+  if (rc) return rc;
+  const Fr inv_d = tx[4].inverse(), inv_g = tx[3].inverse();
+  k_groth16_setup_scalars<<<nblk(m, 128), 128, 0, st>>>(ev.as<Fr>(), (uint32_t)m, (uint32_t)npublic, tx[1], tx[2], inv_d, inv_g,
+                                                         zt * inv_d, tx[0], s1.as<Fr>(), s2.as<Fr>());
+  const Fr v1[3] = {tx[1].from_mont(), tx[2].from_mont(), tx[4].from_mont()};   // Alpha, Beta, Delta in G1
+  const Fr v2[3] = {tx[2].from_mont(), tx[3].from_mont(), tx[4].from_mont()};   // Beta, Gamma, Delta in G2
+  CU(cudaMemcpyAsync(s1.as<Fr>() + *n1 - 3, v1, sizeof v1, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s2.as<Fr>() + m, v2, sizeof v2, cudaMemcpyHostToDevice, st));
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));   // ev is freed on return
+  return B200_OK;
+}
+
+// The Groth16 toxic values (T, Kalpha, Kbeta, Kgamma, Kdelta) as Montgomery elements, checked like the reference.
+int groth16_toxic(const R1cs* r, const uint64_t* toxic, Fr* tx, const char* what) {
+  int rc = load_toxic(toxic, 5, tx, what);
+  if (rc) return rc;
+  if (tx[3].is_zero() || tx[4].is_zero()) return fail(B200_EINVAL, "%s: Kgamma and Kdelta must be non-zero (groth16.go:151,201)", what);
+  return setup_check_tau(r, toxic, what);
+}
+
 int groth16_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uint64_t* at, uint64_t* b1, uint64_t* b2,
                        uint64_t* bacdelta, uint64_t* ptd, uint64_t* z, uint64_t* alpha1, uint64_t* beta1, uint64_t* delta1,
                        uint64_t* beta2, uint64_t* gamma2, uint64_t* delta2, uint64_t* ic) {
@@ -94,29 +129,15 @@ int groth16_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uin
   if (!at || !b1 || !b2 || !bacdelta || !ptd || !z || !alpha1 || !beta1 || !delta1 || !beta2 || !gamma2 || !delta2 || !ic)
     return fail(B200_EINVAL, "%s: null pointer", what);
   Fr tx[5];   // T, Kalpha, Kbeta, Kgamma, Kdelta
-  if ((rc = load_toxic(toxic, 5, tx, what))) return rc;
-  if (tx[3].is_zero() || tx[4].is_zero()) return fail(B200_EINVAL, "%s: Kgamma and Kdelta must be non-zero (groth16.go:151,201)", what);
-  if ((rc = setup_check_tau(r, toxic, what))) return rc;
+  if ((rc = groth16_toxic(r, toxic, tx, what))) return rc;
   const size_t m = r->m, l1 = npublic + 1;
   if ((rc = zero_poly_host(m - 2, z))) return rc;                  // Z = prod_{i=1..m-2}(x - i), groth16.go:122-132
   cudaStream_t st = g_ctx[0].main;
-  const size_t n1 = 4 * m - 1 + l1 + 3, n2 = m + 3;
-  DevBuf ev, s1, s2, p1, p2;
-  CU(ev.alloc(3 * m * sizeof(Fr)));
-  CU(s1.alloc(n1 * sizeof(Fr)));
-  CU(s2.alloc(n2 * sizeof(Fr)));
+  size_t n1, n2;
+  DevBuf s1, s2, p1, p2;
+  if ((rc = groth16_scalars(r, npublic, tx, s1, s2, &n1, &n2))) return rc;
   CU(p1.alloc(n1 * 3 * sizeof(Fq)));
   CU(p2.alloc(n2 * 3 * sizeof(Fq2)));
-  Fr zt;
-  if ((rc = qap_eval_at_enqueue(r, tx[0], m - 2, ev.as<Fr>(), &zt, st))) return rc;
-  const Fr inv_d = tx[4].inverse(), inv_g = tx[3].inverse();
-  k_groth16_setup_scalars<<<nblk(m, 128), 128, 0, st>>>(ev.as<Fr>(), (uint32_t)m, (uint32_t)npublic, tx[1], tx[2], inv_d, inv_g,
-                                                         zt * inv_d, tx[0], s1.as<Fr>(), s2.as<Fr>());
-  const Fr v1[3] = {tx[1].from_mont(), tx[2].from_mont(), tx[4].from_mont()};   // Alpha, Beta, Delta in G1
-  const Fr v2[3] = {tx[2].from_mont(), tx[3].from_mont(), tx[4].from_mont()};   // Beta, Gamma, Delta in G2
-  CU(cudaMemcpyAsync(s1.as<Fr>() + n1 - 3, v1, sizeof v1, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(s2.as<Fr>() + m, v2, sizeof v2, cudaMemcpyHostToDevice, st));
-  CU(cudaGetLastError());
   CU(fixed_base_mul<Fq>(s1.as<Fr>(), n1, p1.as<Fq>(), g_d_err, st));
   CU(fixed_base_mul<Fq2>(s2.as<Fr>(), n2, p2.as<Fq2>(), g_d_err, st));
   const Fq* g1 = p1.as<Fq>();
@@ -135,6 +156,33 @@ int groth16_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uin
   return check_err_flag(what, g_d_err);
 }
 
+// Steps 1-2 of the Pinocchio setup, as groth16_scalars: layouts of k_pinocchio_setup_scalars with Vkb, G1Kbg (G1) and
+// Vka, Vkc, G2Kbg, G2Kg, Vkz (G2) appended.  tx: T, Ka, Kb, Kc, Kbeta, Kgamma, RhoA, RhoB (Montgomery).
+int pinocchio_scalars(R1cs* r, const Fr* tx, DevBuf& s1, DevBuf& s2, size_t* n1, size_t* n2) {
+  const size_t m = r->m;
+  cudaStream_t st = g_ctx[0].main;
+  *n1 = 7 * m - 1 + 2;
+  *n2 = m + 5;
+  DevBuf ev;
+  CU(ev.alloc(3 * m * sizeof(Fr)));
+  CU(s1.alloc(*n1 * sizeof(Fr)));
+  CU(s2.alloc(*n2 * sizeof(Fr)));
+  Fr zt;
+  int rc = qap_eval_at_enqueue(r, tx[0], m - 2, ev.as<Fr>(), &zt, st);
+  if (rc) return rc;
+  const Fr rho_c = tx[6] * tx[7], kbg = tx[4] * tx[5];             // snark.go:150, :223-228
+  k_pinocchio_setup_scalars<<<nblk(m, 128), 128, 0, st>>>(ev.as<Fr>(), (uint32_t)m, tx[6], tx[7], rho_c, tx[1], tx[2], tx[3],
+                                                           tx[4], tx[0], s1.as<Fr>(), s2.as<Fr>());
+  const Fr v1[2] = {tx[2].from_mont(), kbg.from_mont()};                                   // Vkb, G1Kbg
+  const Fr v2[5] = {tx[1].from_mont(), tx[3].from_mont(), kbg.from_mont(), tx[5].from_mont(),
+                    (rho_c * zt).from_mont()};                                             // Vka, Vkc, G2Kbg, G2Kg, Vkz
+  CU(cudaMemcpyAsync(s1.as<Fr>() + *n1 - 2, v1, sizeof v1, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s2.as<Fr>() + m, v2, sizeof v2, cudaMemcpyHostToDevice, st));
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));   // ev is freed on return
+  return B200_OK;
+}
+
 int pinocchio_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, uint64_t* a, uint64_t* ap, uint64_t* b2,
                          uint64_t* bp, uint64_t* c, uint64_t* cp, uint64_t* kp, uint64_t* g1t, uint64_t* z, uint64_t* vk_g1,
                          uint64_t* vk_g2) {
@@ -149,24 +197,11 @@ int pinocchio_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, u
   const size_t m = r->m;
   if ((rc = zero_poly_host(m - 2, z))) return rc;                  // snark.go:210-221
   cudaStream_t st = g_ctx[0].main;
-  const size_t n1 = 7 * m - 1 + 2, n2 = m + 5;
-  DevBuf ev, s1, s2, p1, p2;
-  CU(ev.alloc(3 * m * sizeof(Fr)));
-  CU(s1.alloc(n1 * sizeof(Fr)));
-  CU(s2.alloc(n2 * sizeof(Fr)));
+  size_t n1, n2;
+  DevBuf s1, s2, p1, p2;
+  if ((rc = pinocchio_scalars(r, tx, s1, s2, &n1, &n2))) return rc;
   CU(p1.alloc(n1 * 3 * sizeof(Fq)));
   CU(p2.alloc(n2 * 3 * sizeof(Fq2)));
-  Fr zt;
-  if ((rc = qap_eval_at_enqueue(r, tx[0], m - 2, ev.as<Fr>(), &zt, st))) return rc;
-  const Fr rho_c = tx[6] * tx[7], kbg = tx[4] * tx[5];             // snark.go:150, :223-228
-  k_pinocchio_setup_scalars<<<nblk(m, 128), 128, 0, st>>>(ev.as<Fr>(), (uint32_t)m, tx[6], tx[7], rho_c, tx[1], tx[2], tx[3],
-                                                           tx[4], tx[0], s1.as<Fr>(), s2.as<Fr>());
-  const Fr v1[2] = {tx[2].from_mont(), kbg.from_mont()};                                   // Vkb, G1Kbg
-  const Fr v2[5] = {tx[1].from_mont(), tx[3].from_mont(), kbg.from_mont(), tx[5].from_mont(),
-                    (rho_c * zt).from_mont()};                                             // Vka, Vkc, G2Kbg, G2Kg, Vkz
-  CU(cudaMemcpyAsync(s1.as<Fr>() + n1 - 2, v1, sizeof v1, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(s2.as<Fr>() + m, v2, sizeof v2, cudaMemcpyHostToDevice, st));
-  CU(cudaGetLastError());
   CU(fixed_base_mul<Fq>(s1.as<Fr>(), n1, p1.as<Fq>(), g_d_err, st));
   CU(fixed_base_mul<Fq2>(s2.as<Fr>(), n2, p2.as<Fq2>(), g_d_err, st));
   const Fq* g1 = p1.as<Fq>();
@@ -178,4 +213,99 @@ int pinocchio_setup_host(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, u
   if ((rc = copy_points(b2, g2, 0, m, st))) return rc;
   if ((rc = copy_points(vk_g2, g2, m, 5, st))) return rc;
   return check_err_flag(what, g_d_err);
+}
+
+// ---- setup straight into a resident proving key (b200_groth16_setup_pk, b200_pinocchio_setup_pk) -------------------------
+// The scalars and Z as above, on the device; the generator tables once per group; the Vk points (few) minted and copied
+// out; then the key's load plan (groth16_pk_load / pinocchio_pk_load) mints only the sets, slices and tails this rank
+// holds, each straight into its table's row 0.  No host buffer proportional to m.
+
+// out[k] = the n_vk points minted from d_scalars[0..n_vk), copied to host arrays dst[k] of cnt[k] points each.
+template <class F>
+int mint_vk(const FixedBaseTable<F>& gen, const Fr* d_scalars, std::initializer_list<std::pair<uint64_t*, size_t>> dst) {
+  size_t n = 0;
+  for (const auto& d : dst) n += d.second;
+  DevBuf pts;
+  CU(pts.alloc(n * 3 * sizeof(F)));
+  CU(fixed_base_std<F>(gen, d_scalars, n, pts.as<F>(), g_ctx[0].main));
+  size_t first = 0;
+  for (const auto& d : dst) {
+    int rc = copy_points(d.first, pts.as<F>(), first, d.second, g_ctx[0].main);
+    if (rc) return rc;
+    first += d.second;
+  }
+  CU(cudaStreamSynchronize(g_ctx[0].main));
+  return B200_OK;
+}
+
+int groth16_setup_pk(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, int window_bits, int rank, int world,
+                     b200_pk_t* out, uint64_t* alpha1, uint64_t* beta2, uint64_t* gamma2, uint64_t* delta2, uint64_t* ic) {
+  const char* what = "groth16_setup_pk";
+  R1cs* r;
+  int rc = setup_check(h, npublic, toxic, &r, what);
+  if (rc) return rc;
+  if (!out || !alpha1 || !beta2 || !gamma2 || !delta2 || !ic) return fail(B200_EINVAL, "%s: null pointer", what);
+  if (world < 1 || rank < 0 || rank >= world) return fail(B200_EINVAL, "%s: bad shard %d/%d", what, rank, world);
+  Fr tx[5];
+  if ((rc = groth16_toxic(r, toxic, tx, what))) return rc;
+  const size_t m = r->m, l1 = npublic + 1;
+  cudaStream_t st = g_ctx[0].main;
+  size_t n1, n2;
+  DevBuf s1, s2, z;
+  if ((rc = groth16_scalars(r, npublic, tx, s1, s2, &n1, &n2))) return rc;
+  if ((rc = zero_poly_enqueue(m - 2, z))) return rc;
+  FixedBaseTable<Fq> gen1;
+  FixedBaseTable<Fq2> gen2;
+  CU(gen1.build(g_d_err, st));
+  CU(gen2.build(g_d_err, st));
+  // IC ++ Alpha are one range of the G1 layout, Beta, Gamma, Delta the tail of the G2 one
+  if ((rc = mint_vk<Fq>(gen1, s1.as<Fr>() + 4 * m - 1, {{ic, l1}, {alpha1, 1}}))) return rc;
+  if ((rc = mint_vk<Fq2>(gen2, s2.as<Fr>() + m, {{beta2, 1}, {gamma2, 1}, {delta2, 1}}))) return rc;
+  if ((rc = check_err_flag(what, g_d_err))) return rc;
+  MintSource ms;
+  ms.g1 = s1.as<Fr>();
+  ms.g2 = s2.as<Fr>();
+  ms.gen1 = &gen1;
+  ms.gen2 = &gen2;
+  ms.alpha = tx[1].from_mont();
+  ms.beta = tx[2].from_mont();
+  ms.delta = tx[4].from_mont();
+  ms.d_z = z.as<Fr>();
+  return groth16_pk_load(nullptr, nullptr, nullptr, nullptr, m, nullptr, m - 1, nullptr, m - 1, nullptr, nullptr, nullptr,
+                         nullptr, nullptr, npublic, window_bits, rank, world, out, &ms);
+}
+
+int pinocchio_setup_pk(b200_r1cs_t h, size_t npublic, const uint64_t* toxic, int window_bits, int rank, int world,
+                       b200_pk_t* out, uint64_t* vk_g1, uint64_t* vk_g2, uint64_t* ic) {
+  const char* what = "pinocchio_setup_pk";
+  R1cs* r;
+  int rc = setup_check(h, npublic, toxic, &r, what);
+  if (rc) return rc;
+  if (!out || !vk_g1 || !vk_g2 || !ic) return fail(B200_EINVAL, "%s: null pointer", what);
+  if (world < 1 || rank < 0 || rank >= world) return fail(B200_EINVAL, "%s: bad shard %d/%d", what, rank, world);
+  Fr tx[8];
+  if ((rc = load_toxic(toxic, 8, tx, what))) return rc;
+  if ((rc = setup_check_tau(r, toxic, what))) return rc;
+  const size_t m = r->m, l1 = npublic + 1;
+  cudaStream_t st = g_ctx[0].main;
+  size_t n1, n2;
+  DevBuf s1, s2, z;
+  if ((rc = pinocchio_scalars(r, tx, s1, s2, &n1, &n2))) return rc;
+  if ((rc = zero_poly_enqueue(m - 2, z))) return rc;
+  FixedBaseTable<Fq> gen1;
+  FixedBaseTable<Fq2> gen2;
+  CU(gen1.build(g_d_err, st));
+  CU(gen2.build(g_d_err, st));
+  if ((rc = mint_vk<Fq>(gen1, s1.as<Fr>(), {{ic, l1}}))) return rc;                  // IC = A[0..NPublic]
+  if ((rc = mint_vk<Fq>(gen1, s1.as<Fr>() + n1 - 2, {{vk_g1, 2}}))) return rc;
+  if ((rc = mint_vk<Fq2>(gen2, s2.as<Fr>() + m, {{vk_g2, 5}}))) return rc;
+  if ((rc = check_err_flag(what, g_d_err))) return rc;
+  MintSource ms;
+  ms.g1 = s1.as<Fr>();
+  ms.g2 = s2.as<Fr>();
+  ms.gen1 = &gen1;
+  ms.gen2 = &gen2;
+  ms.d_z = z.as<Fr>();
+  return pinocchio_pk_load(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, m, nullptr, m - 1, nullptr, m - 1,
+                           npublic, window_bits, rank, world, out, &ms);
 }

@@ -301,6 +301,41 @@ def GenerateTrustedSetupSparse(r1cs, nPublic, toxic=None):
     return SparseSetup(r1cs, nPublic, toxic)
 
 
+class ResidentSetup:
+    """A trusted setup made straight into a device-resident proving key: ``pk`` (a DeviceProvingKey), ``Vk`` (the dict
+    VerifyProof takes) and ``Toxic`` (the toxic values it was made with)."""
+
+    def __init__(self, pk, vk, toxic):
+        self.pk, self.Vk, self.Toxic = pk, vk, toxic
+
+
+def _resident_toxic(names, r1cs, toxic, world):
+    if toxic is None and world > 1:
+        raise ValueError("GenerateTrustedSetupResident: a sharded setup (world > 1) needs the toxic values every rank "
+                         "shares; independently drawn ones would give an inconsistent key")
+    tox = draw_toxic(names, r1cs.n) if toxic is None else dict(toxic)
+    return {k: int(tox[k]) for k in names}
+
+
+def GenerateTrustedSetupResident(r1cs, nPublic, toxic=None, window_bits=0, rank=0, world=1, table_windows=0):
+    """GenerateTrustedSetupSparse(r1cs, nPublic, toxic).load_pk(window_bits, rank, world, table_windows) in one call
+    (b200_groth16_setup_pk): the key is minted on the device straight into its tables, no CRS passes through host
+    memory, and rank ``rank`` of ``world`` mints only the part of the key it holds.  Every rank must pass the same toxic
+    values, so ``toxic`` is required when world > 1."""
+    names = SparseSetup.TOXIC
+    tox = _resident_toxic(names, r1cs, toxic, world)
+    g1 = lambda k: np.zeros((k, 12), dtype=np.uint64)
+    g2 = lambda k: np.zeros((k, 24), dtype=np.uint64)
+    alpha1, beta2, gamma2, delta2, ic = g1(1), g2(1), g2(1), g2(1), g1(nPublic + 1)
+    h = _lib._h(0)
+    with _lib.table_windows(table_windows):
+        check(lib().b200_groth16_setup_pk(r1cs.handle, nPublic, ptr(toxic_limbs(tox, names)), window_bits, rank, world, h,
+                                          ptr(alpha1), ptr(beta2), ptr(gamma2), ptr(delta2), ptr(ic)))
+    vk = {"IC": _unflatten_g1(ic), "G1": {"Alpha": _unflatten_g1(alpha1)[0]},
+          "G2": {"Beta": _unflatten_g2(beta2)[0], "Gamma": _unflatten_g2(gamma2)[0], "Delta": _unflatten_g2(delta2)[0]}}
+    return ResidentSetup(DeviceProvingKey.from_handle(h.value, r1cs.m), vk, tox)
+
+
 def VerifyProof(vk, proof, publicSignals, debug=False):
     """groth16.VerifyProof(vk, proof, publicSignals, debug) (groth16/groth16.go:281-305) on the GPU:
     vk = {"IC", "G1": {"Alpha"}, "G2": {"Beta", "Gamma", "Delta"}}, proof = {"PiA", "PiB", "PiC"}."""

@@ -212,6 +212,28 @@ def GenerateTrustedSetupSparse(r1cs, nPublic, toxic=None):
     return SparseSetup(r1cs, nPublic, toxic)
 
 
+def GenerateTrustedSetupResident(r1cs, nPublic, toxic=None, window_bits=0, rank=0, world=1, table_windows=0):
+    """GenerateTrustedSetupSparse(r1cs, nPublic, toxic).load_pk(window_bits, rank, world, table_windows) in one call
+    (b200_pinocchio_setup_pk): the key is minted on the device straight into its tables, no CRS passes through host
+    memory, and rank ``rank`` of ``world`` mints only the sets it holds.  Returns a groth16.ResidentSetup (``pk``, ``Vk``
+    as VerifyProof takes it, ``Toxic`` with RhoC).  Every rank must pass the same toxic values, so ``toxic`` is required
+    when world > 1."""
+    from .groth16 import ResidentSetup, _resident_toxic, toxic_limbs
+    names = SparseSetup.TOXIC
+    tox = _resident_toxic(names, r1cs, toxic, world)
+    vk_g1, vk_g2 = np.zeros((2, 12), dtype=np.uint64), np.zeros((5, 24), dtype=np.uint64)
+    ic = np.zeros((nPublic + 1, 12), dtype=np.uint64)
+    h = _lib._h(0)
+    with _lib.table_windows(table_windows):
+        check(lib().b200_pinocchio_setup_pk(r1cs.handle, nPublic, ptr(toxic_limbs(tox, names)), window_bits, rank, world, h,
+                                            ptr(vk_g1), ptr(vk_g2), ptr(ic)))
+    vk = dict(zip(("Vkb", "G1Kbg"), _unflatten_g1(vk_g1)))
+    vk.update(zip(("Vka", "Vkc", "G2Kbg", "G2Kg", "Vkz"), _unflatten_g2(vk_g2)))
+    vk["IC"] = _unflatten_g1(ic)
+    tox["RhoC"] = tox["RhoA"] * tox["RhoB"] % R
+    return ResidentSetup(DeviceProvingKey.from_handle(h.value), vk, tox)
+
+
 def VerifyProof(vk, proof, publicSignals, debug=False):
     """snark.VerifyProof(vk, proof, publicSignals, debug) (snark.go:292-372): the twelve pairings of the five checks run
     as ONE batched GPU call (lock-step lanes of a warp), the two F_q^12 products as another; the checks are then

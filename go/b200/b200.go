@@ -642,3 +642,56 @@ func (r *R1CS) PinocchioSetup(nPublic int, toxic [8]*big.Int) (*PinocchioSetup, 
 	s.IC = s.A[:nPublic+1]
 	return s, nil
 }
+
+// Groth16Vk holds the verification key of a setup made straight into a resident key: the Vk fields Groth16Setup fills.
+type Groth16Vk struct {
+	IC                    [][3]*big.Int
+	Alpha1                [3]*big.Int
+	Beta2, Gamma2, Delta2 [3][2]*big.Int
+}
+
+// Groth16SetupKey is Groth16Setup followed by LoadGroth16Shard(.., windowBits, rank, world) in one call
+// (b200_groth16_setup_pk): the key is minted on the device straight into its tables and no CRS passes through host
+// memory; a rank mints only the part it holds.  Every rank must pass the same toxic values.
+func (r *R1CS) Groth16SetupKey(nPublic int, toxic [5]*big.Int, windowBits, rank, world int) (*Groth16Key, Groth16Vk, error) {
+	var tox []uint64
+	for _, t := range toxic {
+		tox = limbs(tox, t)
+	}
+	a1, be2, g2, d2, ic := make([]uint64, 12), make([]uint64, 24), make([]uint64, 24), make([]uint64, 24), make([]uint64, 12*(nPublic+1))
+	var h C.b200_pk_t
+	rc := C.b200_groth16_setup_pk(r.h, C.size_t(nPublic), u64(tox), C.int(windowBits), C.int(rank), C.int(world), &h,
+		u64(a1), u64(be2), u64(g2), u64(d2), u64(ic))
+	if err := check(rc); err != nil {
+		return nil, Groth16Vk{}, err
+	}
+	return &Groth16Key{h}, Groth16Vk{IC: g1s(ic), Alpha1: G1FromLimbs(a1), Beta2: G2FromLimbs(be2), Gamma2: G2FromLimbs(g2),
+		Delta2: G2FromLimbs(d2)}, nil
+}
+
+// PinocchioVk holds the verification key of a setup made straight into a resident key: the Vk fields PinocchioSetup
+// fills (IC = A[0..nPublic]).
+type PinocchioVk struct {
+	IC                         [][3]*big.Int
+	Vkb, G1Kbg                 [3]*big.Int
+	Vka, Vkc, G2Kbg, G2Kg, Vkz [3][2]*big.Int
+}
+
+// PinocchioSetupKey is PinocchioSetup followed by LoadPinocchioShard(.., windowBits, rank, world) in one call
+// (b200_pinocchio_setup_pk).  Every rank must pass the same toxic values.
+func (r *R1CS) PinocchioSetupKey(nPublic int, toxic [8]*big.Int, windowBits, rank, world int) (*PinocchioKey, PinocchioVk, error) {
+	var tox []uint64
+	for _, t := range toxic {
+		tox = limbs(tox, t)
+	}
+	vk1, vk2, ic := make([]uint64, 24), make([]uint64, 120), make([]uint64, 12*(nPublic+1))
+	var h C.b200_pk_t
+	rc := C.b200_pinocchio_setup_pk(r.h, C.size_t(nPublic), u64(tox), C.int(windowBits), C.int(rank), C.int(world), &h,
+		u64(vk1), u64(vk2), u64(ic))
+	if err := check(rc); err != nil {
+		return nil, PinocchioVk{}, err
+	}
+	return &PinocchioKey{h}, PinocchioVk{IC: g1s(ic), Vkb: G1FromLimbs(vk1[:12]), G1Kbg: G1FromLimbs(vk1[12:]),
+		Vka: G2FromLimbs(vk2[:24]), Vkc: G2FromLimbs(vk2[24:48]), G2Kbg: G2FromLimbs(vk2[48:72]), G2Kg: G2FromLimbs(vk2[72:96]),
+		Vkz: G2FromLimbs(vk2[96:])}, nil
+}

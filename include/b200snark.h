@@ -376,6 +376,30 @@ int b200_groth16_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[20
 int b200_pinocchio_setup(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[32], uint64_t* a, uint64_t* ap,
                          uint64_t* b2, uint64_t* bp, uint64_t* c, uint64_t* cp, uint64_t* kp, uint64_t* g1t, uint64_t* z,
                          uint64_t vk_g1[24], uint64_t vk_g2[120]);
+/* ---- trusted setup straight into a device-resident proving key ----
+ * The key that b200_groth16_setup followed by b200_groth16_pk_load_shard(.., window_bits, rank, world) gives (Pinocchio:
+ * b200_pinocchio_setup, then b200_pinocchio_pk_load_shard), for the same toxic values and the same b200_config state
+ * (B200_CFG_ACC_MODE, B200_CFG_TABLE_WINDOWS, B200_CFG_PK_CONTEXT, B200_CFG_SHARD_*): the same window-table words, the
+ * same b200_groth16_shard_info and b200_pk_device_bytes, and the same proofs (as group elements: a proof's Jacobian words
+ * vary from run to run on any key, with the order of additions inside a bucket).  No CRS passes
+ * through host memory: the scalars and Z stay on the device and every point of the key is minted straight into its
+ * table.  A rank mints only what it holds (Groth16: its slices of A, B1, B2 and C||PTD and the blinding points of the
+ * sets whose tails it holds; Pinocchio: the whole sets dealt to it); the R1CS evaluation and Z are computed whole on every
+ * rank.  rank = 0, world = 1 gives the whole key.
+ *   - Call every rank with the same R1CS, npublic and toxic values.  No collective runs and no communicator is read.
+ *     Ranks given different toxic values hold parts of different keys: no call can detect it, and their proofs are wrong.
+ *   - Outputs (host): the Vk points as b200_groth16_setup / b200_pinocchio_setup return them, and ic (npublic+1 G1
+ *     points; Pinocchio: A[0..npublic]).  *out receives the key's handle (free with b200_pk_free).
+ *   - Synchronous, on the library stream.
+ *   - Errors: those of the setup (a bad handle, a null pointer, m < 3, npublic >= m, T in {1..n}, Kgamma or Kdelta = 0:
+ *     B200_EINVAL; a toxic value >= r: B200_ERANGE) and of the load (a bad rank / world, window_bits outside [2, 24]
+ *     and not 0, a set beyond 2^26 points or nwin * n >= 2^31: B200_EINVAL; B200_ENOMEM).  On any error no handle is
+ *     created and everything allocated is freed.  The Vk outputs may have been written.                            */
+int b200_groth16_setup_pk(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[20], int window_bits, int rank, int world,
+                          b200_pk_t* out, uint64_t alpha1[12], uint64_t beta2[24], uint64_t gamma2[24], uint64_t delta2[24],
+                          uint64_t* ic);
+int b200_pinocchio_setup_pk(b200_r1cs_t r1cs, size_t npublic, const uint64_t toxic[32], int window_bits, int rank, int world,
+                            b200_pk_t* out, uint64_t vk_g1[24], uint64_t vk_g2[120], uint64_t* ic);
 /* PolynomialField.LagrangeInterpolation over x = 1..n (r1csqap/r1csqap.go:150-158) at any n <= 2^26: n values ->
  * n coefficients.                                                                                                    */
 int b200_interpolate(const uint64_t* values, size_t n, uint64_t* coeffs);

@@ -8,6 +8,16 @@ discrete logs CircuitGroth16 / CircuitPinocchio derive in Python.  Prints one JS
 power limit.  --profile adds the CUDA time of each setup kernel from torch.profiler (a separate, untimed run).
 
     python tools/setup_bench.py --logn 16 --logn 20
+
+--resident compares the two ways to a device-resident proving key instead, per protocol and size (default 2^16, 2^20,
+2^22; add --logn 24 --t 1 for a one-row table): the host-clock wall time of setup + load (GenerateTrustedSetupSparse,
+then load_pk) against the one resident call (GenerateTrustedSetupResident), b200_pk_device_bytes of both keys, and the
+slowest rank of an N = 2 / 4 / 8 shard emulated on one GPU (each rank's resident call in turn) against the unsharded
+call.  One witness-fed proof per key is checked against its known discrete logs.  A size or path that runs out of memory
+is reported as such.
+
+    python tools/setup_bench.py --resident --logn 16 --logn 20 --logn 22
+    python tools/setup_bench.py --resident --logn 24 --t 1
 """
 import argparse
 import ctypes
@@ -166,6 +176,111 @@ def run(logn, reps, bcast_reps, sample, want_profile):
     return res
 
 
+def _qap_dlogs(qap, tox, proto, r, s):
+    """The known discrete logs of a witness-fed proof of qap's own witness (QAP identity h(T) Z(T) = A(T) B(T) - C(T)),
+    without the per-point lists of CircuitGroth16 / CircuitPinocchio (too large at 2^24)."""
+    from gosnark_b200.synthetic import pinocchio_proof_dlogs
+    w = qap.circuit.witness
+    if proto == "pin":
+        return pinocchio_proof_dlogs(qap.at_s, qap.bt_s, qap.ct_s, qap.zt, tox, qap.npublic, w)
+    R_, l1 = o.R, qap.npublic + 1
+    t, ka, kb, kg, kd = (tox[k] for k in ("T", "Kalpha", "Kbeta", "Kgamma", "Kdelta"))
+    dot = lambda v, lo=0, hi=None: sum(a * b for a, b in zip(v[lo:hi], w[lo:hi])) % R_
+    A, B, C = dot(qap.at_s), dot(qap.bt_s), dot(qap.ct_s)
+    Ap, Bp, Cp = dot(qap.at_s, 0, l1), dot(qap.bt_s, 0, l1), dot(qap.ct_s, 0, l1)
+    inv_d = pow(kd, -1, R_)
+    a = (A + ka + r * kd) % R_
+    b = (B + kb + s * kd) % R_
+    c_msm = inv_d * (kb * (A - Ap) + ka * (B - Bp) + (C - Cp)) % R_
+    c = (c_msm + (A * B - C) * inv_d + s * a + r * b - r * s * kd) % R_
+    return {"PiA": a, "PiB": b, "PiC": c}
+
+
+def _proof_ok(proto, pk, qap, tox):
+    r, s = 0x1234567, 0x7654321
+    p = pk.prove_witness_limbs(qap.r1cs, qap.w, r, s) if proto == "g16" else pk.prove_witness_limbs(qap.r1cs, qap.w)
+    for k, d in _qap_dlogs(qap, tox, proto, r, s).items():
+        G = o.BN.G2 if k == "PiB" else o.BN.G1
+        if G.affine(p[k]) != G.affine(G.mul_scalar(G.G, d)):
+            return False
+    return True
+
+
+def _oom(e):
+    return isinstance(e, MemoryError) or (isinstance(e, _lib.B200Error) and e.code == -6)
+
+
+def run_resident(logn, t, reps, protos):
+    """Two-step against resident, per protocol, at 2^logn with t stored window rows (0: all)."""
+    from gosnark_b200.synthetic import SEED_TOXIC, CircuitQAP, pinocchio_toxic, rand_limbs
+    n = 1 << logn
+    res = {"logn": logn, "n": n, "table_windows": t}
+    for proto, mod in (("g16", groth16), ("pin", snark)):
+        if proto not in protos:
+            continue
+        tox = (dict(zip(groth16.SparseSetup.TOXIC, (x % o.R for x in limbs_to_ints(rand_limbs(5, SEED_TOXIC)))))
+               if proto == "g16" else pinocchio_toxic())
+        qap = CircuitQAP(n, tox["T"])
+        r = res[proto] = {}
+
+        def two_step():
+            key = mod.GenerateTrustedSetupSparse(qap.r1cs, qap.npublic, toxic=tox).load_pk(table_windows=t)
+            return key
+
+        def resident(rank=0, world=1):
+            return mod.GenerateTrustedSetupResident(qap.r1cs, qap.npublic, toxic=tox, rank=rank, world=world,
+                                                    table_windows=t).pk
+
+        for name, make in (("two_step", two_step), ("resident", resident)):
+            warm = 1 if logn <= 20 else 0                             # a warm-up call at the small sizes
+            key = None
+            try:
+                ts = []
+                for _ in range(reps + warm):
+                    if key is not None:
+                        key.free()
+                    t0 = time.perf_counter()
+                    key = make()
+                    ts.append(time.perf_counter() - t0)
+                r[name + "_s"] = round(min(ts[warm:]), 3)
+                r[name + "_device_bytes"] = key.device_bytes()
+            except Exception as e:                                    # reported, not estimated
+                if not _oom(e):
+                    raise
+                r[name + "_s"] = "out of memory: " + str(e)[:160]
+            if key is not None and name + "_device_bytes" in r:
+                try:
+                    r[name + "_proof_ok"] = _proof_ok(proto, key, qap, tox)
+                except Exception as e:
+                    if not _oom(e):
+                        raise
+                    r[name + "_proof_ok"] = "out of memory: " + str(e)[:160]
+            if key is not None:
+                key.free()
+        shards = {}
+        for world in (2, 4, 8):
+            key = None
+            try:
+                worst = 0.0
+                for rank in range(world):
+                    t0 = time.perf_counter()
+                    key = resident(rank, world)
+                    worst = max(worst, time.perf_counter() - t0)
+                    key.free()
+                    key = None
+                shards[str(world)] = round(worst, 3)
+            except Exception as e:
+                if not _oom(e):
+                    raise
+                shards[str(world)] = "out of memory: " + str(e)[:160]
+                if key is not None:
+                    key.free()
+        r["resident_slowest_rank_s"] = shards
+        qap.r1cs.free()
+        del qap
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--logn", type=int, action="append", help="log2 of the constraint count (repeatable; default 16 and 20)")
@@ -174,12 +289,19 @@ def main():
     ap.add_argument("--sample", type=int, default=1024, help="points per output array checked against the CPU")
     ap.add_argument("--profile", action="store_true", help="also report per-kernel CUDA time (torch.profiler)")
     ap.add_argument("--out", help="append the JSON lines to this file")
+    ap.add_argument("--resident", action="store_true", help="setup + load against the setup into a resident key")
+    ap.add_argument("--t", type=int, default=0, help="--resident: stored window rows of the keys (0: all)")
+    ap.add_argument("--proto", choices=["g16", "pin", "both"], default="both", help="--resident: protocols to run")
     a = ap.parse_args()
     _lib.init()
     name, power = card()
-    for logn in a.logn or [16, 20]:
+    for logn in a.logn or ([16, 20, 22] if a.resident else [16, 20]):
         res = {"card": name, "power_limit": power}
-        res.update(run(logn, a.reps, a.bcast_reps, a.sample, a.profile))
+        if a.resident:
+            res.update(run_resident(logn, a.t, 1 if logn > 20 else min(a.reps, 3),
+                                    ("g16", "pin") if a.proto == "both" else (a.proto,)))
+        else:
+            res.update(run(logn, a.reps, a.bcast_reps, a.sample, a.profile))
         line = json.dumps(res)
         print(line, flush=True)
         if a.out:
