@@ -29,6 +29,7 @@
 #ifndef B200_NO_PAIRING
 #include "pairing.cuh"
 #include "pairing_warp.cuh"
+#include "verify_batch.cuh"
 #endif
 
 using namespace b200;
@@ -1701,15 +1702,14 @@ __global__ void __launch_bounds__(32 * kPairWarps) k_pairing_batch_warp(const Fq
   }
 }
 // groth16.VerifyProof (groth16/groth16.go:281-305): e(A,B) == e(alpha,beta) * (e(icPubl,gamma) * e(C,delta)).
-// pts1: A, alpha1, icPubl, C ; pts2: B, beta2, gamma2, delta2 (Jacobian standard form).  Four warps, one pairing each; warp 0
-// then forms the right-hand side with two warp-wide F_q^12 products and compares.
-__global__ void __launch_bounds__(128) k_groth16_verify(const Fq* pts1, const Fq2* pts2, int* ok, int* err) {
-  __shared__ wp::Ws wss[4];
+// Warp w of a 128-thread CTA pairs g1 with g2, the w-th of (A, alpha1, icPubl, C) and (B, beta2, gamma2, delta2) (Jacobian
+// standard form); warp 0 then forms the right-hand side with two warp-wide F_q^12 products and compares.
+__device__ void groth16_verify_cta(wp::Ws* wss, const Fq* g1, const Fq2* g2, int* ok, int* err) {
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   wp::Ws& ws = wss[warp];
   F2::B px, py;
   F2 qx, qy;
-  if (warp_pairing_inputs(ws, pts1 + 3 * warp, pts2 + 3 * warp, px, py, qx, qy, err)) wp::pairing(ws, px, py, qx, qy);
+  if (warp_pairing_inputs(ws, g1, g2, px, py, qx, qy, err)) wp::pairing(ws, px, py, qx, qy);
   else wp::f12_set_one(ws, wp::RF);
   __syncthreads();
   if (warp == 0) {
@@ -1725,6 +1725,31 @@ __global__ void __launch_bounds__(128) k_groth16_verify(const Fq* pts1, const Fq
     const unsigned all = __ballot_sync(0xffffffffu, same);
     if (lane == 0) *ok = all == 0xffffffffu ? 1 : 0;
   }
+}
+// pts1: A, alpha1, icPubl, C ; pts2: B, beta2, gamma2, delta2
+__global__ void __launch_bounds__(128) k_groth16_verify(const Fq* pts1, const Fq2* pts2, int* ok, int* err) {
+  __shared__ wp::Ws wss[4];
+  const uint32_t warp = threadIdx.x >> 5;
+  groth16_verify_cta(wss, pts1 + 3 * warp, pts2 + 3 * warp, ok, err);
+}
+// k_groth16_verify over a batch, one CTA per proof (verify_batch.cuh): a regular proof under a passed aggregate is accepted
+// at once, a bad one (coordinate >= q, signal >= r, PiB at infinity) gets 0, every other proof the single call's verdict.
+__global__ void __launch_bounds__(128) k_vb_verify_each(const uint64_t* proofs, const vb::Vk* vk, const Fq* icp,
+                                                        const uint32_t* flags, const uint32_t* agg, size_t k, int* ok,
+                                                        uint32_t* status, int* err) {
+  __shared__ wp::Ws wss[4];
+  const size_t p = blockIdx.x;
+  const uint32_t f = flags[p] | flags[k];
+  if ((f & vb::kBad) || (!f && *agg)) {
+    if (threadIdx.x == 0) ok[p] = (f & vb::kBad) ? 0 : 1;
+    return;
+  }
+  if (threadIdx.x == 0) atomicOr(status, vb::kStPerProof);
+  const uint32_t warp = threadIdx.x >> 5;
+  const vb::ProofView v = vb::proof_at(proofs, p);
+  const Fq* g1 = warp == 0 ? v.a : (warp == 1 ? vk->alpha : (warp == 2 ? icp + 3 * p : v.c));
+  const Fq2* g2 = warp == 0 ? v.b : (warp == 1 ? vk->beta : (warp == 2 ? vk->gamma : vk->delta));
+  groth16_verify_cta(wss, g1, g2, ok + p, err);
 }
 // icPubl = IC[0] + sum publicSignals[i] * IC[i+1] (groth16.go:283-286).  The products are independent: one half-warp each,
 // with the GLV split of prove_host.cuh (128 doublings + ~12 additions deep instead of the 254 + ~127 of MulScalar's
@@ -1835,8 +1860,191 @@ int groth16_verify_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1,
   return check_err_flag("groth16_verify", g_d_err);
 }
 
+// ---- batched verification (verify_batch.cuh) ----------------------------------------------------------------------------
+// Stream-ordered device memory: freed behind the work queued on its stream, so a _device call returns without waiting.
+struct StreamBuf {
+  void* p = nullptr;
+  cudaStream_t st = nullptr;
+  StreamBuf() = default;
+  StreamBuf(const StreamBuf&) = delete;
+  StreamBuf& operator=(const StreamBuf&) = delete;
+  ~StreamBuf() { if (p) cudaFreeAsync(p, st); }
+  cudaError_t alloc(size_t b, cudaStream_t s) {
+    st = s;
+    return cudaMallocAsync(&p, b, s);
+  }
+};
+// per-call scratch of verify_batch_enqueue, carved from one allocation
+struct VbScratch {
+  size_t off[10];
+  size_t bytes;
+  VbScratch(size_t k, size_t npub) {
+    const size_t n = k + 3, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
+    const size_t sz[10] = {(k + 1) * 4, 4, 4, 4, 3 * k * sizeof(Fq), (npub ? npub * k : 1) * sizeof(Jacobian<Fq>),
+                           3 * k * sizeof(Jacobian<Fq>), 3 * sizeof(Jacobian<Fq>), 6 * n * sizeof(F2), 6 * nparts * sizeof(F2)};
+    bytes = 0;
+    for (int i = 0; i < 10; i++) {
+      off[i] = bytes;
+      bytes += (sz[i] + 255) & ~(size_t)255;
+    }
+  }
+};
+// Every launch of a batch verification, on `st`: d_ok[0..k) verdicts, *d_status the status bits (zeroed here first).
+// A fixed launch sequence: no step waits for the host, whatever k and whatever the outcome.
+int verify_batch_enqueue(const Fq* d_ic, const vb::Vk* d_vk, const uint64_t* d_proofs, const uint64_t* d_pub, size_t npub,
+                         size_t k, const uint64_t* d_rho, int* d_ok, uint32_t* d_status, uint8_t* scratch, cudaStream_t st) {
+  const VbScratch L(k, npub);
+  uint32_t* flags = (uint32_t*)(scratch + L.off[0]);
+  uint32_t* k_reg = (uint32_t*)(scratch + L.off[1]);
+  uint32_t* agg = (uint32_t*)(scratch + L.off[2]);
+  int* err = (int*)(scratch + L.off[3]);
+  Fq* icp = (Fq*)(scratch + L.off[4]);
+  Jacobian<Fq>* terms = (Jacobian<Fq>*)(scratch + L.off[5]);
+  Jacobian<Fq>* rterms = (Jacobian<Fq>*)(scratch + L.off[6]);
+  Jacobian<Fq>* sums = (Jacobian<Fq>*)(scratch + L.off[7]);
+  F2* mvals = (F2*)(scratch + L.off[8]);
+  F2* parts = (F2*)(scratch + L.off[9]);
+  const size_t n = k + 3, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
+  CU(cudaMemsetAsync(scratch, 0, L.off[4], st));
+  CU(cudaMemsetAsync(d_status, 0, sizeof(uint32_t), st));
+  vb::k_vb_classify<<<nblk(k + 1, 64), 64, 0, st>>>(d_proofs, d_vk, k, flags, d_status);
+  if (npub) vb::k_vb_ic_terms<<<nblk(npub * k, 2), 32, 0, st>>>(d_ic, d_pub, npub, k, terms, flags, d_status);
+  vb::k_vb_ic_sum<<<nblk(k, 64), 64, 0, st>>>(d_ic, terms, npub, k, icp, flags, d_status);
+  vb::k_vb_rho_terms<<<nblk(3 * k, 2), 32, 0, st>>>(d_proofs, icp, d_rho, k, rterms);
+  vb::k_vb_sums<<<1, vb::kSumThreads, 0, st>>>(d_vk, rterms, d_rho, flags, k, sums, k_reg);
+  const vb::MlArgs ma{d_proofs, d_vk, rterms, sums, flags, k_reg, k};
+  // the kernel rule of b200_pairing_batch (B200_CFG_PAIRING_KERNEL; auto: a warp per pair up to 2048 pairs)
+  const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
+  if (thread_kernel) vb::k_vb_miller_thread<<<nblk(n, 32), 32, 0, st>>>(ma, n, mvals);
+  else vb::k_vb_miller_warp<<<nblk(n, vb::kMlWarps), 32 * vb::kMlWarps, 0, st>>>(ma, n, mvals);
+  vb::k_vb_product<<<(unsigned)nparts, 32 * vb::kProdWarps, 0, st>>>(mvals, n, parts);
+  vb::k_vb_final<<<1, 32 * vb::kProdWarps, 0, st>>>(parts, nparts, k_reg, agg, d_status);
+  k_vb_verify_each<<<(unsigned)k, 128, 0, st>>>(d_proofs, d_vk, icp, flags, agg, k, d_ok, d_status, err);
+  g_launches += npub ? 9 : 8;
+  CU(cudaGetLastError());
+  return B200_OK;
+}
+Fq fq_load_std(const uint64_t* v) {
+  Fq r;
+  memcpy(&r, v, sizeof(Fq));
+  return r;
+}
+// The checks both entries make on the host arguments of the Vk: b200_groth16_verify's, applied to the whole call.
+int verify_batch_check_vk(const char* what, const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2,
+                          const uint64_t* gamma2, const uint64_t* delta2, size_t npub, size_t k, const uint64_t* rho) {
+  if (!ic || !alpha1 || !beta2 || !gamma2 || !delta2 || !rho) return fail(B200_EINVAL, "%s: null pointer", what);
+  if (n_ic < npub + 1) return fail(B200_EINVAL, "%s: len(IC) < len(publicSignals) + 1", what);
+  if (k == 0 || k > vb::kMaxBatch) return fail(B200_EINVAL, "%s: k = %zu outside 1..%zu", what, k, vb::kMaxBatch);
+  for (size_t i = 0; i < k; i++)
+    if (!(rho[2 * i] | rho[2 * i + 1])) return fail(B200_EINVAL, "%s: rho[%zu] = 0", what, i);
+  for (size_t i = 0; i < 3 * n_ic; i++)
+    if (fq_load_std(ic + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: IC coordinate >= q", what);
+  const uint64_t* g2s[3] = {beta2, gamma2, delta2};
+  for (int c = 0; c < 3; c++) {
+    if (fq_load_std(alpha1 + 4 * c).geq_modulus()) return fail(B200_ERANGE, "%s: alpha1 coordinate >= q", what);
+    for (int j = 0; j < 6; j++)
+      if (fq_load_std(g2s[c] + 4 * j).geq_modulus()) return fail(B200_ERANGE, "%s: Vk G2 coordinate >= q", what);
+  }
+  for (int c = 0; c < 3; c++)
+    if (!(g2s[c][16] | g2s[c][17] | g2s[c][18] | g2s[c][19] | g2s[c][20] | g2s[c][21] | g2s[c][22] | g2s[c][23]))
+      return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (Vk G2 point at infinity; the reference panics, bn128.go:238-241)", what);
+  return B200_OK;
+}
+// device image of the Vk, IC and rho: vb::Vk | IC | rho
+size_t vb_vk_bytes(size_t n_ic, size_t k) { return sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq) + 2 * k * sizeof(uint64_t); }
+int vb_upload_vk(uint8_t* d, const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2, const uint64_t* gamma2,
+                 const uint64_t* delta2, size_t k, const uint64_t* rho, cudaStream_t st) {
+  std::vector<uint8_t> h(vb_vk_bytes(n_ic, k));
+  vb::Vk* v = (vb::Vk*)h.data();
+  std::memcpy(v->alpha, alpha1, sizeof v->alpha);
+  std::memcpy(v->beta, beta2, sizeof v->beta);
+  std::memcpy(v->gamma, gamma2, sizeof v->gamma);
+  std::memcpy(v->delta, delta2, sizeof v->delta);
+  std::memcpy(h.data() + sizeof(vb::Vk), ic, n_ic * 3 * sizeof(Fq));
+  std::memcpy(h.data() + sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq), rho, 2 * k * sizeof(uint64_t));
+  CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+  return B200_OK;
+}
+int groth16_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2, const uint64_t* gamma2,
+                              const uint64_t* delta2, const uint64_t* pi_a, const uint64_t* pi_b, const uint64_t* pi_c,
+                              const uint64_t* pub, size_t npub, size_t k, const uint64_t* rho, int* ok, uint32_t* status) {
+  const char* what = "groth16_verify_batch";
+  if (!pi_a || !pi_b || !pi_c || !ok || (npub && !pub)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = verify_batch_check_vk(what, ic, n_ic, alpha1, beta2, gamma2, delta2, npub, k, rho);
+  if (rc) return rc;
+  for (size_t i = 0; i < k * npub; i++)
+    if (fr_load_std(pub + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: scalar / coefficient >= r", what);
+  // the batch prover's layout, PiA | PiC | PiB per proof
+  std::vector<uint64_t> proofs(48 * k);
+  for (size_t p = 0; p < k; p++) {
+    std::memcpy(&proofs[48 * p], pi_a + 12 * p, 12 * sizeof(uint64_t));
+    std::memcpy(&proofs[48 * p + 12], pi_c + 12 * p, 12 * sizeof(uint64_t));
+    std::memcpy(&proofs[48 * p + 24], pi_b + 24 * p, 24 * sizeof(uint64_t));
+  }
+  for (size_t i = 0; i < 12 * k; i++)
+    if (fq_load_std(&proofs[4 * i]).geq_modulus()) return fail(B200_ERANGE, "%s: point coordinate >= q", what);
+  for (size_t p = 0; p < k; p++) {
+    const uint64_t* z = &proofs[48 * p + 40];
+    if (!(z[0] | z[1] | z[2] | z[3] | z[4] | z[5] | z[6] | z[7]))
+      return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (PiB of proof %zu at infinity; the reference panics, bn128.go:238-241)", what, p);
+  }
+  cudaStream_t st = g_ctx[0].main;
+  const size_t vkb = vb_vk_bytes(n_ic, k), pb = proofs.size() * sizeof(uint64_t), ub = (npub ? npub : 1) * k * 32,
+               okb = (k + 1) * sizeof(int);
+  const VbScratch L(k, npub);
+  StreamBuf buf;
+  CU(buf.alloc(vkb + pb + ub + okb + L.bytes + 1024, st));
+  uint8_t* d = (uint8_t*)buf.p;
+  auto carve = [&](size_t b) { uint8_t* r = d; d += (b + 255) & ~(size_t)255; return r; };
+  uint8_t* d_vk = carve(vkb);
+  uint64_t* d_proofs = (uint64_t*)carve(pb);
+  uint64_t* d_pub = (uint64_t*)carve(ub);
+  int* d_ok = (int*)carve(okb);
+  uint8_t* d_scratch = carve(L.bytes);
+  if ((rc = vb_upload_vk(d_vk, ic, n_ic, alpha1, beta2, gamma2, delta2, k, rho, st))) return rc;
+  CU(cudaMemcpyAsync(d_proofs, proofs.data(), pb, cudaMemcpyHostToDevice, st));
+  if (npub) CU(cudaMemcpyAsync(d_pub, pub, npub * k * 32, cudaMemcpyHostToDevice, st));
+  const Fq* d_ic = (const Fq*)(d_vk + sizeof(vb::Vk));
+  const uint64_t* d_rho = (const uint64_t*)(d_vk + sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq));
+  if ((rc = verify_batch_enqueue(d_ic, (const vb::Vk*)d_vk, d_proofs, d_pub, npub, k, d_rho, d_ok, (uint32_t*)(d_ok + k),
+                                 d_scratch, st)))
+    return rc;
+  std::vector<int> h_ok(k + 1);
+  CU(cudaMemcpyAsync(h_ok.data(), d_ok, okb, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  std::memcpy(ok, h_ok.data(), k * sizeof(int));
+  if (status) *status = (uint32_t)h_ok[k];
+  return B200_OK;
+}
+int groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2,
+                                const uint64_t* gamma2, const uint64_t* delta2, const void* d_proofs, const void* d_public,
+                                size_t npub, size_t k, const uint64_t* rho, void* d_ok, cudaStream_t st) {
+  const char* what = "groth16_verify_batch_device";
+  if (!d_proofs || !d_ok || (npub && !d_public)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = verify_batch_check_vk(what, ic, n_ic, alpha1, beta2, gamma2, delta2, npub, k, rho);
+  if (rc) return rc;
+  const size_t vkb = (vb_vk_bytes(n_ic, k) + 255) & ~(size_t)255;
+  const VbScratch L(k, npub);
+  StreamBuf buf;
+  CU(buf.alloc(vkb + L.bytes, st));
+  uint8_t* d = (uint8_t*)buf.p;
+  if ((rc = vb_upload_vk(d, ic, n_ic, alpha1, beta2, gamma2, delta2, k, rho, st))) return rc;
+  return verify_batch_enqueue((const Fq*)(d + sizeof(vb::Vk)), (const vb::Vk*)d, (const uint64_t*)d_proofs,
+                              (const uint64_t*)d_public, npub, k, (const uint64_t*)(d + sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq)),
+                              (int*)d_ok, (uint32_t*)((int*)d_ok + k), d + vkb, st);
+}
+
 #else  // experiment builds without the verifier side (ptxas 12.9 crashes on the pairing kernels under -DB200_KARATSUBA)
 int pairing_batch_host(const uint64_t*, const uint64_t*, size_t, uint64_t*) { return fail(B200_EINVAL, "pairing: not in this build variant"); }
+int groth16_verify_batch_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
+                              const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*, size_t, size_t, const uint64_t*,
+                              int*, uint32_t*) {
+  return fail(B200_EINVAL, "groth16_verify_batch: not in this build variant");
+}
+int groth16_verify_batch_device(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
+                                const void*, const void*, size_t, size_t, const uint64_t*, void*, cudaStream_t) {
+  return fail(B200_EINVAL, "groth16_verify_batch_device: not in this build variant");
+}
 int fq12_mul_batch_host(const uint64_t*, const uint64_t*, size_t, uint64_t*) { return fail(B200_EINVAL, "fq12_mul: not in this build variant"); }
 int groth16_verify_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
                         const uint64_t*, const uint64_t*, const uint64_t*, size_t, int*) {
@@ -2254,6 +2462,22 @@ int b200_groth16_verify(const uint64_t* ic, size_t n_ic, const uint64_t alpha1[1
                         const uint64_t pi_b[24], const uint64_t pi_c[12], const uint64_t* public_signals, size_t n_public,
                         int* ok) {
   B200_API_BODY(groth16_verify_host(ic, n_ic, alpha1, beta2, gamma2, delta2, pi_a, pi_b, pi_c, public_signals, n_public, ok))
+}
+int b200_groth16_verify_batch(const uint64_t* ic, size_t n_ic, const uint64_t alpha1[12], const uint64_t beta2[24],
+                              const uint64_t gamma2[24], const uint64_t delta2[24], const uint64_t* pi_a, const uint64_t* pi_b,
+                              const uint64_t* pi_c, const uint64_t* public_signals, size_t n_public, size_t k, const uint64_t* rho,
+                              int* ok, uint32_t* status) {
+  B200_API_BODY(groth16_verify_batch_host(ic, n_ic, alpha1, beta2, gamma2, delta2, pi_a, pi_b, pi_c, public_signals, n_public, k,
+                                          rho, ok, status))
+}
+int b200_groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t alpha1[12], const uint64_t beta2[24],
+                                     const uint64_t gamma2[24], const uint64_t delta2[24], const void* d_proofs,
+                                     const void* d_public, size_t n_public, size_t k, const uint64_t* rho, void* d_ok,
+                                     void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  return groth16_verify_batch_device(ic, n_ic, alpha1, beta2, gamma2, delta2, d_proofs, d_public, n_public, k, rho, d_ok,
+                                     stream ? (cudaStream_t)stream : g_ctx[0].main);
 }
 int b200_g1_add_batch(const uint64_t* p, const uint64_t* q, size_t n, uint64_t* out) { B200_API_BODY(group_op_host<Fq>(0, p, q, n, out)) }
 int b200_g1_double_batch(const uint64_t* p, size_t n, uint64_t* out) { B200_API_BODY(group_op_host<Fq>(1, p, nullptr, n, out)) }

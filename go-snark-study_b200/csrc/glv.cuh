@@ -27,15 +27,16 @@ __device__ __forceinline__ Jacobian<Fq> shfl_jac(const Jacobian<Fq>& v, int lane
   for (int w = 0; w < (int)(sizeof(Jacobian<Fq>) / 4); w++) dst[w] = __shfl_sync(0xffffffffu, src[w], lane);
   return r;
 }
-// complete addition on top of the reference formula (which has no doubling branch)
-__device__ Jacobian<Fq> jac_add_complete(const Jacobian<Fq>& a, const Jacobian<Fq>& b) {
+// complete addition on top of the reference formula (which has no doubling branch); G1 and G2
+template <class F>
+__device__ Jacobian<F> jac_add_complete(const Jacobian<F>& a, const Jacobian<F>& b) {
   if (a.is_inf()) return b;
   if (b.is_inf()) return a;
-  Jacobian<Fq> r = jac_add_ref(a, b);
+  Jacobian<F> r = jac_add_ref(a, b);
   if (r.Z.is_zero()) {  // same x: either a == b (double) or a == -b (infinity)
-    Fq z1z1 = a.Z.sqr(), z2z2 = b.Z.sqr();
+    F z1z1 = a.Z.sqr(), z2z2 = b.Z.sqr();
     if (a.Y * (b.Z * z2z2) == b.Y * (a.Z * z1z1)) return jac_double_ref(a);
-    return Jacobian<Fq>::inf();
+    return Jacobian<F>::inf();
   }
   return r;
 }
@@ -83,9 +84,10 @@ __device__ Jacobian<Fq> glv_mul_halfwarp(Jacobian<Fq> p, const uint64_t k[4], co
 // k = k1 + k2*lambda (mod r), |k1|, |k2| < 2^128.  Lattice basis of BN254's GLV endomorphism:
 //   a1 = 0x89d3256894d213e3, b1 = -0x6f4d8248eeb859fc8211bbeb7d4f1128, a2 = 0x6f4d8248eeb859fd0be4e1541221250b, b2 = a1
 // c1 = round(b2*k/r), c2 = round(-b1*k/r) through g_i = round(2^256 * |.| / r);  k1 = k - c1*a1 - c2*a2,  k2 = c1*|b1| - c2*b2.
-// Any rounding error only lengthens k1, k2 by a bit; k1 + k2*lambda == k holds by construction.
+// Any rounding error only lengthens k1, k2 by a bit; k1 + k2*lambda == k holds by construction.  Host and device: the
+// batch verifier splits public signals that are already in device memory (verify_batch.cuh).
 struct U5 { uint64_t l[5]; };
-inline U5 u5_mul(const uint64_t* a, int na, const uint64_t* b, int nb) {  // (na + nb <= 5 significant limbs)
+HD U5 u5_mul(const uint64_t* a, int na, const uint64_t* b, int nb) {  // (na + nb <= 5 significant limbs)
   uint64_t t[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   for (int i = 0; i < na; i++) {
     unsigned __int128 c = 0;
@@ -100,7 +102,7 @@ inline U5 u5_mul(const uint64_t* a, int na, const uint64_t* b, int nb) {  // (na
   for (int i = 0; i < 5; i++) r.l[i] = t[i];
   return r;
 }
-inline U5 u5_sub(const U5& a, const U5& b) {
+HD U5 u5_sub(const U5& a, const U5& b) {
   U5 r;
   unsigned __int128 br = 0;
   for (int i = 0; i < 5; i++) {
@@ -110,7 +112,7 @@ inline U5 u5_sub(const U5& a, const U5& b) {
   }
   return r;
 }
-inline bool u5_abs(U5& a) {  // two's complement -> magnitude; returns the sign
+HD bool u5_abs(U5& a) {  // two's complement -> magnitude; returns the sign
   bool neg = (a.l[4] >> 63) != 0;
   if (neg) {
     unsigned __int128 c = 1;
@@ -122,10 +124,10 @@ inline bool u5_abs(U5& a) {  // two's complement -> magnitude; returns the sign
   }
   return neg;
 }
-inline int glv_decompose(const Fr& k_std, uint64_t out[4], uint32_t neg[2]) {
-  static const uint64_t A1[2] = {0x89d3256894d213e3ULL, 0}, B1m[2] = {0x8211bbeb7d4f1128ULL, 0x6f4d8248eeb859fcULL};
-  static const uint64_t A2[2] = {0x0be4e1541221250bULL, 0x6f4d8248eeb859fdULL}, B2[2] = {0x89d3256894d213e3ULL, 0};
-  static const uint64_t G1c[3] = {0xd91d232ec7e0b3d7ULL, 0x2ULL, 0}, G2c[3] = {0x7a7bd9d4391eb18eULL, 0x4ccef014a773d2cfULL, 0x2ULL};
+HD int glv_decompose(const Fr& k_std, uint64_t out[4], uint32_t neg[2]) {
+  const uint64_t A1[2] = {0x89d3256894d213e3ULL, 0}, B1m[2] = {0x8211bbeb7d4f1128ULL, 0x6f4d8248eeb859fcULL};
+  const uint64_t A2[2] = {0x0be4e1541221250bULL, 0x6f4d8248eeb859fdULL}, B2[2] = {0x89d3256894d213e3ULL, 0};
+  const uint64_t G1c[3] = {0xd91d232ec7e0b3d7ULL, 0x2ULL, 0}, G2c[3] = {0x7a7bd9d4391eb18eULL, 0x4ccef014a773d2cfULL, 0x2ULL};
   uint64_t k[4];
   memcpy(k, &k_std, 32);
   auto round_shift = [&](const uint64_t* g, uint64_t c[3]) {  // (k * g + 2^255) >> 256

@@ -201,8 +201,9 @@ HDN F12 final_exp_fast(const F12& f) {
   return f12_mul(f12_sqr(t0), t1);
 }
 
-template <bool FAST_FE>
-HDN F12 pairing_affine_t(const F2::B& px, const F2::B& py, const F2& qx, const F2& qy) {
+// MillerLoop(preComputeG1, preComputeG2) alone (bn128.go:354-398): the value pairing_affine_t exponentiates.  Miller values
+// of several pairs may be multiplied before ONE final exponentiation (verify_batch.cuh).
+HD F12 miller_loop_affine(const F2::B& px, const F2::B& py, const F2& qx, const F2& qy) {
   F2 X = qx, Y = qy, Z = F2::one();
   F12 f = F12::one();
   // bits of LoopCount from BitLen-2 down to 0 (bn128.go:228-236, 354-372), precompute fused with the loop
@@ -223,7 +224,11 @@ HDN F12 pairing_affine_t(const F2::B& px, const F2::B& py, const F2& qx, const F
   EllCoeffs c = pairing_mixed_addition_step(q1x, q1y, X, Y, Z);
   f = pairing_line(f, c, px, py);
   c = pairing_mixed_addition_step(q2x, q2y, X, Y, Z);
-  f = pairing_line(f, c, px, py);
+  return pairing_line(f, c, px, py);
+}
+template <bool FAST_FE>
+HDN F12 pairing_affine_t(const F2::B& px, const F2::B& py, const F2& qx, const F2& qy) {
+  const F12 f = miller_loop_affine(px, py, qx, qy);
   if (FAST_FE) return final_exp_fast(f);
   return final_exp_plain(f);
 }

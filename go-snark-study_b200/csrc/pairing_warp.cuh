@@ -246,10 +246,10 @@ DEV void pairing_constants(Ws& ws) {
   wsync();
 }
 
-// Pairing of affine Montgomery-form inputs: the value of pairing_affine_t<true> in r[0] (all lanes call; px, py, qx, qy
+// Miller loop of affine Montgomery-form inputs: the value of miller_loop_affine in r[0] (all lanes call; px, py, qx, qy
 // need only be valid on lane 0).
 constexpr int RF = 0, RS = 1;   // accumulator, line value
-DEV void pairing(Ws& ws, const F2::B& px, const F2::B& py, const F2& qx, const F2& qy) {
+DEV void miller_loop(Ws& ws, const F2::B& px, const F2::B& py, const F2& qx, const F2& qy) {
   const uint32_t lane = lane_id();
   if (lane == 0) {
     ws.px = px;
@@ -285,7 +285,10 @@ DEV void pairing(Ws& ws, const F2::B& px, const F2::B& py, const F2& qx, const F
   f12_mul(ws, RF, RF, RS);
   addition_step(ws, RS, 2);
   f12_mul(ws, RF, RF, RS);
-  // final exponentiation, Devegili-Scott-Dahab (pairing.cuh final_exp_fast, same operations)
+}
+// r[0] <- r[0]^((q^12 - 1) / r): Devegili-Scott-Dahab (pairing.cuh final_exp_fast, same operations); uses r[1..11] and
+// the Frobenius constants (pairing_constants)
+DEV void final_exp(Ws& ws) {
   enum { M = 2, MU = 3, MU2 = 4, MU3 = 5, Y0 = 6, Y2 = 7, Y3 = 8, Y4 = 9, Y6 = 10, T0 = 11, T1 = 1 };
   f12_inverse(ws, T0, RF);
   f12_conj(ws, M, RF);
@@ -325,6 +328,12 @@ DEV void pairing(Ws& ws, const F2::B& px, const F2::B& py, const F2& qx, const F
   f12_mul(ws, T1, T1, Y0);               // t1 = t1 y0
   f12_sqr(ws, T0, T0);
   f12_mul(ws, RF, T0, T1);
+}
+// Pairing of affine Montgomery-form inputs: the value of pairing_affine_t<true> in r[0] (all lanes call; px, py, qx, qy
+// need only be valid on lane 0).
+DEV void pairing(Ws& ws, const F2::B& px, const F2::B& py, const F2& qx, const F2& qy) {
+  miller_loop(ws, px, py, qx, qy);
+  final_exp(ws);
 }
 
 }  // namespace wp

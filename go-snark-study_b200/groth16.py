@@ -351,3 +351,75 @@ def VerifyProof(vk, proof, publicSignals, debug=False):
     if debug:
         print("✓ groth16 verification passed" if ok.value else "❌ groth16 verification not passed")
     return bool(ok.value)
+
+
+# status word of b200_groth16_verify_batch(_device) (include/b200snark.h)
+VB_AGGREGATE, VB_PER_PROOF, VB_ROUTED, VB_RANGE = 1, 2, 4, 8
+
+
+def draw_rho(k):
+    """k randomisers for a batch verification: secrets.randbits(128), zeros redrawn."""
+    out = []
+    while len(out) < k:
+        v = secrets.randbits(128)
+        if v:
+            out.append(v)
+    return out
+
+
+def _rho_limbs(rho):
+    return np.array([w for v in rho for w in (int(v) & (2**64 - 1), int(v) >> 64)], dtype=np.uint64)
+
+
+def _vk_args(vk):
+    return (_flatten_g1(vk["IC"]), _flatten_g1([vk["G1"]["Alpha"]]), _flatten_g2([vk["G2"]["Beta"]]),
+            _flatten_g2([vk["G2"]["Gamma"]]), _flatten_g2([vk["G2"]["Delta"]]))
+
+
+def verify_batch_limbs(vk, proofs, publicSignalsList, rho=None):
+    """b200_groth16_verify_batch: (list of k verdicts, status word).  ``rho``: k randomisers in 1..2^128 - 1 (drawn
+    with draw_rho when None; pass them for reproducible runs)."""
+    import ctypes
+    k = len(proofs)
+    if k == 0 or len(publicSignalsList) != k:
+        raise ValueError("verify_batch: need k >= 1 proofs and one publicSignals list per proof")
+    npub = len(publicSignalsList[0])
+    if any(len(ps) != npub for ps in publicSignalsList):
+        raise ValueError("verify_batch: every proof needs the same number of public signals")
+    rho = draw_rho(k) if rho is None else list(rho)
+    ic, a1, b2, g2, d2 = _vk_args(vk)
+    pa = _flatten_g1([p["PiA"] for p in proofs])
+    pb = _flatten_g2([p["PiB"] for p in proofs])
+    pc = _flatten_g1([p["PiC"] for p in proofs])
+    pub = (ints_to_limbs([reduce_scalar(x) for ps in publicSignalsList for x in ps]) if npub
+           else np.zeros((1, 4), dtype=np.uint64))
+    ok = np.zeros(k, dtype=np.int32)
+    status = ctypes.c_uint32(0)
+    check(lib().b200_groth16_verify_batch(ptr(ic), len(vk["IC"]), ptr(a1), ptr(b2), ptr(g2), ptr(d2), ptr(pa), ptr(pb),
+                                          ptr(pc), ptr(pub), npub, k, ptr(_rho_limbs(rho)), ptr(ok), ctypes.byref(status)))
+    return [bool(v) for v in ok], status.value
+
+
+def VerifyProofBatch(vk, proofs, publicSignalsList, rho=None):
+    """[groth16.VerifyProof(vk, proofs[i], publicSignalsList[i]) for every i] in one call (b200_groth16_verify_batch): one
+    random linear combination of the regular proofs, k + 3 Miller loops and one final exponentiation; irregular proofs,
+    and every proof of a batch whose combination fails, get the single call's verdict.  ``rho`` defaults to fresh
+    128-bit randomisers (secrets.randbits), which is what makes an invalid proof's acceptance improbable."""
+    return verify_batch_limbs(vk, proofs, publicSignalsList, rho)[0]
+
+
+def VerifyProofBatchDevice(vk, d_proofs, d_public, k, n_public, rho=None, d_ok=None, stream=None):
+    """b200_groth16_verify_batch_device on a batch in device memory: ``d_proofs`` is the output tensor of
+    b200_groth16_prove_witness_batch_device (k x 48 words, PiA | PiC | PiB), ``d_public`` the k x n_public x 4 standard-form
+    signals.  Queued on ``stream`` (a torch.cuda.Stream; None: the library's main stream) without waiting; returns the
+    int32 tensor of k verdicts followed by the status word (``d_ok``, allocated when None)."""
+    import torch
+    rho = draw_rho(k) if rho is None else list(rho)
+    if d_ok is None:
+        d_ok = torch.zeros(k + 1, dtype=torch.int32, device=d_proofs.device)
+    ic, a1, b2, g2, d2 = _vk_args(vk)
+    check(lib().b200_groth16_verify_batch_device(ptr(ic), len(vk["IC"]), ptr(a1), ptr(b2), ptr(g2), ptr(d2),
+                                                 d_proofs.data_ptr(), d_public.data_ptr() if n_public else None, n_public,
+                                                 k, ptr(_rho_limbs(rho)), d_ok.data_ptr(),
+                                                 None if stream is None else stream.cuda_stream))
+    return d_ok

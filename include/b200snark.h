@@ -70,7 +70,8 @@ int b200_version(void);
  * bn128.go:179-421, a long chain of dependent multiplications per pairing) or one WARP per pairing (2: F_q^12 in shared
  * memory, 27 F_q^2 products of a tower multiplication on 27 lanes; csrc/pairing_warp.cuh); 0 = auto: a warp per
  * pairing up to 2048 pairings per call (latency), a thread per pairing above (throughput).
- * Bit-identical F_q^12 values.  b200_groth16_verify always runs four warps.          */
+ * Bit-identical F_q^12 values.  b200_groth16_verify always runs four warps.  The same rule picks the Miller-loop
+ * kernel of b200_groth16_verify_batch(_device) over its k_reg + 3 pairs.                                               */
 #define B200_CFG_PAIRING_KERNEL 5
 /* Partition tuning of SHARDED proving keys loaded afterwards (defaults = the measured best for one proof at a time):
  * cost weight x100 of an A / B1 term (10) and of a G2 term (11) in C||PTD terms, and the
@@ -316,6 +317,42 @@ int b200_groth16_verify(const uint64_t* ic, size_t n_ic, const uint64_t alpha1[1
                         const uint64_t gamma2[24], const uint64_t delta2[24], const uint64_t pi_a[12],
                         const uint64_t pi_b[24], const uint64_t pi_c[12], const uint64_t* public_signals, size_t n_public,
                         int* ok);
+/* ok[i] = groth16.VerifyProof(vk, proof_i, publicSignals_i) for k proofs under one Vk, by one random linear combination:
+ *   prod_i e(rho_i A_i, B_i) * e(-(sum rho_i) alpha, beta) * e(-sum rho_i icPubl_i, gamma) * e(-sum rho_i C_i, delta) == 1
+ * over the REGULAR proofs: k_reg + 3 Miller loops, one F_q^12 product and ONE final exponentiation for the batch.
+ * A proof is regular when PiA and PiC are on y^2 = x^3 + 3 and not infinity, PiB is on the twist and in the order-r
+ * subgroup, and its icPubl_i (computed as b200_groth16_verify does, in the reference's order with its Add) is not
+ * infinity; under a Vk whose alpha1, beta2, gamma2, delta2 fail the same tests no proof is regular.  The contract:
+ *   - every irregular proof gets exactly b200_groth16_verify's verdict (the reference pairs a G1 infinity as (0, 0),
+ *     which is not bilinear, so such proofs never enter the aggregate);
+ *   - when the aggregate fails, every proof gets exactly b200_groth16_verify's verdict (the per-proof check runs);
+ *   - when it passes, every regular proof is accepted.  A batch holding an invalid regular proof passes with probability
+ *     below 2^-127 over that proof's rho_i, PROVIDED the randomisers are unpredictable to whoever made the proofs: draw
+ *     them from a cryptographic source per call.  The caller supplies them so that runs are reproducible.
+ * rho: k x 2 limbs, each 1 <= rho_i < 2^128.  pi_a, pi_c: k x 12, pi_b: k x 24, public_signals: k x n_public x 4,
+ * standard-form Jacobian / scalars as b200_groth16_verify takes them.  1 <= k <= 65536.
+ * status (may be NULL): bit 0 the aggregate ran over at least one proof and passed; bit 1 the per-proof check ran for
+ * some proof; bit 2 an irregular proof or Vk was routed around the aggregate.
+ * Errors are b200_groth16_verify's applied to the whole call: B200_ERANGE for a coordinate >= q or a public signal >= r,
+ * B200_EINVAL for a G2 input at infinity (the reference panics), a null pointer, n_ic < n_public + 1, k outside
+ * 1..65536, or a rho_i of 0.  Runs on context 0's main stream; synchronous.
+ * Launches: a fixed sequence of 9 kernels (8 when n_public = 0), whatever k and whatever the outcome.              */
+int b200_groth16_verify_batch(const uint64_t* ic, size_t n_ic, const uint64_t alpha1[12], const uint64_t beta2[24],
+                              const uint64_t gamma2[24], const uint64_t delta2[24], const uint64_t* pi_a, const uint64_t* pi_b,
+                              const uint64_t* pi_c, const uint64_t* public_signals, size_t n_public, size_t k, const uint64_t* rho,
+                              int* ok, uint32_t* status);
+/* b200_groth16_verify_batch on proofs already in device memory, queued on `stream` (NULL: context 0's main stream)
+ * without waiting: d_proofs is k x 48 uint64, PiA | PiC | PiB per proof — exactly b200_groth16_prove_witness_batch_device's
+ * d_out, so a batch is verified where it lies; d_public is k x n_public x 4 (standard form); d_ok receives k int32
+ * verdicts followed by one uint32 status word (bits 0..2 as above; bit 3: an out-of-range input was seen).
+ * The Vk, IC and rho are host arguments and are checked as b200_groth16_verify_batch checks them (B200_ERANGE /
+ * B200_EINVAL).  A proof coordinate >= q or a public signal >= r gives that proof verdict 0 and sets status bit 3; a PiB
+ * at infinity gives verdict 0.  Neither returns an error code, and nothing of either reaches a later call.  Scratch is
+ * stream-ordered device memory (cudaMallocAsync), freed behind the work.                                             */
+int b200_groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t alpha1[12], const uint64_t beta2[24],
+                                     const uint64_t gamma2[24], const uint64_t delta2[24], const void* d_proofs,
+                                     const void* d_public, size_t n_public, size_t k, const uint64_t* rho, void* d_ok,
+                                     void* stream);
 
 /* ---- dense QAP API upstream of GenerateProofs (small n; the prove path consumes px) ---- */
 /* PolynomialField.R1CSToQAP (r1csqap/r1csqap.go:161-188).  a, b, c: n x m row-major R1CS matrices (coefficients
