@@ -842,9 +842,6 @@ int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint6
     return fail(B200_ERANGE, "groth16_prove_witness: r or s >= field order");
   const size_t npx = 2 * r1->n - 1;
   if (!pk_needs_px(pk)) return groth16_enqueue(pk, d_w, pk->m, nullptr, npx, r, s, d_out, st, err);
-  R1csWork* ws;
-  int rc = r1cs_work(r1, pk->ctx, &ws);
-  if (rc) return rc;
   // the quotient is only consumed on side stream 3 (groth16_enqueue): compute it THERE, so the QAP front end (NTT passes,
   // HBM-bound) overlaps the A / B1 / B2 bucket phases (multiply-bound) on the other streams
   cudaStream_t sq = g_serial ? st : pk->pctx().side[2];
@@ -852,17 +849,10 @@ int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint6
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
-  // h = (ax*bx - cx) / Z straight from the witness (no px): the shapes whose proofs can verify have Z = prod_{i<=n}(x - i)
-  // (m = n + 2, SURVEY H5) or Z = prod_{i<n}(x - i) (m = n + 1: h = (x - n) q + kappa, qap_sparse.cuh) — checked; anything
-  // else goes through px and the division.
-  if (r1->n >= 2 && (pk->Z.nb == r1->n + 1 || pk->Z.nb == r1->n)) {
-    if (pk->Z.nb == r1->n + 1) rc = qap_h_enqueue(r1, *ws, *pk->pctx().poly, d_w, err, sq);
-    else rc = qap_h_short_enqueue(r1, *ws, *pk->pctx().poly, d_w, err, sq);
-    if (rc) return rc;
-    return groth16_enqueue(pk, d_w, pk->m, nullptr, npx, r, s, d_out, st, err, 0, ws->h_std.as<Fr>());
-  }
-  if ((rc = qap_px_enqueue(r1, *ws, *pk->pctx().poly, d_w, nullptr, nullptr, err, sq))) return rc;
-  return groth16_enqueue(pk, d_w, pk->m, ws->px_mont.as<Fr>(), npx, r, s, d_out, st, err, /*px_mont=*/1);
+  const Fr *h, *px;   // h itself, or px for groth16_enqueue's division
+  int rc = qap_quotient_enqueue(r1, pk->Z.nb, pk->ctx, *pk->pctx().poly, d_w, err, sq, &h, &px);
+  if (rc) return rc;
+  return groth16_enqueue(pk, d_w, pk->m, px, npx, r, s, d_out, st, err, /*px_mont=*/1, h);
 }
 
 int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, const uint64_t* r, const uint64_t* s,
@@ -879,14 +869,14 @@ int groth16_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t
   if ((rc = stage_witness(pk, w, pk_needs_px(pk), st))) return rc;
   Fq* o = pk->out_std.as<Fq>();
   if ((rc = groth16_witness_enqueue(pk, r1, pk->w_stage.as<Fr>(), r, s, o, st, pk->d_err_sync.as<int>()))) return rc;
-  return finish_host_proof(pk, o, "groth16_prove_witness", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
+  return finish_host_proof(pk, pk->h_out, o, 1, "groth16_prove_witness", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
 }
 
 // ---- batches: k witness-fed proofs under one key (b200_groth16_prove_witness_batch) ---------------------------------
 // Proof p is the proof of groth16_witness_enqueue for (w_p, r_p, s_p).  The four MSMs run as batched MSMs over k scalar
 // vectors (W_p = w_p ++ [1, r_p, s_p] for A, B1, B2 with one shared sort; C||PTD_p), the quotients as one batched front
-// end (len(Z) = n + 1: qap_h_batch_enqueue; len(Z) = n: qap_h_short_batch_enqueue), the blinding products with one warp
-// per proof: the launches of one proof, whatever k.
+// end (qap_quotient_batch_enqueue; len(Z) = n + 1 or n), the blinding products with one warp per proof: the launches of
+// one proof, whatever k.
 // On a key shard every vector is the rank's part of it (G16Slices), and the batch ends in k partial records.
 
 // Everything that is refused before anything is allocated or enqueued.  On a key shard every refusal is decided on
@@ -901,26 +891,23 @@ int groth16_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_t 
   if (npx - pk->Z.nb + 1 > pk->n_h_bases)
     return fail(B200_EINVAL, "%s: len(hx)=%zu exceeds len(PowersTauDelta)=%zu", what, npx - pk->Z.nb + 1, pk->n_h_bases);
   const size_t terms[4] = {pk->m + 3, pk->m + 3, pk->m + 3, pk->n_c_full + pk->n_h_bases + 1};
+  uint32_t nwin;
   if (pk->world == 1) {
     for (int j = 0; j < 4; j++)
-      if (!pk->g[j] || !batch_fits(pk->g[j].get(), k, terms[j]))
+      if (!pk_batch_fits(pk, j, k, terms[j], &nwin))
         return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
-                    pk->g[j] ? pk->g[j]->sh.nwin : 0u, terms[j], j);
+                    nwin, terms[j], j);
   } else {   // the largest part any rank holds: the shape each rank's set was built with, from its cut
     for (int g = 0; g < pk->world; g++) {
       const G16Slices sl = g16_slices(pk, g);
-      for (int j = 0; j < 4; j++) {
-        const size_t n = sl.terms[j];
-        if (!n) continue;
-        const MsmShape sh = msm_shape(n, pk->window_bits ? pk->window_bits : pick_window_bits(n), pk->table_windows);
-        if (!batch_fits(sh, k, n))
+      for (int j = 0; j < 4; j++)
+        if (sl.terms[j] && !pk_batch_fits(pk, j, k, sl.terms[j], &nwin))
           return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d on rank %d/%d exceed 2^31",
-                      what, k, sh.nwin, n, j, g, pk->world);
-      }
+                      what, k, nwin, sl.terms[j], j, g, pk->world);
     }
   }
-  const uint64_t N = pow2_at_least(r1->n);
-  if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
+  int rc = qap_batch_check(r1, k, what);
+  if (rc) return rc;
   // the scalar vectors are laid out by 2-D copies whose row pitch (one vector, one witness) the device bounds; the
   // unsharded widths bound every rank's
   int max_pitch = 0;
@@ -955,9 +942,7 @@ int groth16_batch_comm_check(const ProvingKey* pk, const char* what) {
 // builds its domains).  Records no `done` event (groth16_batch_enqueue does, behind what reads the records).
 int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const uint64_t* r, const uint64_t* s,
                         Fq* d_proofs, uint8_t* d_recs, cudaStream_t st, int* err, R1csBatch** fb_used) {
-  const size_t m = pk->m, l1 = pk->npublic + 1, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
-  const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as groth16_witness_enqueue
-  const bool short_z = r1->n >= 2 && pk->Z.nb == r1->n;        // m = n + 1: the same front end, h = (x - n) q + kappa
+  const size_t m = pk->m, l1 = pk->npublic + 1;
   const G16Slices sl = g16_slices(pk, pk->rank);
   size_t woff[3];
   g16_w_layout(pk, sl, woff);
@@ -981,11 +966,7 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
   R1csWork* ws = nullptr;
   R1csBatch* fb = nullptr;
   int rc;
-  if (quotient) {
-    if ((rc = r1cs_work(r1, pk->ctx, &ws))) return rc;
-    if ((h_direct || short_z) && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
-    if (short_z && (rc = r1cs_short_u(r1))) return rc;
-  }
+  if (quotient && (rc = qap_quotient_batch_prepare(r1, pk->Z.nb, pk->ctx, k, &ws, &fb))) return rc;
   *fb_used = fb;
   if ((rc = groth16_batch_scratch(pk, k, false))) return rc;
   for (int j = 0; j < 3; j++) {
@@ -996,14 +977,9 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
     if (rc) return rc;
   }
   if (pk->g[3] && (rc = batch_scratch<Fq>(pk->g[3].get(), (uint32_t)k, (uint32_t)nch))) return rc;
-  for (int j = 0; j < 3; j++) {   // a set that reuses another's sort was sized for the same slices (msm_buckets' check)
-    if (!pk->g[j]) continue;
-    const Bases* a = pk->g[j].get();
-    const Bases* src = pk->g[pk->sort_src[j]].get();
-    if (a->sort.max_slices != src->sort.max_slices || a->affine_S != src->affine_S || a->batch->vecs != src->batch->vecs ||
-        a->batch->sort.sh.n != src->batch->sort.sh.n)
+  for (int j = 0; j < 3; j++)
+    if (pk->g[j] && !batch_shares_sort(pk->g[j].get(), pk->g[pk->sort_src[j]].get()))
       return fail(B200_EINVAL, "groth16_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, pk->sort_src[j]);
-  }
   ProveBatch& b = *pk->batch;
   cudaStream_t s1 = pk->pctx().side[0], s2 = pk->pctx().side[1], s3 = pk->pctx().side[2];
   if (g_serial) s1 = s2 = s3 = st;   // measurement mode (b200_profile bit 1)
@@ -1034,32 +1010,9 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
   // --- side stream 3: the quotients into the C||PTD vectors (h_p[p_lo, p_lo + n_p), zeros beyond len(h), -r_p s_p with
   // the tail), then the C||PTD MSMs
   EV_WAIT(s3, e_in);
-  if (quotient) {
-    PolyCtx& pc = *pk->pctx().poly;
-    Fr* chq = CH + n_c;
-    const uint32_t qtotal = (uint32_t)(k * (n_p + 1));
-    const Fr* tail = sl.tail[3] ? rs + 3 : nullptr;
-    if (h_direct) {
-      if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
-      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)n_p,
-                                                          tail, 4, qtotal, chq, (uint32_t)nch, (uint32_t)sl.p_lo);
-      g_launches += 1;
-    } else if (short_z) {   // the store is part of it
-      if ((rc = qap_h_short_batch_enqueue(r1, *fb, pc, d_w, k, err, s3, chq, nch, n_p, sl.p_lo, tail))) return rc;
-    } else {   // not batched: the single-witness px and division of each witness, into its vector (a shard: its slice)
-      const bool direct = sl.p_lo == 0 && nq <= n_p;
-      const size_t have = nq > sl.p_lo ? std::min(nq - sl.p_lo, n_p) : 0;   // quotient coefficients inside the slice
-      for (size_t p = 0; p < k; p++) {
-        if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
-        CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, direct ? chq + p * nch : pk->h_full.as<Fr>(), nullptr, err, s3));
-        if (!direct && have)
-          CU(cudaMemcpyAsync(chq + p * nch, pk->h_full.as<Fr>() + sl.p_lo, have * F, cudaMemcpyDeviceToDevice, s3));
-      }
-      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)n_p, tail, 4, qtotal, chq,
-                                                          (uint32_t)nch, (uint32_t)sl.p_lo);
-      g_launches += 1;
-    }
-  }
+  if (quotient && (rc = qap_quotient_batch_enqueue(r1, ws, fb, *pk->pctx().poly, pk->Z, pk->h_full.as<Fr>(), d_w, k, CH + n_c, nch,
+                                                   n_p, sl.p_lo, sl.tail[3] ? rs + 3 : nullptr, s3, err)))
+    return rc;
   MsmShape sh;
   if (Bases* gch = pk->g[3].get()) {
     sh = gch->sh;
@@ -1116,6 +1069,16 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
   return B200_OK;
 }
 
+// Behind everything of a batch on `st`: what the next regrowth of any of its scratches waits for (the key's, every set's
+// and the quotient front end's, fb, when the batch used it).
+int batch_done_record(ProvingKey* pk, R1csBatch* fb, cudaStream_t st) {
+  EV_REC(pk->batch->done, st);
+  for (const auto& g : pk->g)
+    if (g && g->batch) EV_REC(g->batch->done, st);
+  if (fb) EV_REC(fb->done, st);
+  return B200_OK;
+}
+
 // The k proofs of a batch at d_out + 48p (u64), or with `records` this rank's k partial records at d_out + 1 KB * p.  A
 // sharded key without `records` computes its records, all-gathers them (k records per rank, on the key's prove-context
 // communicator, on `st`) and finalises: every rank receives the k proofs.  After groth16_batch_check and, without
@@ -1141,13 +1104,7 @@ int groth16_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, con
     CU(cudaGetLastError());
   }
   if (rc) return rc;
-  // behind everything of this batch: what the next regrowth of any of its scratches waits for
-  ProveBatch& b = *pk->batch;
-  EV_REC(b.done, st);
-  for (const auto& g : pk->g)
-    if (g && g->batch) EV_REC(g->batch->done, st);
-  if (fb) EV_REC(fb->done, st);
-  return B200_OK;
+  return batch_done_record(pk, fb, st);
 }
 
 int groth16_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, size_t k, const uint64_t* r,
@@ -1168,17 +1125,7 @@ int groth16_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, 
   else if ((rc = stage_witness(pk, w, pk_needs_px(pk), st, b.w_stage.as<Fr>(), k))) return rc;
   Fq* o = b.out.as<Fq>();
   if ((rc = groth16_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, r, s, o, false, st, pk->d_err_sync.as<int>()))) return rc;
-  // as finish_host_proof, for k proofs: the wait runs with the library mutex released
-  CU(cudaMemcpyAsync(b.h_out, o, k * kBatchProofWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(b.h_out + k * kBatchProofWords));
-  if (rc) return rc;
-  for (size_t p = 0; p < k; p++) {
-    const uint64_t* q = b.h_out + kBatchProofWords * p;
-    memcpy(pi_a + 12 * p, q, 12 * sizeof(uint64_t));
-    memcpy(pi_c + 12 * p, q + 12, 12 * sizeof(uint64_t));
-    memcpy(pi_b + 24 * p, q + 24, 24 * sizeof(uint64_t));
-  }
-  return B200_OK;
+  return finish_host_proof(pk, b.h_out, o, k, what, st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
 }
 
 // ---- witness-fed Pinocchio proving (b200_pinocchio_prove_witness and its _device / _batch twins) ---------------------------
@@ -1189,23 +1136,15 @@ int groth16_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, 
 int pinocchio_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, Fq* d_out, bool record, cudaStream_t st, int* err) {
   const size_t npx = 2 * r1->n - 1;
   if (!pk->g[7]) return pinocchio_enqueue(pk, d_w, nullptr, npx, 0, nullptr, d_out, record, st, err);
-  R1csWork* ws;
-  int rc = r1cs_work(r1, pk->ctx, &ws);
-  if (rc) return rc;
   cudaStream_t sq = g_serial ? st : pk->pctx().side[2];   // measurement mode: the front end on the caller's stream
   if (sq != st) {
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
-  PolyCtx& pc = *pk->pctx().poly;
-  if (r1->n >= 2 && (pk->Z.nb == r1->n + 1 || pk->Z.nb == r1->n)) {   // h-direct, as groth16_witness_enqueue
-    if (pk->Z.nb == r1->n + 1) rc = qap_h_enqueue(r1, *ws, pc, d_w, err, sq);
-    else rc = qap_h_short_enqueue(r1, *ws, pc, d_w, err, sq);
-    if (rc) return rc;
-    return pinocchio_enqueue(pk, d_w, nullptr, npx, 0, ws->h_std.as<Fr>(), d_out, record, st, err);
-  }
-  if ((rc = qap_px_enqueue(r1, *ws, pc, d_w, nullptr, nullptr, err, sq))) return rc;
-  return pinocchio_enqueue(pk, d_w, ws->px_mont.as<Fr>(), npx, /*px_mont=*/1, nullptr, d_out, record, st, err);
+  const Fr *h, *px;   // h itself, or px for pinocchio_enqueue's division
+  int rc = qap_quotient_enqueue(r1, pk->Z.nb, pk->ctx, *pk->pctx().poly, d_w, err, sq, &h, &px);
+  if (rc) return rc;
+  return pinocchio_enqueue(pk, d_w, px, npx, /*px_mont=*/1, h, d_out, record, st, err);
 }
 
 // What every witness-fed Pinocchio entry refuses before anything is allocated or enqueued.
@@ -1232,7 +1171,7 @@ int pinocchio_prove_witness(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size
   CU(cudaMemcpyAsync(dw, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
   Fq* o = pk->out_std.as<Fq>();
   if ((rc = pinocchio_witness_enqueue(pk, r1, dw, o, false, st, pk->d_err_sync.as<int>()))) return rc;
-  return finish_host_proof(pk, o, what, st, lk, {{out_g1, 84}, {pi_b, 24}});
+  return finish_host_proof(pk, pk->h_out, o, 1, what, st, lk, {{out_g1, 84}, {pi_b, 24}});
 }
 
 // ---- batches: k witness-fed Pinocchio proofs under one key (b200_pinocchio_prove_witness_batch) -------------------------
@@ -1253,21 +1192,12 @@ int pinocchio_batch_check(const ProvingKey* pk, const R1cs* r1, size_t nw, size_
   if (rc) return rc;
   const size_t ma = pk->m - pk->npublic - 1;
   const size_t terms[8] = {ma, ma, pk->m, pk->m, pk->m, pk->m, pk->m, pk->n_h_bases};
-  for (int j = 0; j < 8; j++) {
-    if (pk->world == 1) {
-      if (pk->g[j] && !batch_fits(pk->g[j].get(), k, terms[j]))
-        return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
-                    pk->g[j]->sh.nwin, terms[j], j);
-    } else if (terms[j]) {
-      const MsmShape sh = msm_shape(terms[j], pk->window_bits ? pk->window_bits : pick_window_bits(terms[j]), pk->table_windows);
-      if (!batch_fits(sh, k, terms[j]))
-        return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
-                    sh.nwin, terms[j], j);
-    }
-  }
-  const uint64_t N = pow2_at_least(r1->n);
-  if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
-  return B200_OK;
+  uint32_t nwin;
+  for (int j = 0; j < 8; j++)
+    if ((pk->world == 1 ? pk->g[j] != nullptr : terms[j] != 0) && !pk_batch_fits(pk, j, k, terms[j], &nwin))
+      return fail(B200_EINVAL, "%s: k * nwin * terms = %zu * %u * %zu sort entries (or the buckets) of set %d exceed 2^31", what, k,
+                  nwin, terms[j], j);
+  return qap_batch_check(r1, k, what);
 }
 
 // The entries that return proofs: a sharded key needs its communicator (checked before anything is enqueued).
@@ -1286,9 +1216,7 @@ int pinocchio_batch_comm_check(const ProvingKey* pk, const char* what) {
 // builds its domains).  Records no `done` event (pinocchio_batch_enqueue does, behind what reads the records).
 int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq* d_out, uint8_t* d_recs, cudaStream_t st,
                           int* err, R1csBatch** fb_used) {
-  const size_t m = pk->m, l1 = pk->npublic + 1, ng = pk->n_h_bases, npx = 2 * r1->n - 1, nq = npx - pk->Z.nb + 1;
-  const bool h_direct = r1->n >= 2 && pk->Z.nb == r1->n + 1;   // as pinocchio_witness_enqueue
-  const bool short_z = r1->n >= 2 && pk->Z.nb == r1->n;
+  const size_t m = pk->m, l1 = pk->npublic + 1, ng = pk->n_h_bases;
   const size_t terms[8] = {m - l1, m - l1, m, m, m, m, m, ng};
   // the set that sorts for set j: the first set of j's group (kPinSortSrc) this key holds
   int src[8];
@@ -1301,11 +1229,7 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
   R1csWork* ws = nullptr;
   R1csBatch* fb = nullptr;
   int rc;
-  if (pk->g[7]) {
-    if ((rc = r1cs_work(r1, pk->ctx, &ws))) return rc;
-    if ((h_direct || short_z) && (rc = qap_batch_prepare(r1, *ws, k, &fb))) return rc;
-    if (short_z && (rc = r1cs_short_u(r1))) return rc;
-  }
+  if (pk->g[7] && (rc = qap_quotient_batch_prepare(r1, pk->Z.nb, pk->ctx, k, &ws, &fb))) return rc;
   *fb_used = fb;
   if ((rc = pinocchio_batch_scratch(pk, k, false))) return rc;
   for (int j = 0; j < 8; j++) {
@@ -1315,15 +1239,9 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
                 : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own);
     if (rc) return rc;
   }
-  for (int j = 0; j < 8; j++) {   // a set that reuses another's sort was sized for the same slices (msm_buckets' check)
-    if (!pk->g[j]) continue;
-    const Bases* a = pk->g[j].get();
-    const Bases* sb = pk->g[src[j]].get();
-    if (a->sh.c != sb->sh.c || a->sh.table_stride != sb->sh.table_stride || a->sh.rows != sb->sh.rows ||
-        a->sort.max_slices != sb->sort.max_slices || a->affine_S != sb->affine_S || a->batch->vecs != sb->batch->vecs ||
-        a->batch->sort.sh.n != sb->batch->sort.sh.n)
+  for (int j = 0; j < 8; j++)
+    if (pk->g[j] && !batch_shares_sort(pk->g[j].get(), pk->g[src[j]].get()))
       return fail(B200_EINVAL, "pinocchio_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, src[j]);
-  }
   ProveBatch& b = *pk->batch;
   cudaStream_t side[3] = {pk->pctx().side[0], pk->pctx().side[1], pk->pctx().side[2]};
   if (g_serial) side[0] = side[1] = side[2] = st;   // measurement mode (b200_profile bit 1)
@@ -1352,24 +1270,9 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
   cudaStream_t s3 = side[2];
   if (pk->g[7]) {
     if (s3 != st) EV_WAIT(s3, e_in);
-    PolyCtx& pc = *pk->pctx().poly;
-    Fr* H = b.CH.as<Fr>();
-    const uint32_t qtotal = (uint32_t)(k * (ng + 1));
-    if (h_direct) {
-      if ((rc = qap_h_batch_enqueue(r1, *fb, pc, d_w, k, err, s3))) return rc;
-      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(fb->hw.coef.as<Fr>(), (uint32_t)r1->hd->tree.N, (uint32_t)nq, (uint32_t)ng,
-                                                          nullptr, 0, qtotal, H, (uint32_t)ng);
-      g_launches += 1;
-    } else if (short_z) {   // the store is part of it
-      if ((rc = qap_h_short_batch_enqueue(r1, *fb, pc, d_w, k, err, s3, H, ng, ng, 0, nullptr))) return rc;
-    } else {   // not batched: the single-witness px and division of each witness, straight into its vector
-      for (size_t p = 0; p < k; p++) {
-        if ((rc = qap_px_enqueue(r1, *ws, pc, d_w + p * m, nullptr, nullptr, err, s3))) return rc;
-        CU(poly_div_device(pc, pk->Z, ws->px_mont.as<Fr>(), npx, 1, H + p * ng, nullptr, err, s3));
-      }
-      k_quotient_store<<<nblk(qtotal, 256), 256, 0, s3>>>(nullptr, 0, (uint32_t)nq, (uint32_t)ng, nullptr, 0, qtotal, H, (uint32_t)ng);
-      g_launches += 1;
-    }
+    Fr* H = b.CH.as<Fr>();   // len(h) <= len(G1T) (pinocchio_check_px): every quotient is divided straight into its vector
+    if ((rc = qap_quotient_batch_enqueue(r1, ws, fb, *pk->pctx().poly, pk->Z, nullptr, d_w, k, H, ng, ng, 0, nullptr, s3, err)))
+      return rc;
     if ((rc = sort_of(7, H, ng, s3))) return rc;
     if ((rc = buckets_of(7, s3))) return rc;
   }
@@ -1441,13 +1344,7 @@ int pinocchio_batch_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, F
     CU(cudaGetLastError());
   }
   if (rc) return rc;
-  // behind everything of this batch: what the next regrowth of any of its scratches waits for
-  ProveBatch& b = *pk->batch;
-  EV_REC(b.done, st);
-  for (const auto& g : pk->g)
-    if (g && g->batch) EV_REC(g->batch->done, st);
-  if (fb) EV_REC(fb->done, st);
-  return B200_OK;
+  return batch_done_record(pk, fb, st);
 }
 
 int pinocchio_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w, size_t nw, size_t k, uint64_t* out_g1,
@@ -1466,16 +1363,7 @@ int pinocchio_prove_witness_batch(b200_pk_t h, b200_r1cs_t hr, const uint64_t* w
   CU(cudaMemcpyAsync(b.w_stage.p, w, k * nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
   Fq* o = b.out.as<Fq>();
   if ((rc = pinocchio_batch_enqueue(pk, r1, b.w_stage.as<Fr>(), k, o, false, st, pk->d_err_sync.as<int>()))) return rc;
-  // as finish_host_proof, for k proofs: the wait runs with the library mutex released
-  CU(cudaMemcpyAsync(b.h_out, o, k * kHostProofWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(b.h_out + k * kHostProofWords));
-  if (rc) return rc;
-  for (size_t p = 0; p < k; p++) {
-    const uint64_t* q = b.h_out + kHostProofWords * p;
-    memcpy(out_g1 + 84 * p, q, 84 * sizeof(uint64_t));
-    memcpy(pi_b + 24 * p, q + 84, 24 * sizeof(uint64_t));
-  }
-  return B200_OK;
+  return finish_host_proof(pk, b.h_out, o, k, what, st, lk, {{out_g1, 84}, {pi_b, 24}});
 }
 
 // ---- dense QAP API (small n) -------------------------------------------------

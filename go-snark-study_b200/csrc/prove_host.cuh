@@ -368,10 +368,12 @@ size_t g16_w_layout(const ProvingKey* pk, const G16Slices& sl, size_t woff[3]) {
   return total;
 }
 
-// Grows the key's batch scratch to k proofs (host: also the host entry's witness staging, proof buffer and pinned landing
-// area).  A regrowth first waits for the key's last batch (its `done` event), not for the device.  A sharded key's
-// vectors are those of its own part (G16Slices), and it keeps k partial records for the all-gather.
-int groth16_batch_scratch(ProvingKey* pk, size_t k, bool host) {
+// The key's batch scratch for k proofs of `words` u64 each, created on the first batch.  Before anything of it grows the
+// host waits for the key's last batch (its `done` event), not for the device.  grow_device(b) reallocates the protocol's
+// device buffers for k proofs when k exceeds their capacity; with `host`, the host entry's witness staging, proof buffer
+// and pinned landing area (the k proofs + the error word) grow too.
+template <class GrowDevice>
+int prove_batch_scratch(ProvingKey* pk, size_t k, bool host, size_t words, GrowDevice grow_device) {
   if (!pk->batch) {
     auto b = std::make_unique<ProveBatch>();
     for (auto& e : b->ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -379,29 +381,59 @@ int groth16_batch_scratch(ProvingKey* pk, size_t k, bool host) {
     pk->batch = std::move(b);
   }
   ProveBatch& b = *pk->batch;
-  const size_t m = pk->m;
+  const bool grow_host = host && b.out.bytes < k * words * sizeof(uint64_t);
+  if (b.k < k || grow_host) CU(cudaEventSynchronize(b.done));
+  if (b.k < k) {
+    int rc = grow_device(b);
+    if (rc) return rc;
+    b.k = k;
+  }
+  if (grow_host) {
+    CU(b.w_stage.alloc(k * pk->m * sizeof(Fr)));
+    CU(b.out.alloc(k * words * sizeof(uint64_t)));
+    if (b.h_out) CU(cudaFreeHost(b.h_out));
+    b.h_out = nullptr;
+    CU(cudaHostAlloc(reinterpret_cast<void**>(&b.h_out), (k * words + 1) * sizeof(uint64_t), cudaHostAllocDefault));
+  }
+  return B200_OK;
+}
+
+// Grows the key's batch scratch to k proofs (prove_batch_scratch).  A sharded key's vectors are those of its own part
+// (G16Slices), and it keeps k partial records for the all-gather.
+int groth16_batch_scratch(ProvingKey* pk, size_t k, bool host) {
   const G16Slices sl = g16_slices(pk, pk->rank);
   size_t woff[3];
   const size_t nw = g16_w_layout(pk, sl, woff), nch = pk->g[3] ? sl.terms[3] : 0;
-  const bool grow_host = host && b.out.bytes < k * kBatchProofWords * sizeof(uint64_t);
-  if (b.k < k || grow_host) CU(cudaEventSynchronize(b.done));
-  if (b.k < k) {
+  return prove_batch_scratch(pk, k, host, kBatchProofWords, [&](ProveBatch& b) -> int {
     CU(b.W.alloc(k * nw * sizeof(Fr)));
     CU(b.CH.alloc(k * nch * sizeof(Fr)));
     CU(b.rec.alloc(k * (5 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>))));
     CU(b.rs.alloc(k * 4 * sizeof(Fr)));
     CU(b.glv.alloc(k * sizeof(GlvScalars)));
     if (pk->world > 1) CU(b.parts.alloc(k * kPartialBytes));
-    b.k = k;
+    return B200_OK;
+  });
+}
+
+// A set whose batches reuse set src's digit sort was sized for the same slices and windows (msm_buckets' check).  On a
+// Groth16 key c, table_stride and rows agree by construction: sort_src pairs only sets of equal slices and rows.
+bool batch_shares_sort(const Bases* a, const Bases* src) {
+  return a->sh.c == src->sh.c && a->sh.table_stride == src->sh.table_stride && a->sh.rows == src->sh.rows &&
+         a->sort.max_slices == src->sort.max_slices && a->affine_S == src->affine_S && a->batch->vecs == src->batch->vecs &&
+         a->batch->sort.sh.n == src->batch->sort.sh.n;
+}
+
+// Whether a batch of k vectors of n terms fits set j as its rank built it: on one GPU the set's own shape (a set the key
+// lacks fits nothing, *nwin = 0), on a shard msm_shape with the key's window bits and table rows, so that every rank
+// decides alike.  *nwin: the shape's windows.
+bool pk_batch_fits(const ProvingKey* pk, int j, size_t k, size_t n, uint32_t* nwin) {
+  if (pk->world == 1 && !pk->g[j]) {
+    *nwin = 0;
+    return false;
   }
-  if (grow_host) {
-    CU(b.w_stage.alloc(k * m * sizeof(Fr)));
-    CU(b.out.alloc(k * kBatchProofWords * sizeof(uint64_t)));
-    if (b.h_out) CU(cudaFreeHost(b.h_out));
-    b.h_out = nullptr;
-    CU(cudaHostAlloc(reinterpret_cast<void**>(&b.h_out), (k * kBatchProofWords + 1) * sizeof(uint64_t), cudaHostAllocDefault));
-  }
-  return B200_OK;
+  const MsmShape sh = pk->world == 1 ? pk->g[j]->sh : msm_shape(n, pk->window_bits ? pk->window_bits : pick_window_bits(n), pk->table_windows);
+  *nwin = sh.nwin;
+  return batch_fits(sh, k, n);
 }
 
 // host F_r helpers for the blinding scalars (the reference does this with big.Int, groth16.go:274)
@@ -655,21 +687,23 @@ int stage_witness(ProvingKey* pk, const uint64_t* w, bool all, cudaStream_t st, 
   return B200_OK;
 }
 
-// Copy the proof out to the key's pinned landing area, read the key's d_err_sync behind it and wait (with `lk`: the wait
-// runs with the library mutex released), then split the proof into the caller's arrays: `outs` lists each array and its
-// word count, in the order of the device layout.
-int finish_host_proof(ProvingKey* pk, const Fq* d_proof, const char* what, cudaStream_t st, std::unique_lock<std::mutex>* lk,
-                      std::initializer_list<std::pair<uint64_t*, size_t>> outs) {
+// Copy k proofs out to the pinned landing area h_out (the key's, or its batch scratch's), read the key's d_err_sync
+// behind them into the word after the k proofs and wait (with `lk`: the wait runs with the library mutex released), then
+// split each proof into the caller's arrays: `outs` lists each array and its words per proof, in the order of the device
+// layout; proof p's part lands at array + p * words.
+int finish_host_proof(ProvingKey* pk, uint64_t* h_out, const Fq* d_proof, size_t k, const char* what, cudaStream_t st,
+                      std::unique_lock<std::mutex>* lk, std::initializer_list<std::pair<uint64_t*, size_t>> outs) {
   size_t words = 0;
   for (const auto& o : outs) words += o.second;
-  uint64_t* host_out = pk->h_out;
-  CU(cudaMemcpyAsync(host_out, d_proof, words * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  int rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(host_out + kHostProofWords));
+  CU(cudaMemcpyAsync(h_out, d_proof, k * words * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  int rc = check_err_flag(what, pk->d_err_sync.as<int>(), st, lk, reinterpret_cast<int*>(h_out + k * words));
   if (rc) return rc;
-  for (const auto& o : outs) {
-    memcpy(o.first, host_out, o.second * sizeof(uint64_t));
-    host_out += o.second;
-  }
+  const uint64_t* q = h_out;
+  for (size_t p = 0; p < k; p++)
+    for (const auto& o : outs) {
+      memcpy(o.first + p * o.second, q, o.second * sizeof(uint64_t));
+      q += o.second;
+    }
   return B200_OK;
 }
 
@@ -701,7 +735,7 @@ int groth16_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* px,
   Fq* o = pk->out_std.as<Fq>();
   rc = groth16_enqueue(pk, pk->w_stage.as<Fr>(), nw, pk->px.as<Fr>(), npx, r, s, o, st, pk->d_err_sync.as<int>());
   if (rc) return rc;
-  return finish_host_proof(pk, o, "groth16_prove", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
+  return finish_host_proof(pk, pk->h_out, o, 1, "groth16_prove", st, lk, {{pi_a, 12}, {pi_c, 12}, {pi_b, 24}});
 }
 
 // Pinocchio result slots (XYZZ, 256 B each): 0 PiA, 1 PiAp, 2 PiBp, 3 PiC, 4 PiCp, 5 PiH, 6 PiKp, 7 PiB (G2).
@@ -886,35 +920,18 @@ int pinocchio_prove(b200_pk_t h, const uint64_t* w, size_t nw, const uint64_t* p
   }
   Fq* o = pk->out_std.as<Fq>();
   if ((rc = pinocchio_enqueue(pk, dw, pk->px.as<Fr>(), npx, 0, nullptr, o, false, st, err))) return rc;
-  return finish_host_proof(pk, o, "pinocchio_prove", st, nullptr, {{out_g1, 84}, {pi_b, 24}});
+  return finish_host_proof(pk, pk->h_out, o, 1, "pinocchio_prove", st, nullptr, {{out_g1, 84}, {pi_b, 24}});
 }
 
-// Grows a Pinocchio key's batch scratch to k proofs (host: also the host entry's witness staging, proof buffer and pinned
-// landing area), as groth16_batch_scratch does for a Groth16 key.
+// Grows a Pinocchio key's batch scratch to k proofs (prove_batch_scratch): the quotient vectors, the records and, on a
+// shard, the k records for the all-gather.
 int pinocchio_batch_scratch(ProvingKey* pk, size_t k, bool host) {
-  if (!pk->batch) {
-    auto b = std::make_unique<ProveBatch>();
-    for (auto& e : b->ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
-    pk->batch = std::move(b);
-  }
-  ProveBatch& b = *pk->batch;
-  const bool grow_host = host && b.out.bytes < k * kHostProofWords * sizeof(uint64_t);
-  if (b.k < k || grow_host) CU(cudaEventSynchronize(b.done));
-  if (b.k < k) {
+  return prove_batch_scratch(pk, k, host, kHostProofWords, [&](ProveBatch& b) -> int {
     CU(b.CH.alloc(k * pk->n_h_bases * sizeof(Fr)));
     CU(b.rec.alloc(k * (7 * sizeof(XYZZ<Fq>) + sizeof(XYZZ<Fq2>))));
     if (pk->world > 1) CU(b.parts.alloc(k * kPinRecordBytes));
-    b.k = k;
-  }
-  if (grow_host) {
-    CU(b.w_stage.alloc(k * pk->m * sizeof(Fr)));
-    CU(b.out.alloc(k * kHostProofWords * sizeof(uint64_t)));
-    if (b.h_out) CU(cudaFreeHost(b.h_out));
-    b.h_out = nullptr;
-    CU(cudaHostAlloc(reinterpret_cast<void**>(&b.h_out), (k * kHostProofWords + 1) * sizeof(uint64_t), cudaHostAllocDefault));
-  }
-  return B200_OK;
+    return B200_OK;
+  });
 }
 
 // one-GPU emulation of the collective: sum `world` gathered records (device) -> the proof (host)

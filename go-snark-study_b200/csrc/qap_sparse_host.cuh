@@ -394,6 +394,89 @@ int qap_h_short_batch_enqueue(R1cs* r, R1csBatch& b, PolyCtx& pc, const Fr* d_w,
   return qap_short_store(r, b.hw.coef.as<Fr>(), r->hd->tree.N, b.coef.as<Fr>(), b.part.as<Fr>(), k, vec, stride, n_ptd, off, tail, st);
 }
 
+// ---- the witness-fed quotient h = (ax*bx - cx) / Z, whichever Z the key has ------------------------------------------
+// The shapes whose proofs can verify have Z = prod_{i<=n}(x - i) (m = n + 2, SURVEY H5: h straight from the rows' values)
+// or Z = prod_{i<n}(x - i) (m = n + 1: the same front end, h = (x - n) q + kappa); both need n >= 2.  Any other Z goes
+// through px and the key's division, one witness at a time.  The only place that compares len(Z) with n.
+enum class QapForm { HDirect, ShortZ, PxDivision };
+QapForm qap_form(const R1cs* r, size_t nz) {
+  if (r->n >= 2 && nz == r->n + 1) return QapForm::HDirect;
+  if (r->n >= 2 && nz == r->n) return QapForm::ShortZ;
+  return QapForm::PxDivision;
+}
+
+// One witness's quotient on `st`, in the workspace of prove context ctx: either *h_std (the standard-form h) or *px_mont
+// (the Montgomery px, for the caller's division by Z) is set, the other null.
+int qap_quotient_enqueue(R1cs* r, size_t nz, int ctx, PolyCtx& pc, const Fr* d_w, int* err, cudaStream_t st,
+                         const Fr** h_std, const Fr** px_mont) {
+  *h_std = *px_mont = nullptr;
+  R1csWork* ws;
+  int rc = r1cs_work(r, ctx, &ws);
+  if (rc) return rc;
+  switch (qap_form(r, nz)) {
+    case QapForm::HDirect: rc = qap_h_enqueue(r, *ws, pc, d_w, err, st); break;
+    case QapForm::ShortZ: rc = qap_h_short_enqueue(r, *ws, pc, d_w, err, st); break;
+    case QapForm::PxDivision:
+      if ((rc = qap_px_enqueue(r, *ws, pc, d_w, nullptr, nullptr, err, st))) return rc;
+      *px_mont = ws->px_mont.as<Fr>();
+      return B200_OK;
+  }
+  if (rc) return rc;
+  *h_std = ws->h_std.as<Fr>();
+  return B200_OK;
+}
+
+// Before a batch of k witnesses: every scratch of its quotients (the workspace of prove context ctx; the batch scratch
+// of the batched forms; u for len(Z) = n), so that enqueueing the batch allocates nothing.  *fb: the batch scratch, or
+// null (px-division), whose `done` the caller records behind the batch.
+int qap_quotient_batch_prepare(R1cs* r, size_t nz, int ctx, size_t k, R1csWork** ws, R1csBatch** fb) {
+  *fb = nullptr;
+  int rc = r1cs_work(r, ctx, ws);
+  if (rc) return rc;
+  const QapForm f = qap_form(r, nz);
+  if (f != QapForm::PxDivision && (rc = qap_batch_prepare(r, **ws, k, fb))) return rc;
+  return f == QapForm::ShortZ ? r1cs_short_u(r) : B200_OK;
+}
+
+// A batch of k witnesses stays inside 32-bit transform indexing: 3k * 2N < 2^32 (N = the power of two >= n).
+int qap_batch_check(const R1cs* r, size_t k, const char* what) {
+  const uint64_t N = pow2_at_least(r->n);
+  if (6 * (uint64_t)k * N >= (1ull << 32)) return fail(B200_EINVAL, "%s: 3k * 2N = 3 * %zu * %llu transform elements exceed 2^32", what, k, (unsigned long long)(2 * N));
+  return B200_OK;
+}
+
+// d_w: k witnesses (standard form, witness p at d_w + p*m) -> coefficients [off, off + n_ptd) of each quotient h_p by Z
+// into the vectors at vec + p * stride, standard form, zeros beyond len(h), then tail[4p] when given.  After
+// qap_quotient_batch_prepare for >= k with the same ws and fb.  px-division: each witness's px is divided straight into
+// its vector when the slice is all of h from h[0], else into `scratch` (>= len(h) coefficients) and the slice copied out.
+int qap_quotient_batch_enqueue(R1cs* r, R1csWork* ws, R1csBatch* fb, PolyCtx& pc, Divisor& Z, Fr* scratch,
+                               const Fr* d_w, size_t k, Fr* vec, size_t stride, size_t n_ptd, size_t off, const Fr* tail,
+                               cudaStream_t st, int* err) {
+  const size_t npx = 2 * r->n - 1, nq = npx - Z.nb + 1;
+  const QapForm f = qap_form(r, Z.nb);
+  int rc;
+  if (f == QapForm::ShortZ)   // the store is part of it
+    return qap_h_short_batch_enqueue(r, *fb, pc, d_w, k, err, st, vec, stride, n_ptd, off, tail);
+  const Fr* q = nullptr;   // px-division: the quotients are already in place, the store only zero-fills and adds the tail
+  if (f == QapForm::HDirect) {
+    if ((rc = qap_h_batch_enqueue(r, *fb, pc, d_w, k, err, st))) return rc;
+    q = fb->hw.coef.as<Fr>();
+  } else {
+    const bool direct = off == 0 && nq <= n_ptd;
+    const size_t have = nq > off ? std::min(nq - off, n_ptd) : 0;   // quotient coefficients inside the slice
+    for (size_t p = 0; p < k; p++) {
+      if ((rc = qap_px_enqueue(r, *ws, pc, d_w + p * r->m, nullptr, nullptr, err, st))) return rc;
+      CU(poly_div_device(pc, Z, ws->px_mont.as<Fr>(), npx, 1, direct ? vec + p * stride : scratch, nullptr, err, st));
+      if (!direct && have) CU(cudaMemcpyAsync(vec + p * stride, scratch + off, have * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  const uint32_t qtotal = (uint32_t)(k * (n_ptd + 1));
+  k_quotient_store<<<nblk(qtotal, 256), 256, 0, st>>>(q, q ? (uint32_t)r->hd->tree.N : 0, (uint32_t)nq, (uint32_t)n_ptd, tail, 4,
+                                                      qtotal, vec, (uint32_t)stride, (uint32_t)off);
+  g_launches += 1;
+  return B200_OK;
+}
+
 // Enqueues at | bt | ct (Montgomery, m each) into d_out on `st`; *zt = prod_{i=1..nz}(tau - i) (Montgomery).  t: tau in
 // Montgomery form.  tau in 1..n sets bit 4 of g_d_err.
 int qap_eval_at_enqueue(R1cs* r, Fr t, size_t nz, Fr* d_out, Fr* zt, cudaStream_t st) {

@@ -189,7 +189,7 @@ def go_verify(g, proof):
 @pytest.mark.parametrize("name", ["x3x5", "chain21", "mul"])
 def test_go_binary_circuits(L, golden_dir, name):
     """The Go binary's circuits: the witness-fed proof equals the binary's proofs.json, and the binary verifies it.  x3x5
-    and chain21 (len(Z) = n) take px and the key's division on the device, mul the h-direct quotient."""
+    and chain21 (len(Z) = n) take the short-Z quotient on the device, mul the h-direct one."""
     from gosnark_b200 import snark
     from gosnark_b200._lib import ints_to_limbs
     from gosnark_b200.bn128 import reduce_scalar

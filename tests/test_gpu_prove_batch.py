@@ -392,7 +392,7 @@ def groth_vk(setup):
 def test_golden_circuits(L, golden_dir, name):
     """The Go binary's circuits, the golden witness in a batch of three with other (r, s): each proof equals
     b200_groth16_prove with the golden px for its (r, s) and verifies under the golden Vk.  x3x5 and chain21 (len(Z) = n)
-    take the px branch, mul the h-direct one."""
+    take the short-Z quotient, mul the h-direct one."""
     from gosnark_b200 import groth16
     from gosnark_b200._lib import ints_to_limbs
     from gosnark_b200.bn128 import reduce_scalar

@@ -157,7 +157,7 @@ def _groth_vk(setup):
 @pytest.mark.parametrize("name", ["x3x5", "chain21", "mul"])
 def test_golden_circuits(L, golden_dir, name):
     """The Go binary's circuits: x3x5 and chain21 have m = n + 1 and len(Z) = n, so the witness entries take the
-    px-then-divide branch (mul, len(Z) = n + 1, the h-direct one).  The device witness entry, the host witness entry
+    short-Z quotient (mul, len(Z) = n + 1, the h-direct one).  The device witness entry, the host witness entry
     (DeviceProvingKey.prove_witness_limbs) and b200_groth16_prove with the golden px give the same proof for the same
     r, s, and it verifies under the golden Vk."""
     import torch
