@@ -18,6 +18,7 @@
 #include "msm.cuh"
 #include "bucket_affine.cuh"
 #include "poly_host.cuh"
+#include "msm_host.cuh"
 #include "qap.cuh"
 #include "qap_sparse.cuh"
 #include "fixed_base.cuh"
@@ -158,134 +159,60 @@ int init_locked(int device) {
   return B200_OK;
 }
 
-inline unsigned nblocks(size_t n, unsigned bs) { return nblk(n, bs); }
-
-int pick_window_bits(size_t n) {
-  // cost model: nwin*n bucket adds (~10 M) + 2*2^(c-1) reduction adds (~14 M), see DESIGN.md §3
-  int best = 8;
-  double best_cost = 1e300;
-  for (int c = 8; c <= 18; c++) {
-    double nwin = (255 + c - 1) / c;
-    double cost = nwin * (double)n * 10.0 + 2.0 * (double)(1u << (c - 1)) * 14.0 * 4.0;
-    if (cost < best_cost) { best_cost = cost; best = c; }
+// ---- the MSM engine (msm_host.cuh) under the library's settings.  msm_env() is filled from the globals at every call,
+// so that b200_config (B200_CFG_TMA_STAGING) and b200_profile take effect on the next MSM.  The wrappers below keep the
+// argument checks and their messages, and map the engine's cudaError_t to B200 codes.
+ProfRec g_prof_open{};   // the accumulation being timed (one at a time: the library mutex is held)
+void prof_begin(int group, size_t terms, cudaStream_t st) {
+  g_prof_open = ProfRec{prof_event(), prof_event(), group, terms};
+  cudaEventRecord(g_prof_open.e0, st);
+}
+void prof_end(cudaStream_t st) {
+  cudaEventRecord(g_prof_open.e1, st);
+  g_prof_recs.push_back(g_prof_open);
+}
+MsmEnv msm_env() {
+  MsmEnv env;
+  env.launch_counter = &g_launches;
+  env.tma_staging = g_tma_staging;
+  if (g_prof) {
+    env.prof_begin = prof_begin;
+    env.prof_end = prof_end;
   }
-  return best;
+  return env;
 }
 
-// Records of launch_bucket_tail's scratch: H rows, K columns and c planes per window group of every scalar vector.
-size_t bucket_tail_records(const MsmShape& sh) {
-  const uint32_t bits = sh.c - 1, kl = (bits + 1) / 2, kh = bits - kl;
-  return (size_t)sh.vecs * sh.groups * ((1u << kh) + (1u << kl) + bits + 1);
-}
-
-// Output of the digit-recode / counting-sort front end for one scalar vector.  It depends only on the
-// scalars and the window shape, so base sets that consume the SAME scalars (A, B1, B2 of a Groth16
-// proof) share one SortScratch read-only.
-struct SortScratch {
-  MsmShape sh{};            // shape it was allocated for (n = capacity)
-  DevBuf counts, offsets, cursor, entries, slice_off, slice_start, slice_end;
-  uint32_t max_slices = 0;
-  uint32_t slice_S = 0;     // > 0: fixed-size slices of S slots (batched-affine mode)
-  SliceTables tables() const { return SliceTables{slice_off.as<uint32_t>(), slice_start.as<uint32_t>(), slice_end.as<uint32_t>()}; }
-};
-
-// Scratch of the bucket phase: slice sums, buckets, tail records and, for batched-affine accumulation (affine_S > 0),
-// ping-pong node buffers, prefix products and per-thread / per-block products.
-struct BucketScratch {
-  DevBuf slice_out, buckets, partials;
-  DevBuf nodeA, nodeB, aff_pre, aff_others, aff_btot, aff_ids;
-};
-
-// Front-end and bucket scratch of b200_msm_device_batch on one base set, sized for `vecs` scalar vectors of the set's
-// full size.  Allocated on the set's first batch and grown (never shrunk) when a later batch has more vectors.
-struct MsmBatch {
-  uint32_t vecs = 0;
-  SortScratch sort;
-  BucketScratch bk;
-  DevBuf scan_totals;   // per-block totals of the multi-block counter scan
-  cudaEvent_t done = nullptr;   // recorded behind the last batch on the set: a regrowth waits for it, not for the device
-  MsmBatch() = default;
-  MsmBatch(const MsmBatch&) = delete;
-  MsmBatch& operator=(const MsmBatch&) = delete;
-  ~MsmBatch() { if (done) cudaEventDestroy(done); }
-};
-constexpr uint32_t kScanBlocks = 1024;   // upper bound on the blocks of a batch's counter scan
-
-struct Bases {
-  int group = 0;  // 1: G1 (Fq), 2: G2 (Fq2)
-  size_t n = 0;
-  MsmShape sh{};
-  DevBuf table;    // [nwin][n] Affine<F>
-  // per-base-set scratch of the bucket phase (different base sets may run concurrently)
-  DevBuf scalars;  // n * 32 B (host-scalar entry points)
-  BucketScratch bk;
-  DevBuf result, out_std;
-  SortScratch sort;  // own front-end scratch (stand-alone MSMs)
-  uint32_t nseg = 0, seg = 0;
-  uint32_t affine_S = 0;   // > 0: batched-affine accumulation with slices of affine_S entries
-  std::unique_ptr<MsmBatch> batch;   // b200_msm_device_batch scratch (null until the first batch)
-  // error word of b200_msm_device on this set: written by the kernels, never read (the call cannot wait for it, and a
-  // later call on any object must not report it; see b200snark.h).  Host-pointer MSMs use g_d_err.
-  DevBuf d_err;
-};
-
-// Device memory held by the buffers (b200_bases_device_bytes / b200_pk_device_bytes).
-size_t dev_bytes(std::initializer_list<const DevBuf*> bufs) {
-  size_t s = 0;
-  for (const DevBuf* d : bufs) s += d->p ? d->bytes : 0;
-  return s;
-}
-size_t scratch_device_bytes(const SortScratch& ss, const BucketScratch& bk) {
-  return dev_bytes({&ss.counts, &ss.offsets, &ss.cursor, &ss.entries, &ss.slice_off, &ss.slice_start, &ss.slice_end,
-                    &bk.slice_out, &bk.buckets, &bk.partials, &bk.nodeA, &bk.nodeB, &bk.aff_pre, &bk.aff_others,
-                    &bk.aff_btot, &bk.aff_ids});
-}
-size_t bases_device_bytes(const Bases& b) {
-  size_t s = dev_bytes({&b.table, &b.scalars, &b.result, &b.out_std, &b.d_err}) + scratch_device_bytes(b.sort, b.bk);
-  if (b.batch) s += scratch_device_bytes(b.batch->sort, b.batch->bk) + dev_bytes({&b.batch->scan_totals});
-  return s;
-}
-
-// slices: every bucket owns >= 1; a bucket above cap = 2*mean entries is cut => at most B + B/2 + 1
-uint32_t sort_max_slices(const MsmShape& sh, uint32_t slice_S) {
-  const size_t entries = (size_t)sh.vecs * sh.nwin * sh.n;
-  const uint32_t B = total_buckets(sh);
-  return slice_S ? B + (uint32_t)((entries + slice_S - 1) / slice_S) + 2 : B + B / 2 + 2;
-}
-
-int sort_alloc(SortScratch& ss, const MsmShape& sh, uint32_t slice_S) {
-  ss.sh = sh;
-  ss.slice_S = slice_S;
-  size_t entries = (size_t)sh.vecs * sh.nwin * sh.n;
-  const uint32_t B = total_buckets(sh);
-  CU(ss.counts.alloc((B + 2) * sizeof(uint32_t)));
-  CU(ss.offsets.alloc((B + 3) * sizeof(uint32_t)));
-  CU(ss.cursor.alloc((B + 2) * sizeof(uint32_t)));
-  CU(ss.entries.alloc(entries * sizeof(uint32_t)));
-  ss.max_slices = sort_max_slices(sh, slice_S);
-  CU(ss.slice_off.alloc((B + 3) * sizeof(uint32_t)));
-  CU(ss.slice_start.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
-  CU(ss.slice_end.alloc((size_t)ss.max_slices * sizeof(uint32_t)));
+int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, int* err, cudaStream_t st,
+             unsigned long long* scan_totals = nullptr) {
+  if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride || shape.rows != ss.sh.rows ||
+      shape.vecs > ss.sh.vecs)
+    return fail(B200_EINVAL, "msm_sort: shape mismatch");
+  CU(b200::msm_sort(msm_env(), ss, shape, d_scalars, n, mont, err, st, scan_totals));
   return B200_OK;
 }
 
-// Bucket scratch for the shape `sh` (its vecs included) over a sort scratch of max_slices slices: affine_S > 0 adds the
-// batched-affine buffers; nseg: segments per window group of the c < 7 tail.
 template <class F>
-int bucket_alloc(BucketScratch& bk, const MsmShape& sh, uint32_t max_slices, uint32_t affine_S, uint32_t nseg) {
-  CU(bk.buckets.alloc((size_t)total_buckets(sh) * sizeof(XYZZ<F>)));
-  if (const uint32_t S = affine_S) {
-    size_t nsl = max_slices;
-    CU(bk.nodeA.alloc(nsl * (S / 2) * sizeof(Affine<F>)));
-    CU(bk.nodeB.alloc(nsl * (S / 4 ? S / 4 : 1) * sizeof(Affine<F>)));
-    CU(bk.aff_pre.alloc(nsl * (S / 2) * sizeof(F)));
-    CU(bk.aff_ids.alloc(nsl * (S / 2) * sizeof(uint2)));
-    size_t nblk_max = (nsl * (S / 2) + kAffBlock * kAffPairs - 1) / (kAffBlock * kAffPairs);
-    CU(bk.aff_others.alloc(nblk_max * kAffBlock * sizeof(F)));
-    CU(bk.aff_btot.alloc(nblk_max * sizeof(F)));
-  }
-  CU(bk.slice_out.alloc((size_t)(affine_S ? 1 : max_slices) * sizeof(XYZZ<F>)));
-  CU(bk.partials.alloc(std::max((size_t)sh.vecs * sh.groups * nseg + 1024, bucket_tail_records(sh)) * sizeof(XYZZ<F>)));
+int bucket_phase(Bases* b, const SortScratch& ss, BucketScratch& bk, uint32_t vecs, size_t n_terms, XYZZ<F>* d_out,
+                 cudaStream_t st) {
+  if (b->affine_S && ss.slice_S != b->affine_S) return fail(B200_EINVAL, "msm_buckets: slice size mismatch");
+  CU(b200::bucket_phase<F>(msm_env(), b, ss, bk, vecs, n_terms, d_out, st));
+  return B200_OK;
+}
+
+// One MSM's back end in the set's own bucket scratch, over `ss` (the set's own sort or that of a set sharing it).
+template <class F>
+int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out, cudaStream_t st) {
+  const MsmShape& sh = b->sh;
+  if (ss.sh.c != sh.c || ss.sh.table_stride != sh.table_stride || ss.sh.rows != sh.rows || ss.max_slices != b->sort.max_slices ||
+      ss.slice_S != b->sort.slice_S)
+    return fail(B200_EINVAL, "msm_buckets: sort scratch does not match the base set");
+  return bucket_phase<F>(b, ss, b->bk, 1, n_terms, d_out, st);
+}
+
+template <class F>
+int msm_enqueue(Bases* b, const Fr* d_scalars, size_t n, int mont, XYZZ<F>* d_out, int* err, cudaStream_t st) {
+  if (n > b->n) return fail(B200_EINVAL, "msm: n=%zu exceeds base set size %zu", n, b->n);
+  CU(b200::msm_enqueue<F>(msm_env(), b, d_scalars, n, mont, d_out, err, st));
   return B200_OK;
 }
 
@@ -318,26 +245,9 @@ int check_err_flag(const char* what, int* d_err, cudaStream_t st = nullptr, std:
   return B200_OK;
 }
 
-// The window shape of a base set of n points with c-bit windows, t = B200_CFG_TABLE_WINDOWS as it was at the set's load.
-MsmShape msm_shape(size_t n, int c, int t) {
-  MsmShape sh{};
-  sh.n = (uint32_t)n;
-  sh.c = (uint32_t)c;
-  sh.nwin = (255 + c - 1) / c;
-  sh.nbuckets = 1u << (c - 1);
-  sh.table_stride = (uint32_t)n;
-  // B200_CFG_TABLE_WINDOWS: keep t of the nwin window rows; window w reads row w mod t and feeds bucket group w / t
-  sh.rows = t > 0 && (uint32_t)t < sh.nwin ? (uint32_t)t : sh.nwin;
-  sh.groups = (sh.nwin + sh.rows - 1) / sh.rows;
-  return sh;
-}
-
-// prefer_affine: batched-affine bucket accumulation (6 multiplies per add instead of 10) whenever the buckets are
-// populated enough to amortise its per-round launches; since the per-round inversion became a binary-Euclid warp
-// it also wins for a stand-alone MSM.  A proving-key
-// shard that leaves a rank only a small MSM passes false (prove_host.cuh); B200_ACC_MODE=xyzz|affine forces either.
 // The points: n standard-form Jacobian points `pts` on the host, or, with `gen`, d_scalars[i] * G minted on the device
 // straight into the table's row 0 (n standard-form scalars < r, device memory): the same table words either way.
+// prefer_affine: see affine_slice_size (msm_host.cuh).
 template <class F>
 int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_ptr<Bases>& out_b, bool prefer_affine = true,
                  const FixedBaseTable<F>* gen = nullptr, const Fr* d_scalars = nullptr) {
@@ -348,33 +258,12 @@ int bases_create(const uint64_t* pts, size_t n, int c, int group, std::unique_pt
   b->group = group;
   b->n = n;
   b->sh = msm_shape(n, c, g_table_windows);
-  MsmShape& sh = b->sh;
-  const bool reduced = sh.rows < sh.nwin;
+  const MsmShape& sh = b->sh;
   if ((uint64_t)sh.nwin * n >= (1ull << 31)) return fail(B200_EINVAL, "nwin*n exceeds 2^31 entries");
   CU(b->table.alloc((size_t)sh.rows * n * sizeof(Affine<F>)));
   CU(b->scalars.alloc(n * sizeof(Fr)));
-  {
-    // accumulation mode: batched affine (6.5 multiplies per add, 3 launches per round) where the buckets are populated
-    // enough to amortise the rounds, else XYZZ mixed adds (10 multiplies, one launch); b200_config forces either.  Auto
-    // mode keeps a reduced table on XYZZ: the batched-affine node scratch alone is about the size of a full table.
-    const bool xyzz_mode = g_acc_mode == 2 || (g_acc_mode == 0 && (!prefer_affine || reduced));
-    uint32_t S = 0;
-    uint64_t mean = ((uint64_t)sh.nwin * n) / total_buckets(sh);
-    const uint64_t min_mean = g_acc_mode == 1 ? 16 : 96;
-    if (!xyzz_mode && mean >= min_mean) {
-      S = 8;
-      while (S < 128 && (uint64_t)S * 2 * 6 <= mean) S *= 2;   // largest power of two <= mean/6, in [8, 128]
-    }
-    b->affine_S = S;
-    int rc_ = sort_alloc(b->sort, sh, S);
-    if (rc_) return rc_;
-  }
-  // short latency chain: 4-bucket segments (8 adds + one small scalar mul per thread), then a two-level tree sum
-  // (c < 7); nseg segments per window group.  c >= 7: the scratch of launch_bucket_tail.
-  b->seg = sh.nbuckets >= 256 ? 4 : 1;
-  b->nseg = (sh.nbuckets + b->seg - 1) / b->seg;
-  int rc_ = bucket_alloc<F>(b->bk, sh, b->sort.max_slices, b->affine_S, b->nseg);
-  if (rc_) return rc_;
+  b->affine_S = affine_slice_size(sh, g_acc_mode, prefer_affine);
+  CU(bases_scratch<F>(*b));
   CU(b->result.alloc(sizeof(XYZZ<F>)));
   CU(b->out_std.alloc(3 * sizeof(F)));
   CU(b->d_err.alloc(sizeof(int)));
@@ -416,321 +305,6 @@ Bases* find_bases(b200_bases_t h, int group) {
   return it->second.get();
 }
 
-// Enqueue one MSM on `st`; result XYZZ written to d_out (device).
-// Accumulate launch: LPB lanes per bucket slice (2 / 4 / 8 by mean bucket population).  Register budget:
-// G1 runs at 128 regs (4 CTAs/SM); occupancy / prefetch variants were no faster — the kernel is bound by the
-// IMAD.WIDE issue rate, not by latency hiding.
-template <class F, int LPB>
-void launch_accumulate_l(const Affine<F>* table, const uint32_t* entries, SliceTables stb, uint32_t m,
-                         XYZZ<F>* out, uint32_t max_slices, cudaStream_t st) {
-  unsigned grid = nblocks((size_t)max_slices * LPB, 128);
-  if constexpr (sizeof(F) == sizeof(Fq)) {
-    k_accumulate<F, LPB, 4><<<grid, 128, 0, st>>>(table, entries, stb, m, out);
-  } else {
-    k_accumulate<F, LPB, 1><<<grid, 128, 0, st>>>(table, entries, stb, m, out);
-  }
-}
-template <class F>
-void launch_accumulate(int lpb, const Affine<F>* table, const uint32_t* entries, SliceTables stb, uint32_t m,
-                       XYZZ<F>* out, uint32_t max_slices, cudaStream_t st) {
-  switch (lpb) {
-    case 2: launch_accumulate_l<F, 2>(table, entries, stb, m, out, max_slices, st); break;
-    case 4: launch_accumulate_l<F, 4>(table, entries, stb, m, out, max_slices, st); break;
-    default: launch_accumulate_l<F, 8>(table, entries, stb, m, out, max_slices, st); break;
-  }
-}
-
-constexpr int kLPB = 8;
-
-// d_out[0] = sum of partials[0..n): one block if small, else 512 inputs per first-level block + a final block.
-// `partials` must have room for n + ceil(n/512) records.
-template <class F>
-void launch_tree_sum(XYZZ<F>* partials, uint32_t n, XYZZ<F>* d_out, cudaStream_t st) {
-  if (n <= 1024) {
-    k_sum_points<F><<<1, 256, 0, st>>>(partials, n, n, d_out);
-    g_launches += 1;
-    return;
-  }
-  uint32_t nb = (n + 511) / 512;
-  k_sum_points<F><<<nb, 256, 0, st>>>(partials, n, 512, partials + n);
-  k_sum_points<F><<<1, 256, 0, st>>>(partials + n, nb, nb, d_out);
-  g_launches += 2;
-}
-
-constexpr uint32_t kMaxGridY = 65535;   // gridDim.y limit: rows per launch of the (vector, group) tail kernels
-
-// sum_g 2^(c*t*g) sum_b b * S_(g,b) over the bucket array -> one XYZZ record per scalar vector (msm.cuh: rows / columns
-// and bit planes of every window group, one Horner chain over the groups of each vector).  `scratch` holds
-// bucket_tail_records(sh) records.  Tiny bucket sets keep the segment kernel.
-template <class F>
-void launch_bucket_tail(const XYZZ<F>* buckets, const MsmShape& sh, XYZZ<F>* scratch, XYZZ<F>* d_out, cudaStream_t st) {
-  const uint32_t bits = sh.c - 1, kl = (bits + 1) / 2, kh = bits - kl, K = 1u << kl, H = 1u << kh, G = sh.groups;
-  const uint32_t GV = sh.vecs * G;
-  XYZZ<F>* R = scratch;
-  XYZZ<F>* C = scratch + (size_t)GV * H;
-  XYZZ<F>* planes = C + (size_t)GV * K;
-  for_each_tail_chunk(sh, kMaxGridY, [&](uint32_t y0, uint32_t ny) {
-    k_tail_rowcol<F><<<dim3(nblocks((size_t)(H + K) * 32, 128), ny), 128, 0, st>>>(buckets + (size_t)y0 * H * K, kl, H,
-                                                                                    R + (size_t)y0 * H, C + (size_t)y0 * K);
-    k_tail_planes<F><<<dim3(nblocks((size_t)(bits + 1) * 32, 128), ny), 128, 0, st>>>(
-        R + (size_t)y0 * H, C + (size_t)y0 * K, kl, kh, planes + (size_t)y0 * (bits + 1));
-    g_launches += 2;
-  });
-  k_tail_horner<F><<<sh.vecs, 32, 0, st>>>(planes, bits, d_out, G, sh.c * sh.rows);
-  g_launches += 1;
-}
-
-// The c < 7 tail: segment sums of every window group, each scaled by 2^(c*t*g), then one tree sum over all of them (one
-// block per scalar vector in a batch).
-template <class F>
-void launch_segment_tail(const Bases* b, const MsmShape& sh, const XYZZ<F>* buckets, XYZZ<F>* partials, XYZZ<F>* d_out,
-                         cudaStream_t st) {
-  if (sh.vecs == 1) {
-    k_bucket_reduce<F><<<dim3(nblocks(b->nseg, 128), sh.groups), 128, 0, st>>>(buckets, sh.nbuckets, b->seg, partials, b->nseg,
-                                                                                sh.c * sh.rows);
-    launch_tree_sum<F>(partials, sh.groups * b->nseg, d_out, st);
-    return;
-  }
-  for_each_tail_chunk(sh, kMaxGridY, [&](uint32_t y0, uint32_t ny) {
-    k_bucket_reduce<F, true><<<dim3(nblocks(b->nseg, 128), ny), 128, 0, st>>>(
-        buckets + (size_t)y0 * sh.nbuckets, sh.nbuckets, b->seg, partials + (size_t)y0 * b->nseg, b->nseg, sh.c * sh.rows,
-        sh.groups);
-    if (y0) g_launches += 1;   // the caller counts the first k_bucket_reduce
-  });
-  const uint32_t per = sh.groups * b->nseg;
-  k_sum_points<F><<<sh.vecs, 256, 0, st>>>(partials, sh.vecs * per, per, d_out);
-  g_launches += 1;
-}
-
-// Front end: signed-digit recode + counting sort of n scalars (of each of shape.vecs vectors) into bucket order.  A
-// standard-form scalar >= r is read as 0 and sets bit 1 of *err.  With `scan_totals` (room for kScanBlocks values) a
-// large batch scans its counters with several blocks (one more launch).
-int msm_sort(SortScratch& ss, const MsmShape& shape, const Fr* d_scalars, size_t n, int mont, int* err, cudaStream_t st,
-             unsigned long long* scan_totals = nullptr) {
-  if (n > ss.sh.n || shape.c != ss.sh.c || shape.table_stride != ss.sh.table_stride || shape.rows != ss.sh.rows ||
-      shape.vecs > ss.sh.vecs)
-    return fail(B200_EINVAL, "msm_sort: shape mismatch");
-  MsmShape sh = shape;
-  sh.n = (uint32_t)n;
-  const uint32_t B = total_buckets(sh);
-  uint32_t m = B + 1;  // counts[0] unused (digit 0), buckets 1..B of all window groups
-  // slice cap: twice the mean bucket population (uniform scalars never split), at least 4 per lane.  The mean over a
-  // batch's buckets is that of one vector.
-  uint64_t mean = ((uint64_t)sh.vecs * sh.nwin * n + B - 1) / B;
-  uint32_t cap = (uint32_t)(2 * mean < 4 * kLPB ? 4 * kLPB : 2 * mean);
-  int fixed = 0;
-  if (ss.slice_S) {
-    cap = ss.slice_S;
-    fixed = 1;
-  }
-  uint32_t* counts = ss.counts.as<uint32_t>();
-  const size_t nterm = (size_t)sh.vecs * n;
-  CU(cudaMemsetAsync(counts, 0, (m + 1) * sizeof(uint32_t), st));
-  if (n) k_digits_count<<<nblocks(nterm, 256), 256, 0, st>>>(d_scalars, sh, mont, counts, err);
-  // one block walks up to 64 tiles of counters; beyond that, blocks of 64 tiles each (at most kScanBlocks)
-  constexpr uint32_t kScanTile = 1024, kScanChunk = 64 * kScanTile;
-  if (scan_totals && m > kScanChunk) {
-    uint32_t chunk = kScanChunk;
-    while ((m + chunk - 1) / chunk > kScanBlocks) chunk *= 2;
-    const uint32_t nb = (m + chunk - 1) / chunk;
-    k_scan_totals<<<nb, kScanTile, 0, st>>>(counts, m, cap, chunk, scan_totals);
-    k_scan<<<nb, kScanTile, 0, st>>>(counts, m, cap, fixed, ss.offsets.as<uint32_t>(), ss.cursor.as<uint32_t>(), ss.tables(),
-                                     chunk, scan_totals);
-    g_launches += 1;
-  } else {
-    k_scan<<<1, kScanTile, 0, st>>>(counts, m, cap, fixed, ss.offsets.as<uint32_t>(), ss.cursor.as<uint32_t>(), ss.tables());
-  }
-  k_fill_slices<<<nblocks(m, 256), 256, 0, st>>>(counts, ss.offsets.as<uint32_t>(), m, cap, fixed, ss.tables());
-  if (n) k_digits_scatter<<<nblocks(nterm, 256), 256, 0, st>>>(d_scalars, sh, mont, ss.cursor.as<uint32_t>(),
-                                                               ss.entries.as<uint32_t>(), err);
-  g_launches += n ? 4 : 2;
-  CU(cudaGetLastError());
-  return B200_OK;
-}
-
-// Back end: bucket accumulation over the sorted entries of `ss`, slice merge, weighted bucket
-// reduction and final tree sum -> one XYZZ record in d_out per scalar vector (vecs of them), in the scratch `bk`.
-template <class F>
-int bucket_phase(Bases* b, const SortScratch& ss, BucketScratch& bk, uint32_t vecs, size_t n_terms, XYZZ<F>* d_out,
-                 cudaStream_t st) {
-  MsmShape sh = b->sh;
-  sh.vecs = vecs;
-  const uint32_t B = total_buckets(sh);
-  uint32_t m = B + 1;
-  XYZZ<F>* buckets = bk.buckets.as<XYZZ<F>>();
-  XYZZ<F>* partials = bk.partials.as<XYZZ<F>>();
-  SliceTables stb = ss.tables();
-  // The out-of-line F_q multiply wins here: the fully inlined madd body (~38 KB of SASS) thrashes the
-  // instruction caches.
-  ProfRec pr{};
-  if (g_prof) {
-    pr = ProfRec{prof_event(), prof_event(), b->group, (size_t)vecs * n_terms};
-    cudaEventRecord(pr.e0, st);
-  }
-  if (b->affine_S) {
-    if (ss.slice_S != b->affine_S) return fail(B200_EINVAL, "msm_buckets: slice size mismatch");
-    const uint32_t S = b->affine_S;
-    uint32_t R = 0;
-    while ((1u << R) < S) R++;
-    // host-side bound on the live slice count for this call (the exact count lives on the device)
-    uint64_t total = (uint64_t)vecs * sh.nwin * n_terms;
-    uint64_t nsl_bound = (uint64_t)B + (total + S - 1) / S + 2;
-    if (nsl_bound > ss.max_slices) nsl_bound = ss.max_slices;
-    AffineRound<F> ar{};
-    ar.table = b->table.as<Affine<F>>();
-    ar.entries = ss.entries.as<uint32_t>();
-    ar.slice_start = stb.slice_start;
-    ar.slice_end = stb.slice_end;
-    ar.nslices_ptr = stb.slice_off + m;
-    ar.pre = bk.aff_pre.as<F>();
-    ar.others = bk.aff_others.as<F>();
-    ar.btot = bk.aff_btot.as<F>();
-    ar.pair_ids = g_tma_staging == 1 ? bk.aff_ids.as<uint2>() : nullptr;
-    // node buffers, x- and y-coordinates in separate halves (bucket_affine.cuh NodeBuf)
-    const size_t capA = (size_t)ss.max_slices * (S / 2), capB = (size_t)ss.max_slices * (S / 4 ? S / 4 : 1);
-    NodeBuf<F> bufs[2] = {{bk.nodeA.as<F>(), bk.nodeA.as<F>() + capA}, {bk.nodeB.as<F>(), bk.nodeB.as<F>() + capB}};
-    NodeBuf<F> prev{nullptr, nullptr};
-    // all R rounds affine: inside a proof the per-round inversion latency is hidden by the other MSMs' streams
-    for (uint32_t r = 1; r <= R; r++) {
-      ar.round = r;
-      ar.q_log = R - r;
-      ar.prev = prev;
-      ar.out = bufs[(r - 1) & 1];
-      uint64_t npairs_max = nsl_bound << ar.q_log;
-      unsigned nb = (unsigned)((npairs_max + kAffBlock * kAffPairs - 1) / (kAffBlock * kAffPairs));
-      // CTAs/SM bounds = register caps (forward 8 + backward 5 CTAs/SM for G1, 4 + 4 for G2); chosen by a sweep on an
-      // earlier target and not re-swept on the H100
-      if (sizeof(F) == 32) {
-        k_affine_forward<F, kAffPairs, 8><<<nb, kAffBlock, 0, st>>>(ar);
-        k_affine_invert<F><<<nblocks((size_t)nb * 32, 128), 128, 0, st>>>(ar.btot, nb);
-        if (g_tma_staging == 1 || (g_tma_staging == 2 && r >= 2)) k_affine_backward_staged<F, kAffPairs, 5><<<nb, kAffBlock, AffStageLayout<F>::kSmem, st>>>(ar);
-        else k_affine_backward<F, kAffPairs, 5><<<nb, kAffBlock, 0, st>>>(ar);
-      } else {
-        k_affine_forward<F, kAffPairs, 4><<<nb, kAffBlock, 0, st>>>(ar);
-        k_affine_invert<F><<<nblocks((size_t)nb * 32, 128), 128, 0, st>>>(ar.btot, nb);
-        if (g_tma_staging == 1 || (g_tma_staging == 2 && r >= 2)) k_affine_backward_staged<F, kAffPairs, 4><<<nb, kAffBlock, AffStageLayout<F>::kSmem, st>>>(ar);
-        else k_affine_backward<F, kAffPairs, 4><<<nb, kAffBlock, 0, st>>>(ar);
-      }
-      prev = ar.out;
-      g_launches += 3;
-    }
-    if (g_prof) {
-      cudaEventRecord(pr.e1, st);
-      g_prof_recs.push_back(pr);
-    }
-    k_merge_slices_affine<F><<<nblocks(B, 128), 128, 0, st>>>(prev, stb, B, buckets);
-    if (sh.c >= 7) {
-      launch_bucket_tail<F>(buckets, sh, partials, d_out, st);
-      g_launches += 1;
-    } else {
-      launch_segment_tail<F>(b, sh, buckets, partials, d_out, st);
-      g_launches += 2;
-    }
-    CU(cudaGetLastError());
-    return B200_OK;
-  }
-  uint64_t mean = ((uint64_t)vecs * sh.nwin * n_terms + B - 1) / B;   // that of one vector
-  int lpb = mean >= 384 ? 8 : (mean >= 96 ? 4 : 2);
-  launch_accumulate<F>(lpb, b->table.as<Affine<F>>(), ss.entries.as<uint32_t>(), stb, m,
-                       bk.slice_out.as<XYZZ<F>>(), ss.max_slices, st);
-  if (g_prof) {
-    cudaEventRecord(pr.e1, st);
-    g_prof_recs.push_back(pr);
-  }
-  k_merge_slices<F><<<nblocks(B, 128), 128, 0, st>>>(bk.slice_out.as<XYZZ<F>>(), stb, B, buckets);
-  if (sh.c >= 7) {
-    launch_bucket_tail<F>(buckets, sh, partials, d_out, st);
-    g_launches += 1;
-  } else {
-    launch_segment_tail<F>(b, sh, buckets, partials, d_out, st);
-    g_launches += 3;
-  }
-  CU(cudaGetLastError());
-  return B200_OK;
-}
-
-// One MSM's back end in the set's own bucket scratch (4 launches + the tail).
-template <class F>
-int msm_buckets(Bases* b, const SortScratch& ss, size_t n_terms, XYZZ<F>* d_out, cudaStream_t st) {
-  const MsmShape& sh = b->sh;
-  if (ss.sh.c != sh.c || ss.sh.table_stride != sh.table_stride || ss.sh.rows != sh.rows || ss.max_slices != b->sort.max_slices ||
-      ss.slice_S != b->sort.slice_S)
-    return fail(B200_EINVAL, "msm_buckets: sort scratch does not match the base set");
-  return bucket_phase<F>(b, ss, b->bk, 1, n_terms, d_out, st);
-}
-
-template <class F>
-int msm_enqueue(Bases* b, const Fr* d_scalars, size_t n, int mont, XYZZ<F>* d_out, int* err, cudaStream_t st) {
-  if (n > b->n) return fail(B200_EINVAL, "msm: n=%zu exceeds base set size %zu", n, b->n);
-  int rc = msm_sort(b->sort, b->sh, d_scalars, n, mont, err, st);
-  if (rc) return rc;
-  return msm_buckets<F>(b, b->sort, n, d_out, st);
-}
-
-// ---- batches: k scalar vectors over one base set -----------------------------------------------------------------
-// Term i of vector p is scalar p*stride + i times base i; vector p's digits go to its own window groups, so one recode,
-// one counting sort, one accumulation and one tail serve all k vectors.  Populations per bucket, and so the slice cap,
-// the lanes per bucket and the accumulation kernel, are those of one vector.
-bool batch_fits(const MsmShape& sh, size_t k, size_t n) {
-  return (uint64_t)k * sh.nwin * n < (1ull << 31) && (uint64_t)k * total_buckets(sh) + 3 < (1ull << 31);
-}
-bool batch_fits(const Bases* b, size_t k, size_t n) { return batch_fits(b->sh, k, n); }
-
-// The batch scratch of `b` for k vectors of n terms: allocated on the first batch, regrown to the larger of the old and
-// the new capacity in each dimension when a batch exceeds it.  Before the old buffers are freed the host waits for the
-// set's last batch (its `done` event); batches on one set are ordered on one stream (b200snark.h), so nothing else of
-// this set can still read them, and work on other sets and prove contexts is not waited for.
-// with_sort = false (a proving-key set whose batches reuse another set's sort of the same scalars): bucket scratch
-// only, for that sort's slices; the shape is recorded in `sort.sh`, and nothing else of `sort` is allocated.
-template <class F>
-int batch_scratch(Bases* b, uint32_t k, uint32_t n, bool with_sort = true) {
-  if (n == 0) n = 1;
-  if (b->batch && b->batch->vecs >= k && b->batch->sort.sh.n >= n && (!with_sort || b->batch->sort.entries.p)) return B200_OK;
-  if (b->batch) {
-    CU(cudaEventSynchronize(b->batch->done));
-    const uint32_t k2 = std::max(k, b->batch->vecs), n2 = std::max(n, b->batch->sort.sh.n);
-    if (batch_fits(b, k2, n2)) k = k2, n = n2;   // else: exactly this batch's size
-  }
-  b->batch.reset();
-  auto mb = std::make_unique<MsmBatch>();
-  MsmShape sh = b->sh;
-  sh.n = n;
-  sh.vecs = k;
-  int rc;
-  if (with_sort) {
-    if ((rc = sort_alloc(mb->sort, sh, b->affine_S))) return rc;
-    CU(mb->scan_totals.alloc(kScanBlocks * sizeof(unsigned long long)));
-  } else {
-    mb->sort.sh = sh;
-  }
-  if ((rc = bucket_alloc<F>(mb->bk, sh, sort_max_slices(sh, b->affine_S), b->affine_S, b->nseg))) return rc;
-  CU(cudaEventCreateWithFlags(&mb->done, cudaEventDisableTiming));
-  mb->vecs = k;
-  b->batch = std::move(mb);
-  return B200_OK;
-}
-
-template <class F>
-int msm_batch_enqueue(Bases* b, const Fr* d_scalars, size_t n, size_t k, size_t stride, int mont, XYZZ<F>* d_out, int* err,
-                      cudaStream_t st) {
-  if (k == 0) return fail(B200_EINVAL, "msm_device_batch: k = 0");
-  if (n > b->n) return fail(B200_EINVAL, "msm_device_batch: n=%zu exceeds base set size %zu", n, b->n);
-  if (stride > 0xffffffffull) return fail(B200_EINVAL, "msm_device_batch: stride %zu exceeds 2^32 - 1", stride);
-  if (!batch_fits(b, k, n ? n : 1))
-    return fail(B200_EINVAL, "msm_device_batch: k * nwin * n = %zu * %u * %zu sort entries (or the buckets) exceed 2^31", k,
-                b->sh.nwin, n);
-  int rc = batch_scratch<F>(b, (uint32_t)k, (uint32_t)n);
-  if (rc) return rc;
-  MsmBatch& mb = *b->batch;
-  MsmShape sh = b->sh;
-  sh.vecs = (uint32_t)k;
-  sh.vec_stride = (uint32_t)stride;
-  if ((rc = msm_sort(mb.sort, sh, d_scalars, n, mont, err, st, mb.scan_totals.as<unsigned long long>()))) return rc;
-  if ((rc = bucket_phase<F>(b, mb.sort, mb.bk, (uint32_t)k, n, d_out, st))) return rc;
-  CU(cudaEventRecord(mb.done, st));
-  return B200_OK;
-}
-
 template <class F>
 int msm_host(b200_bases_t h, int group, const uint64_t* scalars, size_t n, uint64_t* out) {
   Bases* b = find_bases(h, group);
@@ -769,7 +343,7 @@ int mul_batch(const uint64_t* pts, int bcast, const uint64_t* scalars, size_t n,
   CU(dout.alloc(n * 3 * sizeof(F)));
   CU(cudaMemcpyAsync(dp.p, pts, np * 3 * sizeof(F), cudaMemcpyHostToDevice, g_ctx[0].main));
   CU(cudaMemcpyAsync(ds.p, scalars, n * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
-  k_mul_batch_ref<F><<<nblocks(n, 128), 128, 0, g_ctx[0].main>>>(dp.as<F>(), bcast, ds.as<Fr>(), n, dout.as<F>(), g_d_err);
+  k_mul_batch_ref<F><<<nblk(n, 128), 128, 0, g_ctx[0].main>>>(dp.as<F>(), bcast, ds.as<Fr>(), n, dout.as<F>(), g_d_err);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, dout.p, n * 3 * sizeof(F), cudaMemcpyDeviceToHost, g_ctx[0].main));
   return check_err_flag("mul_batch", g_d_err);
@@ -973,10 +547,9 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
     if (!pk->g[j]) continue;
     const bool own = pk->sort_src[j] == j;
     const uint32_t n = (uint32_t)sl.terms[j];
-    rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, n, own) : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, n, own);
-    if (rc) return rc;
+    CU(j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, n, own) : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, n, own));
   }
-  if (pk->g[3] && (rc = batch_scratch<Fq>(pk->g[3].get(), (uint32_t)k, (uint32_t)nch))) return rc;
+  if (pk->g[3]) CU(batch_scratch<Fq>(pk->g[3].get(), (uint32_t)k, (uint32_t)nch));
   for (int j = 0; j < 3; j++)
     if (pk->g[j] && !batch_shares_sort(pk->g[j].get(), pk->g[pk->sort_src[j]].get()))
       return fail(B200_EINVAL, "groth16_prove_witness_batch: batch scratch of set %d does not match the sort of set %d", j, pk->sort_src[j]);
@@ -1235,9 +808,8 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
   for (int j = 0; j < 8; j++) {
     if (!pk->g[j]) continue;   // a set another rank owns, or A, Ap of a circuit whose signals are all public
     const bool own = src[j] == j;
-    rc = j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own)
-                : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own);
-    if (rc) return rc;
+    CU(j == 2 ? batch_scratch<Fq2>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own)
+              : batch_scratch<Fq>(pk->g[j].get(), (uint32_t)k, (uint32_t)terms[j], own));
   }
   for (int j = 0; j < 8; j++)
     if (pk->g[j] && !batch_shares_sort(pk->g[j].get(), pk->g[src[j]].get()))
@@ -2523,9 +2095,16 @@ int b200_msm_device_batch(b200_bases_t h, const void* d_scalars, size_t n, size_
   Bases* b = find_bases(h, 0);
   if (!b || !d_out || (!d_scalars && n)) return fail(B200_EINVAL, "msm_device_batch: bad arguments");
   cudaStream_t st = stream ? (cudaStream_t)stream : g_ctx[0].main;
+  if (k == 0) return fail(B200_EINVAL, "msm_device_batch: k = 0");
+  if (n > b->n) return fail(B200_EINVAL, "msm_device_batch: n=%zu exceeds base set size %zu", n, b->n);
+  if (stride > 0xffffffffull) return fail(B200_EINVAL, "msm_device_batch: stride %zu exceeds 2^32 - 1", stride);
+  if (!batch_fits(b, k, n ? n : 1))
+    return fail(B200_EINVAL, "msm_device_batch: k * nwin * n = %zu * %u * %zu sort entries (or the buckets) exceed 2^31", k,
+                b->sh.nwin, n);
   int* err = b->d_err.as<int>();
-  if (b->group == 1) return msm_batch_enqueue<Fq>(b, (const Fr*)d_scalars, n, k, stride, mont, (XYZZ<Fq>*)d_out, err, st);
-  return msm_batch_enqueue<Fq2>(b, (const Fr*)d_scalars, n, k, stride, mont, (XYZZ<Fq2>*)d_out, err, st);
+  if (b->group == 1) CU(msm_batch_enqueue<Fq>(msm_env(), b, (const Fr*)d_scalars, n, k, stride, mont, (XYZZ<Fq>*)d_out, err, st));
+  else CU(msm_batch_enqueue<Fq2>(msm_env(), b, (const Fr*)d_scalars, n, k, stride, mont, (XYZZ<Fq2>*)d_out, err, st));
+  return B200_OK;
 }
 
 int b200_g1_sum_partials(const void* d, size_t count, uint64_t out[12], void* stream) {

@@ -9,11 +9,15 @@
 
 // Kernel launches of the polynomial orchestration go through these two macros so that the SAME host code (transform
 // plans, division, interpolation, subproduct trees) also runs in the CPU test vehicle (tests/host: the macros become
-// loops over emulated CTAs).  _CTA marks kernels that synchronise inside a block.
+// loops over emulated CTAs).  _CTA marks kernels that synchronise inside a block, _CTA_SMEM those that also take dynamic
+// shared memory.  `grid` may be a dim3.  B200_K protects the commas of a template kernel's arguments:
+// B200_LAUNCH(B200_K(k<F, 2>), grid, block, stream, args...).
 #ifndef B200_LAUNCH
 #define B200_LAUNCH(kernel, grid, block, stream, ...) kernel<<<(grid), (block), 0, (stream)>>>(__VA_ARGS__)
 #define B200_LAUNCH_CTA(kernel, grid, block, stream, ...) kernel<<<(grid), (block), 0, (stream)>>>(__VA_ARGS__)
+#define B200_LAUNCH_CTA_SMEM(kernel, grid, block, smem, stream, ...) kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)
 #endif
+#define B200_K(...) __VA_ARGS__
 
 namespace b200 {
 

@@ -2,7 +2,8 @@
 // variants — the product kernel and the experiment kernels k_affine_backward_lr / _sp — are run one emulated thread at
 // a time over all rounds of a small slice forest, against a plain host restatement of the forward pass.  What this
 // checks is the kernels' own index logic (pair <-> slice <-> entry mapping, staging queues, fast/slow path split,
-// sign and infinity handling); the field arithmetic underneath is covered by host_arith_test.cpp.
+// sign and infinity handling); the field arithmetic underneath is covered by host_arith_test.cpp.  Whole MSMs run the
+// library's own MSM engine (msm_host.cuh) on the emulated kernels.
 // Test infrastructure only: never linked into libb200snark.
 #include "host_stub/cuda_runtime.h"
 
@@ -14,13 +15,18 @@
 #include "bucket_affine.cuh"
 #include "ntt.cuh"
 
-// the polynomial orchestration (poly_host.cuh, qap_sparse.cuh) launches through these: sequential emulated threads for
-// plain kernels, one OS thread per CUDA thread for kernels that synchronise inside a CTA
-template <class K> void stub_launch_threads(unsigned nblocks, unsigned nthreads, K k);
-template <class K> void stub_launch_cta(unsigned nblocks, unsigned nthreads, K k);
-#define B200_LAUNCH(kernel, grid, block, stream, ...) stub_launch_threads((unsigned)(grid), (unsigned)(block), [&] { kernel(__VA_ARGS__); })
-#define B200_LAUNCH_CTA(kernel, grid, block, stream, ...) stub_launch_cta((unsigned)(grid), (unsigned)(block), [&] { kernel(__VA_ARGS__); })
+// the host orchestration (poly_host.cuh, qap_sparse.cuh, msm_host.cuh) launches through these: sequential emulated
+// threads for plain kernels, one OS thread per CUDA thread for kernels that synchronise inside a CTA (with `smem` bytes of
+// dynamic shared memory per CTA)
+template <class K> void stub_launch_threads(dim3 grid, unsigned nthreads, K k);
+template <class K> void stub_launch_cta(dim3 grid, unsigned nthreads, size_t smem, K k);
+#define B200_LAUNCH(kernel, grid, block, stream, ...) stub_launch_threads(dim3(grid), (unsigned)(block), [&] { kernel(__VA_ARGS__); })
+#define B200_LAUNCH_CTA(kernel, grid, block, stream, ...) stub_launch_cta(dim3(grid), (unsigned)(block), 0, [&] { kernel(__VA_ARGS__); })
+#define B200_LAUNCH_CTA_SMEM(kernel, grid, block, smem, stream, ...) \
+  stub_launch_cta(dim3(grid), (unsigned)(block), (size_t)(smem), [&] { kernel(__VA_ARGS__); })
 #include "qap_sparse.cuh"
+#include "fixed_base.cuh"
+#include "msm_host.cuh"
 #include "pairing_warp.cuh"
 #include "glv.cuh"
 
@@ -64,9 +70,10 @@ unsigned stub_ballot(int pred) {
   return r;
 }
 namespace {
-// run `kernel()` for every thread of CTA `b` (nthreads a multiple of 32, <= 256)
+// run `kernel()` for every thread of CTA (b, y) of an nblocks x ny grid (nthreads a multiple of 32, <= 1024), with
+// `smem` as its dynamic shared memory
 template <class K>
-void run_cta(unsigned b, unsigned nthreads, unsigned nblocks, K kernel) {
+void run_cta(unsigned b, unsigned nthreads, unsigned nblocks, K kernel, unsigned y = 0, unsigned ny = 1, uint8_t* smem = nullptr) {
   pthread_barrier_init(&g_block_bar, nullptr, nthreads);
   for (unsigned w = 0; w < nthreads / 32; w++) pthread_barrier_init(&g_warp_bar[w], nullptr, 32);
   g_cta_mode = true;
@@ -75,8 +82,11 @@ void run_cta(unsigned b, unsigned nthreads, unsigned nblocks, K kernel) {
     th.emplace_back([=] {
       threadIdx.x = t;
       blockIdx.x = b;
+      blockIdx.y = y;
       blockDim.x = nthreads;
       gridDim.x = nblocks;
+      gridDim.y = ny;
+      g_stub_dyn_smem = smem;
       kernel();
     });
   for (auto& x : th) x.join();
@@ -231,8 +241,74 @@ int affine_rounds(int variant, int fwd_variant, const uint32_t* table_std, uint3
   return 0;
 }
 
-// Back end of an MSM after the accumulation: slices -> buckets (k_merge_slices_affine), sum_b b*S_b by segments
-// (k_bucket_reduce), tree sum (k_sum_points, one or two levels like launch_tree_sum), normalisation (k_finalize).
+template <class K>
+void run_threads(dim3 grid, unsigned nthreads, K kernel) {  // kernels without barriers: one thread at a time
+  blockDim.x = nthreads;
+  gridDim.x = grid.x;
+  gridDim.y = grid.y;
+  for (unsigned y = 0; y < grid.y; y++)
+    for (unsigned b = 0; b < grid.x; b++)
+      for (unsigned t = 0; t < nthreads; t++) {
+        blockIdx.x = b;
+        blockIdx.y = y;
+        threadIdx.x = t;
+        kernel();
+      }
+}
+inline unsigned cdiv(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
+
+// The MSM engine's settings in the vehicles: launch limits lowered so that small inputs reach two-level tree sums (above
+// 64 records, 32 per first-level block), chunked tails (max_rows rows per launch) and multi-block counter scans (blocks of
+// scan_chunk counters; 0: one block); staging = B200_CFG_TMA_STAGING.
+inline MsmEnv test_env(int staging, uint32_t max_rows = kMaxGridY, uint32_t scan_chunk = 0) {
+  MsmEnv env;
+  env.tma_staging = staging;
+  env.tail_rows = max_rows;
+  env.scan_chunk = scan_chunk ? scan_chunk : 0xffffffffu;
+  env.tree_sum_max = 64;
+  env.tree_sum_leaf = 32;
+  return env;
+}
+
+// A base set as bases_create makes one, on the emulated device: n standard-form Jacobian points, c-bit windows, t table
+// rows (0: all) built by window_table_enqueue, and the engine's scratch for batched-affine slices of S entries (0: XYZZ).
+// Bit 0 of err: a coordinate >= q.
+template <class F>
+int make_bases(Bases& b, int group, const uint32_t* jac_std, uint32_t n, uint32_t c, uint32_t t, uint32_t S, int* err) {
+  b.group = group;
+  b.n = n;
+  b.sh = msm_shape(n, (int)c, (int)t);
+  std::vector<F> staging((size_t)n * 3);
+  std::memcpy(staging.data(), jac_std, staging.size() * sizeof(F));
+  std::vector<XYZZ<F>> state(n);
+  if (b.table.alloc((size_t)b.sh.rows * n * sizeof(Affine<F>))) return 91;
+  window_table_enqueue<F>(staging.data(), n, b.sh.rows, (int)c, b.table.as<Affine<F>>(), state.data(), err, nullptr);
+  b.affine_S = S;
+  return bases_scratch<F>(b) ? 92 : 0;
+}
+
+// The sort's own invariants: every entry reads one of the `rows` stored table rows of a base < n, each bucket is filled
+// exactly to the next one's offset, and the slices fit the scratch.
+inline int check_sort(const SortScratch& ss, const MsmShape& sh) {
+  const uint32_t m = total_buckets(sh) + 1;
+  const uint32_t *offsets = ss.offsets.as<uint32_t>(), *cursor = ss.cursor.as<uint32_t>(), *entries = ss.entries.as<uint32_t>();
+  for (uint32_t e = 0; e < offsets[m]; e++)
+    if ((entries[e] >> 1) >= (size_t)sh.rows * sh.table_stride || (entries[e] >> 1) % sh.table_stride >= sh.n) return 96;
+  for (uint32_t b = 1; b < m; b++)
+    if (cursor[b] != offsets[b + 1]) return 97;
+  return ss.tables().slice_off[m] > ss.max_slices ? 99 : 0;
+}
+
+template <class F>
+void finalize_std(const XYZZ<F>& rec, uint32_t* out_std) {
+  F out[3];
+  run_cta(0, 32, 1, [&] { k_finalize<F>(&rec, out); });
+  std::memcpy(out_std, out, sizeof out);
+}
+
+// Back end of an MSM after the accumulation: slices -> buckets (k_merge_slices_affine), then the engine's tails:
+// seg = 0 the rows / columns + bit planes + Horner tail (launch_bucket_tail, nbuckets = 2^(c-1)), else segment sums of seg
+// buckets and a one- or two-level tree sum (launch_segment_tail); normalisation (k_finalize).
 template <class F>
 int msm_tail(const uint32_t* slice_pts_std, const uint32_t* slice_off, uint32_t nbuckets, uint32_t seg, uint32_t* out_std) {
   constexpr int W = sizeof(F) / 4;
@@ -247,159 +323,43 @@ int msm_tail(const uint32_t* slice_pts_std, const uint32_t* slice_off, uint32_t 
   SliceTables st{const_cast<uint32_t*>(slice_off), nullptr, nullptr};
   unsigned nb = (nbuckets + 127) / 128;
   for (unsigned b = 0; b < nb; b++) run_cta(b, 128, nb, [&] { k_merge_slices_affine<F>(NodeBuf<F>{pts.data(), pts.data() + cap_t}, st, nbuckets, buckets.data()); });
+  const MsmEnv env = test_env(0);
   XYZZ<F> total;
-  if (seg == 0) {   // the rows / columns + bit planes + Horner tail (nbuckets = 2^(c-1)), as launch_bucket_tail issues it
+  if (seg == 0) {
     uint32_t bits = 0;
     while ((1u << bits) < nbuckets) bits++;
     if ((1u << bits) != nbuckets) return 7;
-    const uint32_t kl = (bits + 1) / 2, kh = bits - kl, K = 1u << kl, H = 1u << kh;
-    std::vector<XYZZ<F>> scratch((size_t)H + K + bits + 1);
-    XYZZ<F>*R = scratch.data(), *C = R + H, *planes = C + K;
-    unsigned nb1 = ((H + K) * 32 + 127) / 128, nb2 = ((bits + 1) * 32 + 127) / 128;
-    for (unsigned b = 0; b < nb1; b++) run_cta(b, 128, nb1, [&] { k_tail_rowcol<F>(buckets.data(), kl, H, R, C); });
-    for (unsigned b = 0; b < nb2; b++) run_cta(b, 128, nb2, [&] { k_tail_planes<F>(R, C, kl, kh, planes); });
-    run_cta(0, 32, 1, [&] { k_tail_horner<F>(planes, bits, &total); });
-    F out[3];
-    run_cta(0, 32, 1, [&] { k_finalize<F>(&total, out); });
-    std::memcpy(out_std, out, sizeof out);
-    return 0;
-  }
-  uint32_t nseg = (nbuckets + seg - 1) / seg;
-  std::vector<XYZZ<F>> partials((size_t)nseg + 1024);
-  nb = (nseg + 127) / 128;
-  for (unsigned b = 0; b < nb; b++) run_cta(b, 128, nb, [&] { k_bucket_reduce<F>(buckets.data(), nbuckets, seg, partials.data(), nseg); });
-  if (nseg <= 64) {  // (the library switches at 1024; a low threshold here exercises the two-level path on small inputs)
-    run_cta(0, 256, 1, [&] { k_sum_points<F>(partials.data(), nseg, nseg, &total); });
+    const MsmShape sh = msm_shape(0, (int)bits + 1, 0);
+    std::vector<XYZZ<F>> scratch(bucket_tail_records(sh));
+    launch_bucket_tail<F>(env, buckets.data(), sh, scratch.data(), &total, nullptr);
   } else {
-    uint32_t per = 32, nb2 = (nseg + per - 1) / per;
-    for (unsigned b = 0; b < nb2; b++) run_cta(b, 256, nb2, [&] { k_sum_points<F>(partials.data(), nseg, per, partials.data() + nseg); });
-    run_cta(0, 256, 1, [&] { k_sum_points<F>(partials.data() + nseg, nb2, nb2, &total); });
+    MsmShape sh{};   // one window group of nbuckets buckets
+    sh.nbuckets = nbuckets;
+    const uint32_t nseg = (nbuckets + seg - 1) / seg;
+    std::vector<XYZZ<F>> partials((size_t)nseg + 1024);
+    launch_segment_tail<F>(env, sh, seg, nseg, buckets.data(), partials.data(), &total, nullptr);
   }
-  F out[3];
-  run_cta(0, 32, 1, [&] { k_finalize<F>(&total, out); });
-  std::memcpy(out_std, out, sizeof out);
+  finalize_std<F>(total, out_std);
   return 0;
 }
-// ---- a whole MSM, kernel by kernel, in the order and with the parameters the library's msm_sort / msm_buckets /
-// bases_create use (capi.cu): window precompute, digit recode + counting sort + slice tables, bucket accumulation
-// (batched-affine rounds when S != 0, else the XYZZ kernel with LPB lanes per slice), slice merge, weighted bucket
-// reduction, tree sum, normalisation.
-template <class K>
-void run_threads(unsigned nblocks, unsigned nthreads, K kernel) {  // kernels without barriers: one thread at a time
-  blockDim.x = nthreads;
-  gridDim.x = nblocks;
-  for (unsigned b = 0; b < nblocks; b++)
-    for (unsigned t = 0; t < nthreads; t++) {
-      blockIdx.x = b;
-      threadIdx.x = t;
-      kernel();
-    }
-}
-inline unsigned cdiv(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 
+// ---- a whole MSM through the library's engine (msm_host.cuh: msm_enqueue — digit recode, counting sort, slice
+// tables, bucket accumulation (batched-affine rounds when S != 0, else the XYZZ kernel with 2, 4 or 8 lanes per slice),
+// slice merge, bucket tail) over a base set built as bases_create builds it, then k_finalize.  G1 runs the staged
+// backward pass in every round (B200_CFG_TMA_STAGING 1), G2 from round 2 on (2).
 template <class F>
-int msm_full(const uint32_t* jac_std, const uint32_t* scalars_std, uint32_t n, uint32_t c, uint32_t S, uint32_t* out_std) {
-  MsmShape sh{n, c, (255 + c - 1) / c, 1u << (c - 1), n};
+int msm_full(int group, const uint32_t* jac_std, const uint32_t* scalars_std, uint32_t n, uint32_t c, uint32_t S, uint32_t* out_std) {
   int err = 0;
-  // --- bases_create: table[w][i] = 2^(c w) P_i
-  std::vector<F> staging((size_t)n * 3);
-  std::memcpy(staging.data(), jac_std, staging.size() * sizeof(F));
-  std::vector<Affine<F>> table((size_t)sh.nwin * n);
-  std::vector<XYZZ<F>> state(n);
-  run_threads(cdiv(n, 128), 128, [&] { k_load_bases<F>(staging.data(), n, table.data(), &err); });
-  run_threads(cdiv(n, 128), 128, [&] { k_affine_to_xyzz<F>(table.data(), state.data(), n); });
-  for (uint32_t w = 1; w < sh.nwin; w++) {
-    run_threads(cdiv(n, 128), 128, [&] { k_window_step<F>(state.data(), n, (int)c); });
-    run_threads(cdiv(cdiv(n, 8), 128), 128, [&] { k_batch_to_affine<F, 8>(state.data(), table.data() + (size_t)w * n, n); });
-  }
-  // --- msm_sort
-  uint32_t m = sh.nbuckets + 1;
-  uint64_t total = (uint64_t)sh.nwin * n;
-  uint64_t mean = (total + sh.nbuckets - 1) / sh.nbuckets;
-  const uint32_t kLPBh = 8;
-  uint32_t cap = (uint32_t)(2 * mean < 4 * kLPBh ? 4 * kLPBh : 2 * mean);
-  int fixed = 0;
-  if (S) {
-    cap = S;
-    fixed = 1;
-  }
-  size_t max_slices = sh.nbuckets + total / (S ? S : cap) + 8 + (S ? 0 : sh.nbuckets);
+  Bases b;
+  int rc = make_bases<F>(b, group, jac_std, n, c, 0, S, &err);
+  if (rc) return rc;
   std::vector<Fr> scalars(n);
   std::memcpy(scalars.data(), scalars_std, (size_t)n * sizeof(Fr));
-  std::vector<uint32_t> counts(m + 1, 0), offsets(m + 1, 0), cursor(m + 1, 0), entries(total + 8, 0);
-  std::vector<uint32_t> slice_off(m + 2, 0), slice_start(max_slices, 0), slice_end(max_slices, 0);
-  SliceTables stb{slice_off.data(), slice_start.data(), slice_end.data()};
-  run_threads(cdiv(n, 256), 256, [&] { k_digits_count(scalars.data(), sh, 0, counts.data(), &err); });
-  run_cta(0, 256, 1, [&] { k_scan(counts.data(), m, cap, fixed, offsets.data(), cursor.data(), stb); });
-  run_threads(cdiv(m, 256), 256, [&] { k_fill_slices(counts.data(), offsets.data(), m, cap, fixed, stb); });
-  run_threads(cdiv(n, 256), 256, [&] { k_digits_scatter(scalars.data(), sh, 0, cursor.data(), entries.data(), &err); });
+  XYZZ<F> rec;
+  if (msm_enqueue<F>(test_env(group == 1 ? 1 : 2), &b, scalars.data(), n, 0, &rec, &err, nullptr)) return 95;
   if (err) return 100 + err;
-  uint32_t nslices = slice_off[m];
-  if (nslices > max_slices) return 99;
-  // --- msm_buckets
-  std::vector<XYZZ<F>> buckets(sh.nbuckets);
-  if (S) {
-    uint32_t R = 0;
-    while ((1u << R) < S) R++;
-    constexpr int T = 8;
-    const size_t cap = (size_t)nslices * (S / 2) + 1;
-    std::vector<F> bufA(2 * cap), bufB(2 * cap);      // x | y halves (NodeBuf)
-    std::vector<F> pre((size_t)nslices * (S / 2) + 1);
-    std::vector<uint2> ids((size_t)nslices * (S / 2) + 1);
-    unsigned nb_max = cdiv((size_t)nslices * (S / 2), kAffBlock * T) + 1;
-    std::vector<F> others((size_t)nb_max * kAffBlock), btot(nb_max);
-    AffineRound<F> ar{};
-    ar.table = table.data();
-    ar.entries = entries.data();
-    ar.slice_start = slice_start.data();
-    ar.slice_end = slice_end.data();
-    ar.nslices_ptr = slice_off.data() + m;
-    ar.pre = pre.data();
-    ar.others = others.data();
-    ar.btot = btot.data();
-    ar.pair_ids = ids.data();
-    NodeBuf<F> prev{nullptr, nullptr};
-    NodeBuf<F> bufs[2] = {{bufA.data(), bufA.data() + cap}, {bufB.data(), bufB.data() + cap}};
-    for (uint32_t r = 1; r <= R; r++) {
-      ar.round = r;
-      ar.q_log = R - r;
-      ar.prev = prev;
-      ar.out = bufs[(r - 1) & 1];
-      unsigned nb = cdiv((size_t)nslices << ar.q_log, kAffBlock * T);
-      if (nb == 0) nb = 1;
-      for (unsigned b = 0; b < nb; b++) run_cta(b, kAffBlock, nb, [&] { k_affine_forward<F, T, 1>(ar); });
-      for (unsigned b = 0; b < cdiv((size_t)nb * 32, 128); b++) run_cta(b, 128, cdiv((size_t)nb * 32, 128), [&] { k_affine_invert<F>(ar.btot, nb); });
-      run_backward<F, T>(1, ar, nb);   // the staged kernel, as the library launches it
-      prev = ar.out;
-    }
-    for (unsigned b = 0; b < cdiv(sh.nbuckets, 128); b++)
-      run_cta(b, 128, cdiv(sh.nbuckets, 128), [&] { k_merge_slices_affine<F>(prev, stb, sh.nbuckets, buckets.data()); });
-  } else {
-    std::vector<XYZZ<F>> slice_out(max_slices);
-    unsigned nb = cdiv((size_t)max_slices * 4, 128);
-    for (unsigned b = 0; b < nb; b++) run_cta(b, 128, nb, [&] { k_accumulate<F, 4>(table.data(), entries.data(), stb, m, slice_out.data()); });
-    for (unsigned b = 0; b < cdiv(sh.nbuckets, 128); b++)
-      run_cta(b, 128, cdiv(sh.nbuckets, 128), [&] { k_merge_slices<F>(slice_out.data(), stb, sh.nbuckets, buckets.data()); });
-  }
-  XYZZ<F> total_pt;
-  if (c >= 7) {
-    const uint32_t bits = c - 1, kl = (bits + 1) / 2, kh = bits - kl, K = 1u << kl, H = 1u << kh;
-    std::vector<XYZZ<F>> scratch((size_t)H + K + bits + 1);
-    XYZZ<F>*Rr = scratch.data(), *Cc = Rr + H, *planes = Cc + K;
-    unsigned nb1 = cdiv((size_t)(H + K) * 32, 128), nb2 = cdiv((size_t)(bits + 1) * 32, 128);
-    for (unsigned b = 0; b < nb1; b++) run_cta(b, 128, nb1, [&] { k_tail_rowcol<F>(buckets.data(), kl, H, Rr, Cc); });
-    for (unsigned b = 0; b < nb2; b++) run_cta(b, 128, nb2, [&] { k_tail_planes<F>(Rr, Cc, kl, kh, planes); });
-    run_cta(0, 32, 1, [&] { k_tail_horner<F>(planes, bits, &total_pt); });
-  } else {
-    uint32_t seg = sh.nbuckets >= 256 ? 4 : 1, nseg = (sh.nbuckets + seg - 1) / seg;
-    std::vector<XYZZ<F>> partials((size_t)nseg + 1024);
-    for (unsigned b = 0; b < cdiv(nseg, 128); b++)
-      run_cta(b, 128, cdiv(nseg, 128), [&] { k_bucket_reduce<F>(buckets.data(), sh.nbuckets, seg, partials.data(), nseg); });
-    run_cta(0, 256, 1, [&] { k_sum_points<F>(partials.data(), nseg, nseg, &total_pt); });
-  }
-  F out[3];
-  run_cta(0, 32, 1, [&] { k_finalize<F>(&total_pt, out); });
-  std::memcpy(out_std, out, sizeof out);
+  if ((rc = check_sort(b.sort, b.sh))) return rc;
+  finalize_std<F>(rec, out_std);
   return 0;
 }
 // out = a * b over F_r with the NTT kernels, in the order of PolyCtx::forward / pointwise / inverse_unscaled
@@ -466,9 +426,11 @@ int ntt_compare(const uint32_t* in_std, int logn, int dit, int max_k, uint32_t* 
 }
 }  // namespace
 
-template <class K> void stub_launch_threads(unsigned nblocks, unsigned nthreads, K k) { run_threads(nblocks, nthreads, k); }
-template <class K> void stub_launch_cta(unsigned nblocks, unsigned nthreads, K k) {
-  for (unsigned b = 0; b < nblocks; b++) run_cta(b, nthreads, nblocks, k);
+template <class K> void stub_launch_threads(dim3 grid, unsigned nthreads, K k) { run_threads(grid, nthreads, k); }
+template <class K> void stub_launch_cta(dim3 grid, unsigned nthreads, size_t smem, K k) {
+  std::vector<uint8_t> shared(smem ? smem + 128 : 0);
+  for (unsigned y = 0; y < grid.y; y++)
+    for (unsigned b = 0; b < grid.x; b++) run_cta(b, nthreads, grid.x, k, y, grid.y, smem ? shared.data() : nullptr);
 }
 
 namespace {
@@ -565,9 +527,10 @@ int t_ntt_compare(const uint32_t* in_std, int logn, int dit, int max_k, uint32_t
 int t_poly_mul_kernels(const uint32_t* a, uint32_t la, const uint32_t* b, uint32_t lb, uint32_t* out) {
   return poly_mul_kernels(a, la, b, lb, out);
 }
-// sum_i scalars[i] * P_i through every kernel of the pipeline; S = 0: XYZZ accumulation, else batched-affine slices of S
+// sum_i scalars[i] * P_i through the library's MSM engine; S = 0: XYZZ accumulation, else batched-affine slices of S
 int t_msm_full(int group, const uint32_t* jac_std, const uint32_t* scalars_std, uint32_t n, uint32_t c, uint32_t S, uint32_t* out_std) {
-  return group == 1 ? msm_full<Fq>(jac_std, scalars_std, n, c, S, out_std) : msm_full<Fq2>(jac_std, scalars_std, n, c, S, out_std);
+  return group == 1 ? msm_full<Fq>(group, jac_std, scalars_std, n, c, S, out_std)
+                    : msm_full<Fq2>(group, jac_std, scalars_std, n, c, S, out_std);
 }
 // glv.cuh on a 32-thread emulated warp: lanes 0..15 compute k0 * P0, lanes 16..31 k1 * P1 — the two half-warps of
 // k_groth16_products / k_ic_terms — with the scalars split by glv_decompose exactly as the host side of the library does.

@@ -22,12 +22,24 @@
 
 struct Dim3Stub { unsigned x = 0, y = 0, z = 0; };
 inline thread_local Dim3Stub threadIdx, blockIdx, blockDim, gridDim;
+struct dim3 {   // launch grids (the emulated launches take x and y)
+  unsigned x, y, z;
+  dim3(unsigned x_ = 1, unsigned y_ = 1, unsigned z_ = 1) : x(x_), y(y_), z(z_) {}
+};
 struct uint2 { unsigned x, y; };
 inline uint2 make_uint2(unsigned x, unsigned y) { return uint2{x, y}; }
 typedef void* cudaStream_t;
-// just enough of the runtime API for the host orchestration of poly_host.cuh / qap_sparse.cuh (device memory = heap)
+// just enough of the runtime API for the host orchestration of poly_host.cuh / qap_sparse.cuh / msm_host.cuh (device
+// memory = heap; launches and copies are synchronous, so events order nothing)
 typedef int cudaError_t;
 constexpr cudaError_t cudaSuccess = 0;
+typedef void* cudaEvent_t;
+constexpr unsigned cudaEventDisableTiming = 2;
+inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { static char token; *e = &token; return 0; }
+inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t = nullptr) { return 0; }
+inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return 0; }
+inline cudaError_t cudaEventDestroy(cudaEvent_t) { return 0; }
+inline cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned = 0) { return 0; }
 enum cudaMemcpyKind { cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice };
 inline cudaError_t cudaMalloc(void** p, size_t b) { *p = std::malloc(b ? b : 1); return *p ? 0 : 2; }
 template <class T> inline cudaError_t cudaMalloc(T** p, size_t b) { return cudaMalloc(reinterpret_cast<void**>(p), b); }

@@ -1,9 +1,9 @@
-"""CPU: batches of MSMs over one base set (b200_msm_device_batch) through every kernel on the CPU emulation
-(tests/host/batch_msm_test.cpp, csrc/host_stub): the batched signed-digit recode and counting sort over k*G*2^(c-1)
-buckets, the multi-block counter scan, both accumulation kernels, the slice merge and the per-vector tails.  Every record
-is the oracle's sum_i s_(p,i) * P_i, for G1 and G2, k in {1, 2, 5}, t in {1, 2, nwin} and c below and above the c = 7
-switch between the segment tail and the rows / columns / planes tail.  k = 1 through the batch sequence leaves the same
-offsets, slice tables, sorted entries, buckets and record as the one-MSM sequence."""
+"""CPU: batches of MSMs over one base set (b200_msm_device_batch) through the library's MSM engine (msm_host.cuh:
+msm_batch_enqueue) on the CPU emulation (tests/host/batch_msm_test.cpp, csrc/host_stub): the batched signed-digit recode
+and counting sort over k*G*2^(c-1) buckets, the multi-block counter scan, both accumulation kernels, the slice merge and
+the per-vector tails.  Every record is the oracle's sum_i s_(p,i) * P_i, for G1 and G2, k in {1, 2, 5}, t in {1, 2, nwin}
+and c below and above the c = 7 switch between the segment tail and the rows / columns / planes tail.  k = 1 through the
+batch path leaves the same offsets, slice tables, sorted entries, buckets and record as the one-MSM path (msm_enqueue)."""
 import ctypes
 import random
 
@@ -158,7 +158,7 @@ def test_tail_launches_split_into_row_chunks(lib, group, c, S, t, max_rows):
                                                (2, 5, 0, "1"), (2, 7, 0, "nwin")])
 @pytest.mark.parametrize("scan_chunk", [0, 300])
 def test_single_vector_batch_is_bit_identical(lib, group, c, S, which_t, scan_chunk):
-    """k = 1 through the batch sequence, with one scan block or several, against the one-MSM sequence: the same
+    """k = 1 through the engine's batch path, with one scan block or several, against its one-MSM path: the same
     offsets, slice tables, sorted entries and buckets byte for byte, and the same record (byte for byte where the tail
     launches are the same, c >= 7; the same point for c < 7, whose tree sum differs in shape)."""
     nwin = (255 + c - 1) // c

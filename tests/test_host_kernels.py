@@ -124,8 +124,9 @@ def test_g2_forward_kernel_cta_emulation(lib):
                                                 (1, 64, 0), (1, 128, 0), (1, 2048, 0), (2, 256, 0)])
 def test_msm_tail_kernels(lib, group, nbuckets, seg):
     """k_merge_slices_affine (thread-per-bucket path and the warp path for buckets with > 24 slices, ballot + shuffles),
-    k_bucket_reduce (running sums + small scalar multiple per segment), k_sum_points (one and two levels) and k_finalize:
-    sum_b b * (sum of the slices of bucket b) against the oracle."""
+    then the engine's tails (msm_host.cuh): launch_segment_tail — k_bucket_reduce (running sums + small scalar multiple per
+    segment), launch_tree_sum (one and two levels) — or launch_bucket_tail, and k_finalize: sum_b b * (sum of the slices
+    of bucket b) against the oracle."""
     G = o.BN.G1 if group == 1 else o.BN.G2
     rng = random.Random(50 + nbuckets)
     zero = (0, 0) if group == 1 else ((0, 0), (0, 0))
@@ -168,9 +169,10 @@ def test_msm_tail_kernels(lib, group, nbuckets, seg):
                                          # ~17 slices per bucket: above the old thread-path bound of k_merge_slices_affine (12), inside the new one (24)
                                          (1, 100, 6, 8), (2, 110, 6, 8)])
 def test_whole_msm_pipeline_on_the_cpu(lib, group, n, c, S):
-    """Every kernel of an MSM in the library's order (window precompute, signed-digit recode, counting sort, slice tables,
-    bucket accumulation in both modes, slice merge, weighted bucket reduction, tree sum, normalisation) on the CPU
-    emulation == sum_i s_i * P_i by the oracle.  Scalars include 0, 1, r - 1, small values and repeated points."""
+    """The library's own MSM engine (msm_host.cuh: window precompute, signed-digit recode, counting sort, slice tables,
+    bucket accumulation in both modes — the batched-affine rounds with the staged backward pass, the XYZZ kernel with the
+    lanes per slice it picks —, slice merge, bucket tail) and k_finalize on the CPU emulation == sum_i s_i * P_i by the
+    oracle.  Scalars include 0, 1, r - 1, small values and repeated points."""
     G = o.BN.G1 if group == 1 else o.BN.G2
     rng = random.Random(1000 * group + n + c)
     ks = [rng.randrange(1, R_) for _ in range(n)]

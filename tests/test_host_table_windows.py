@@ -1,5 +1,5 @@
-"""CPU: MSMs over reduced window tables (B200_CFG_TABLE_WINDOWS) through every kernel on the CPU emulation
-(tests/host/table_windows_test.cpp, csrc/host_stub): the library's table build with t rows, the grouped signed-digit recode
+"""CPU: MSMs over reduced window tables (B200_CFG_TABLE_WINDOWS) through the library's MSM engine (msm_host.cuh) on the
+CPU emulation (tests/host/table_windows_test.cpp, csrc/host_stub): the library's table build with t rows, the grouped signed-digit recode
 and counting sort, both accumulation kernels, the grouped tails and the Horner chain over all window groups.  Every result
 is the oracle's sum_i s_i * P_i, for G1 and G2, t in {1, 2, 5, nwin - 1, nwin} and c below and above the c = 7 switch
 between the segment tail and the rows / columns / planes tail."""
