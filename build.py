@@ -212,6 +212,18 @@ def build_host_verify_batch(force=False):
     return target
 
 
+def build_host_pinocchio_verify_batch(force=False):
+    """g++ build of the batched Pinocchio verifier's kernels (classification, the reference sums S_i and T_i, the aggregate
+    in launch order) over csrc/host_stub (CPU test vehicle, tests/test_host_pinocchio_verify_batch.py)."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    target = os.path.join(LIBDIR, "libb200_host_pinocchio_verify_batch.so")
+    if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):
+        return target
+    _run(["g++", "-O2", "-std=c++17", "-pthread", "-x", "c++", "-shared", "-fPIC", "-Wno-psabi", "-I", os.path.join(HOSTTEST, "host_stub"),
+          "-I", HOSTTEST, "-I", CSRC, "-o", target, os.path.join(HOSTTEST, "pinocchio_verify_batch_test.cpp")])
+    return target
+
+
 def build_shard_partition(force=False):
     """g++ build of csrc/shard_partition.h behind a C entry point (CPU test vehicle, tests/test_shard_partition.py)."""
     os.makedirs(LIBDIR, exist_ok=True)

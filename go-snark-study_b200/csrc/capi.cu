@@ -31,6 +31,7 @@
 #include "pairing.cuh"
 #include "pairing_warp.cuh"
 #include "verify_batch.cuh"
+#include "verify_batch_pinocchio.cuh"
 #endif
 
 using namespace b200;
@@ -1211,6 +1212,52 @@ __global__ void __launch_bounds__(128) k_vb_verify_each(const uint64_t* proofs, 
   const Fq2* g2 = warp == 0 ? v.b : (warp == 1 ? vk->beta : (warp == 2 ? vk->gamma : vk->delta));
   groth16_verify_cta(wss, g1, g2, ok + p, err);
 }
+// snark.VerifyProof over a batch, one CTA per proof (verify_batch_pinocchio.cuh): a regular proof under a passed aggregate
+// is accepted at once, a bad one (coordinate >= q, signal >= r, PiB at infinity) gets 0, every other proof the reference's
+// verdict: its twelve pairings (warp w runs pairings 3w .. 3w + 2 with warp_pairing_inputs' semantics), the two F_q^12
+// products e7 e8 and e9 e10, and the five comparisons of snark.go:292-372.
+__global__ void __launch_bounds__(128) k_pvb_verify_each(const uint64_t* proofs, const vb::PVk* vk, const Fq* st,
+                                                         const uint32_t* flags, const uint32_t* agg, size_t k, int* ok,
+                                                         uint32_t* status, int* err) {
+  __shared__ wp::Ws wss[4];
+  __shared__ F2 e[vb::kPvbPairings][6];
+  const size_t p = blockIdx.x;
+  const uint32_t f = flags[p] | flags[k];
+  if ((f & vb::kBad) || (!f && *agg)) {
+    if (threadIdx.x == 0) ok[p] = (f & vb::kBad) ? 0 : 1;
+    return;
+  }
+  if (threadIdx.x == 0) atomicOr(status, vb::kStPerProof);
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  wp::Ws& ws = wss[warp];
+  for (int j = 3 * (int)warp; j < 3 * (int)warp + 3; j++) {
+    F2::B px, py;
+    F2 qx, qy;
+    if (warp_pairing_inputs(ws, vb::pvb_pairing_g1(proofs, vk, st, p, j), vb::pvb_pairing_g2(proofs, vk, p, j), px, py, qx, qy, err))
+      wp::pairing(ws, px, py, qx, qy);
+    else
+      wp::f12_set_one(ws, wp::RF);
+    if (lane < 6) e[j][lane] = ws.r[wp::RF][lane];
+    wp::wsync();
+  }
+  __syncthreads();
+  if (warp != 0) return;
+  if (lane < 6) {
+    ws.r[2][lane] = e[7][lane];
+    ws.r[3][lane] = e[8][lane];
+    ws.r[4][lane] = e[9][lane];
+    ws.r[5][lane] = e[10][lane];
+  }
+  wp::wsync();
+  wp::f12_mul(ws, 2, 2, 3);   // e(PiH, Vkz) e(PiC, g2)
+  wp::f12_mul(ws, 4, 4, 5);   // e(T, G2Kbg) e(G1Kbg, PiB)
+  int same = 1;
+  if (lane < 6)
+    same = e[0][lane] == e[1][lane] && e[2][lane] == e[3][lane] && e[4][lane] == e[5][lane] && e[6][lane] == ws.r[2][lane] &&
+           ws.r[4][lane] == e[11][lane];
+  const unsigned all = __ballot_sync(0xffffffffu, same);
+  if (lane == 0) ok[p] = all == 0xffffffffu ? 1 : 0;
+}
 // icPubl = IC[0] + sum publicSignals[i] * IC[i+1] (groth16.go:283-286).  The products are independent: one half-warp each,
 // with the GLV split of prove_host.cuh (128 doublings + ~12 additions deep instead of the 254 + ~127 of MulScalar's
 // double-and-add; the same group element, which is all the pairing — it normalises its inputs — can see); the sum then runs
@@ -1494,6 +1541,160 @@ int groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t*
                               (int*)d_ok, (uint32_t*)((int*)d_ok + k), d + vkb, st);
 }
 
+// ---- batched Pinocchio verification (verify_batch_pinocchio.cuh) ------------------------------------------------------
+// per-call scratch of pvb_enqueue, carved from one allocation
+struct PvbScratch {
+  size_t off[10];
+  size_t bytes;
+  PvbScratch(size_t k, size_t npub) {
+    const size_t n = k + vb::kPvbSums, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
+    const size_t sz[10] = {(k + 1) * 4, 4, 4, 4, 6 * k * sizeof(Fq), (npub ? npub * k : 1) * sizeof(Jacobian<Fq>),
+                           vb::kPvbRhoTerms * k * sizeof(Jacobian<Fq>), vb::kPvbSums * sizeof(Jacobian<Fq>),
+                           6 * n * sizeof(F2), 6 * nparts * sizeof(F2)};
+    bytes = 0;
+    for (int i = 0; i < 10; i++) {
+      off[i] = bytes;
+      bytes += (sz[i] + 255) & ~(size_t)255;
+    }
+  }
+};
+// Every launch of a batched Pinocchio verification, on `st`: d_ok[0..k) verdicts, *d_status the status bits (zeroed here
+// first).  A fixed launch sequence: no step waits for the host, whatever k and whatever the outcome.
+int pvb_enqueue(const Fq* d_ic, const vb::PVk* d_vk, const uint64_t* d_proofs, const uint64_t* d_pub, size_t npub, size_t k,
+                const uint64_t* d_rho, int* d_ok, uint32_t* d_status, uint8_t* scratch, cudaStream_t st) {
+  const PvbScratch L(k, npub);
+  uint32_t* flags = (uint32_t*)(scratch + L.off[0]);
+  uint32_t* k_reg = (uint32_t*)(scratch + L.off[1]);
+  uint32_t* agg = (uint32_t*)(scratch + L.off[2]);
+  int* err = (int*)(scratch + L.off[3]);
+  Fq* sts = (Fq*)(scratch + L.off[4]);
+  Jacobian<Fq>* terms = (Jacobian<Fq>*)(scratch + L.off[5]);
+  Jacobian<Fq>* rterms = (Jacobian<Fq>*)(scratch + L.off[6]);
+  Jacobian<Fq>* sums = (Jacobian<Fq>*)(scratch + L.off[7]);
+  F2* mvals = (F2*)(scratch + L.off[8]);
+  F2* parts = (F2*)(scratch + L.off[9]);
+  const size_t n = k + vb::kPvbSums, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
+  CU(cudaMemsetAsync(scratch, 0, L.off[4], st));
+  CU(cudaMemsetAsync(d_status, 0, sizeof(uint32_t), st));
+  vb::k_pvb_classify<<<nblk(k + 7, 64), 64, 0, st>>>(d_proofs, d_vk, k, flags, d_status);
+  if (npub) vb::k_vb_ic_terms<<<nblk(npub * k, 2), 32, 0, st>>>(d_ic, d_pub, npub, k, terms, flags, d_status);
+  vb::k_pvb_st<<<nblk(k, 64), 64, 0, st>>>(d_ic, terms, d_proofs, npub, k, sts, flags, d_status);
+  vb::k_pvb_rho_terms<<<nblk(vb::kPvbRhoTerms * k, 2), 32, 0, st>>>(d_proofs, d_vk, sts, d_rho, k, rterms);
+  vb::k_pvb_sums<<<vb::kPvbSums, vb::kSumThreads, 0, st>>>(rterms, flags, k, sums, k_reg);
+  const vb::PvbMlArgs ma{d_proofs, d_vk, rterms, sums, flags, k_reg, k};
+  // the kernel rule of b200_pairing_batch (B200_CFG_PAIRING_KERNEL; auto: a warp per pair up to 2048 pairs)
+  const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
+  if (thread_kernel) vb::k_vb_miller_thread<<<nblk(n, 32), 32, 0, st>>>(ma, n, mvals);
+  else vb::k_vb_miller_warp<<<nblk(n, vb::kMlWarps), 32 * vb::kMlWarps, 0, st>>>(ma, n, mvals);
+  vb::k_vb_product<<<(unsigned)nparts, 32 * vb::kProdWarps, 0, st>>>(mvals, n, parts);
+  vb::k_vb_final<<<1, 32 * vb::kProdWarps, 0, st>>>(parts, nparts, k_reg, agg, d_status);
+  k_pvb_verify_each<<<(unsigned)k, 128, 0, st>>>(d_proofs, d_vk, sts, flags, agg, k, d_ok, d_status, err);
+  g_launches += npub ? 9 : 8;
+  CU(cudaGetLastError());
+  return B200_OK;
+}
+// The checks both entries make on the host arguments of the Vk, IC and rho.
+int pvb_check_vk(const char* what, const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2, size_t npub,
+                 size_t k, const uint64_t* rho) {
+  if (!ic || !vk_g1 || !vk_g2 || !rho) return fail(B200_EINVAL, "%s: null pointer", what);
+  if (n_ic < npub + 1) return fail(B200_EINVAL, "%s: len(IC) < len(publicSignals) + 1", what);
+  if (k == 0 || k > vb::kMaxBatch) return fail(B200_EINVAL, "%s: k = %zu outside 1..%zu", what, k, vb::kMaxBatch);
+  for (size_t i = 0; i < 5 * k; i++)
+    if (!(rho[2 * i] | rho[2 * i + 1])) return fail(B200_EINVAL, "%s: rho[%zu][%zu] = 0", what, i / 5, i % 5 + 1);
+  for (size_t i = 0; i < 3 * n_ic; i++)
+    if (fq_load_std(ic + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: IC coordinate >= q", what);
+  for (int i = 0; i < 6; i++)
+    if (fq_load_std(vk_g1 + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: Vk G1 coordinate >= q", what);
+  for (int i = 0; i < 30; i++)
+    if (fq_load_std(vk_g2 + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: Vk G2 coordinate >= q", what);
+  for (int c = 0; c < 5; c++) {
+    const uint64_t* z = vk_g2 + 24 * c + 16;
+    if (!(z[0] | z[1] | z[2] | z[3] | z[4] | z[5] | z[6] | z[7]))
+      return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (Vk G2 point at infinity; the reference panics, bn128.go:238-241)", what);
+  }
+  return B200_OK;
+}
+// device image of the Vk, IC and rho: vb::PVk | IC | rho
+size_t pvb_vk_bytes(size_t n_ic, size_t k) { return sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq) + 10 * k * sizeof(uint64_t); }
+int pvb_upload_vk(uint8_t* d, const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2, size_t k,
+                  const uint64_t* rho, cudaStream_t st) {
+  static_assert(sizeof(vb::PVk) == (24 + 120 + 24) * sizeof(uint64_t), "PVk is vk_g1 | vk_g2 | g2");
+  std::vector<uint8_t> h(pvb_vk_bytes(n_ic, k));
+  std::memcpy(h.data(), vk_g1, 24 * sizeof(uint64_t));
+  std::memcpy(h.data() + 24 * sizeof(uint64_t), vk_g2, 120 * sizeof(uint64_t));
+  std::memcpy(h.data() + 144 * sizeof(uint64_t), kG2GenJacStd, 24 * sizeof(uint64_t));
+  std::memcpy(h.data() + sizeof(vb::PVk), ic, n_ic * 3 * sizeof(Fq));
+  std::memcpy(h.data() + sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq), rho, 10 * k * sizeof(uint64_t));
+  CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+  return B200_OK;
+}
+int pinocchio_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2,
+                                const uint64_t* out_g1, const uint64_t* pi_b, const uint64_t* pub, size_t npub, size_t k,
+                                const uint64_t* rho, int* ok, uint32_t* status) {
+  const char* what = "pinocchio_verify_batch";
+  if (!out_g1 || !pi_b || !ok || (npub && !pub)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = pvb_check_vk(what, ic, n_ic, vk_g1, vk_g2, npub, k, rho);
+  if (rc) return rc;
+  for (size_t i = 0; i < k * npub; i++)
+    if (fr_load_std(pub + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: scalar / coefficient >= r", what);
+  // the batch prover's device layout: the seven G1 points, then PiB, per proof
+  std::vector<uint64_t> proofs(vb::kPvbProofWords * k);
+  for (size_t p = 0; p < k; p++) {
+    std::memcpy(&proofs[vb::kPvbProofWords * p], out_g1 + 84 * p, 84 * sizeof(uint64_t));
+    std::memcpy(&proofs[vb::kPvbProofWords * p + 84], pi_b + 24 * p, 24 * sizeof(uint64_t));
+  }
+  for (size_t i = 0; i < 27 * k; i++)
+    if (fq_load_std(&proofs[4 * i]).geq_modulus()) return fail(B200_ERANGE, "%s: point coordinate >= q", what);
+  for (size_t p = 0; p < k; p++) {
+    const uint64_t* z = &proofs[vb::kPvbProofWords * p + 100];
+    if (!(z[0] | z[1] | z[2] | z[3] | z[4] | z[5] | z[6] | z[7]))
+      return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (PiB of proof %zu at infinity; the reference panics, bn128.go:238-241)", what, p);
+  }
+  cudaStream_t st = g_ctx[0].main;
+  const size_t vkb = pvb_vk_bytes(n_ic, k), pb = proofs.size() * sizeof(uint64_t), ub = (npub ? npub : 1) * k * 32,
+               okb = (k + 1) * sizeof(int);
+  const PvbScratch L(k, npub);
+  StreamBuf buf;
+  CU(buf.alloc(vkb + pb + ub + okb + L.bytes + 1024, st));
+  uint8_t* d = (uint8_t*)buf.p;
+  auto carve = [&](size_t b) { uint8_t* r = d; d += (b + 255) & ~(size_t)255; return r; };
+  uint8_t* d_vk = carve(vkb);
+  uint64_t* d_proofs = (uint64_t*)carve(pb);
+  uint64_t* d_pub = (uint64_t*)carve(ub);
+  int* d_ok = (int*)carve(okb);
+  uint8_t* d_scratch = carve(L.bytes);
+  if ((rc = pvb_upload_vk(d_vk, ic, n_ic, vk_g1, vk_g2, k, rho, st))) return rc;
+  CU(cudaMemcpyAsync(d_proofs, proofs.data(), pb, cudaMemcpyHostToDevice, st));
+  if (npub) CU(cudaMemcpyAsync(d_pub, pub, npub * k * 32, cudaMemcpyHostToDevice, st));
+  const Fq* d_ic = (const Fq*)(d_vk + sizeof(vb::PVk));
+  const uint64_t* d_rho = (const uint64_t*)(d_vk + sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq));
+  if ((rc = pvb_enqueue(d_ic, (const vb::PVk*)d_vk, d_proofs, d_pub, npub, k, d_rho, d_ok, (uint32_t*)(d_ok + k), d_scratch, st)))
+    return rc;
+  std::vector<int> h_ok(k + 1);
+  CU(cudaMemcpyAsync(h_ok.data(), d_ok, okb, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  std::memcpy(ok, h_ok.data(), k * sizeof(int));
+  if (status) *status = (uint32_t)h_ok[k];
+  return B200_OK;
+}
+int pinocchio_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2,
+                                  const void* d_proofs, const void* d_public, size_t npub, size_t k, const uint64_t* rho,
+                                  void* d_ok, cudaStream_t st) {
+  const char* what = "pinocchio_verify_batch_device";
+  if (!d_proofs || !d_ok || (npub && !d_public)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = pvb_check_vk(what, ic, n_ic, vk_g1, vk_g2, npub, k, rho);
+  if (rc) return rc;
+  const size_t vkb = (pvb_vk_bytes(n_ic, k) + 255) & ~(size_t)255;
+  const PvbScratch L(k, npub);
+  StreamBuf buf;
+  CU(buf.alloc(vkb + L.bytes, st));
+  uint8_t* d = (uint8_t*)buf.p;
+  if ((rc = pvb_upload_vk(d, ic, n_ic, vk_g1, vk_g2, k, rho, st))) return rc;
+  return pvb_enqueue((const Fq*)(d + sizeof(vb::PVk)), (const vb::PVk*)d, (const uint64_t*)d_proofs, (const uint64_t*)d_public,
+                     npub, k, (const uint64_t*)(d + sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq)), (int*)d_ok,
+                     (uint32_t*)((int*)d_ok + k), d + vkb, st);
+}
+
 #else  // experiment builds without the verifier side (ptxas 12.9 crashes on the pairing kernels under -DB200_KARATSUBA)
 int pairing_batch_host(const uint64_t*, const uint64_t*, size_t, uint64_t*) { return fail(B200_EINVAL, "pairing: not in this build variant"); }
 int groth16_verify_batch_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
@@ -1504,6 +1705,14 @@ int groth16_verify_batch_host(const uint64_t*, size_t, const uint64_t*, const ui
 int groth16_verify_batch_device(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
                                 const void*, const void*, size_t, size_t, const uint64_t*, void*, cudaStream_t) {
   return fail(B200_EINVAL, "groth16_verify_batch_device: not in this build variant");
+}
+int pinocchio_verify_batch_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
+                                const uint64_t*, size_t, size_t, const uint64_t*, int*, uint32_t*) {
+  return fail(B200_EINVAL, "pinocchio_verify_batch: not in this build variant");
+}
+int pinocchio_verify_batch_device(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const void*, const void*, size_t,
+                                  size_t, const uint64_t*, void*, cudaStream_t) {
+  return fail(B200_EINVAL, "pinocchio_verify_batch_device: not in this build variant");
 }
 int fq12_mul_batch_host(const uint64_t*, const uint64_t*, size_t, uint64_t*) { return fail(B200_EINVAL, "fq12_mul: not in this build variant"); }
 int groth16_verify_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
@@ -1938,6 +2147,19 @@ int b200_groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint
   NEED_INIT();
   return groth16_verify_batch_device(ic, n_ic, alpha1, beta2, gamma2, delta2, d_proofs, d_public, n_public, k, rho, d_ok,
                                      stream ? (cudaStream_t)stream : g_ctx[0].main);
+}
+int b200_pinocchio_verify_batch(const uint64_t* ic, size_t n_ic, const uint64_t vk_g1[24], const uint64_t vk_g2[120],
+                                const uint64_t* out_g1, const uint64_t* pi_b, const uint64_t* public_signals, size_t n_public,
+                                size_t k, const uint64_t* rho, int* ok, uint32_t* status) {
+  B200_API_BODY(pinocchio_verify_batch_host(ic, n_ic, vk_g1, vk_g2, out_g1, pi_b, public_signals, n_public, k, rho, ok, status))
+}
+int b200_pinocchio_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t vk_g1[24], const uint64_t vk_g2[120],
+                                       const void* d_proofs, const void* d_public, size_t n_public, size_t k, const uint64_t* rho,
+                                       void* d_ok, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  NEED_INIT();
+  return pinocchio_verify_batch_device(ic, n_ic, vk_g1, vk_g2, d_proofs, d_public, n_public, k, rho, d_ok,
+                                       stream ? (cudaStream_t)stream : g_ctx[0].main);
 }
 int b200_g1_add_batch(const uint64_t* p, const uint64_t* q, size_t n, uint64_t* out) { B200_API_BODY(group_op_host<Fq>(0, p, q, n, out)) }
 int b200_g1_double_batch(const uint64_t* p, size_t n, uint64_t* out) { B200_API_BODY(group_op_host<Fq>(1, p, nullptr, n, out)) }

@@ -266,8 +266,10 @@ DEV bool ml_pair(const MlArgs& a, size_t i, F2::B& px, F2::B& py, F2& qx, F2& qy
   qy = qa.y;
   return true;
 }
-// one warp per pair (wp::miller_loop); mvals: six F_q^2 per pair, Montgomery form
-__global__ void __launch_bounds__(32 * kMlWarps) k_vb_miller_warp(MlArgs a, size_t n, F2* mvals) {
+// one warp per pair (wp::miller_loop); mvals: six F_q^2 per pair, Montgomery form.  Args selects the pairs through its
+// ml_pair overload: MlArgs above, PvbMlArgs (verify_batch_pinocchio.cuh).
+template <class Args>
+__global__ void __launch_bounds__(32 * kMlWarps) k_vb_miller_warp(Args a, size_t n, F2* mvals) {
   __shared__ wp::Ws wss[kMlWarps];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   const size_t i = (size_t)blockIdx.x * kMlWarps + warp;
@@ -282,7 +284,8 @@ __global__ void __launch_bounds__(32 * kMlWarps) k_vb_miller_warp(MlArgs a, size
   if (lane < 6) mvals[6 * i + lane] = ws.r[wp::RF][lane];
 }
 // one thread per pair (miller_loop_affine)
-__global__ void __launch_bounds__(32) k_vb_miller_thread(MlArgs a, size_t n, F2* mvals) {
+template <class Args>
+__global__ void __launch_bounds__(32) k_vb_miller_thread(Args a, size_t n, F2* mvals) {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   F2::B px, py;

@@ -269,3 +269,63 @@ def VerifyProof(vk, proof, publicSignals, debug=False):
         if not ok:
             return False
     return True
+
+
+def _vk_args(vk):
+    return (_flatten_g1(vk["IC"]), _flatten_g1([vk["Vkb"], vk["G1Kbg"]]),
+            _flatten_g2([vk["Vka"], vk["Vkc"], vk["G2Kbg"], vk["G2Kg"], vk["Vkz"]]))
+
+
+def verify_batch_limbs(vk, proofs, publicSignalsList, rho=None):
+    """b200_pinocchio_verify_batch: (list of k verdicts, status word; its bits are groth16.VB_*).  ``rho``: 5k randomisers in 1..2^128 - 1, rho[5 i + c - 1]
+    for check c of proof i (drawn with groth16.draw_rho when None; pass them for reproducible runs)."""
+    import ctypes
+    from .groth16 import _rho_limbs, draw_rho
+    k = len(proofs)
+    if k == 0 or len(publicSignalsList) != k:
+        raise ValueError("verify_batch: need k >= 1 proofs and one publicSignals list per proof")
+    npub = len(publicSignalsList[0])
+    if any(len(ps) != npub for ps in publicSignalsList):
+        raise ValueError("verify_batch: every proof needs the same number of public signals")
+    rho = draw_rho(5 * k) if rho is None else list(rho)
+    if len(rho) != 5 * k:
+        raise ValueError("verify_batch: need five randomisers per proof")
+    ic, g1, g2 = _vk_args(vk)
+    out_g1 = _flatten_g1([p[s] for p in proofs for s in _ORDER])
+    pb = _flatten_g2([p["PiB"] for p in proofs])
+    pub = (ints_to_limbs([reduce_scalar(x) for ps in publicSignalsList for x in ps]) if npub
+           else np.zeros((1, 4), dtype=np.uint64))
+    ok = np.zeros(k, dtype=np.int32)
+    status = ctypes.c_uint32(0)
+    check(lib().b200_pinocchio_verify_batch(ptr(ic), len(vk["IC"]), ptr(g1), ptr(g2), ptr(out_g1), ptr(pb), ptr(pub), npub, k,
+                                            ptr(_rho_limbs(rho)), ptr(ok), ctypes.byref(status)))
+    return [bool(v) for v in ok], status.value
+
+
+def VerifyProofBatch(vk, proofs, publicSignalsList, rho=None):
+    """[snark.VerifyProof(vk, proofs[i], publicSignalsList[i]) for every i] in one call (b200_pinocchio_verify_batch): one
+    random linear combination of the five checks of the regular proofs, k + 6 Miller loops and one final exponentiation;
+    irregular proofs, and every proof of a batch whose combination fails, get VerifyProof's verdict.  ``rho`` defaults to
+    fresh 128-bit randomisers (secrets.randbits), five per proof, which is what makes an invalid proof's acceptance
+    improbable."""
+    return verify_batch_limbs(vk, proofs, publicSignalsList, rho)[0]
+
+
+def VerifyProofBatchDevice(vk, d_proofs, d_public, k, n_public, rho=None, d_ok=None, stream=None):
+    """b200_pinocchio_verify_batch_device on a batch in device memory: ``d_proofs`` is the output tensor of
+    b200_pinocchio_prove_witness_batch_device (k x 108 words: PiA, PiAp, PiBp, PiC, PiCp, PiH, PiKp, PiB), ``d_public`` the
+    k x n_public x 4 standard-form signals.  Queued on ``stream`` (a torch.cuda.Stream; None: the library's main stream)
+    without waiting; returns the int32 tensor of k verdicts followed by the status word (``d_ok``, allocated when None)."""
+    import torch
+    from .groth16 import _rho_limbs, draw_rho
+    rho = draw_rho(5 * k) if rho is None else list(rho)
+    if len(rho) != 5 * k:
+        raise ValueError("verify_batch: need five randomisers per proof")
+    if d_ok is None:
+        d_ok = torch.zeros(k + 1, dtype=torch.int32, device=d_proofs.device)
+    ic, g1, g2 = _vk_args(vk)
+    check(lib().b200_pinocchio_verify_batch_device(ptr(ic), len(vk["IC"]), ptr(g1), ptr(g2), d_proofs.data_ptr(),
+                                                   d_public.data_ptr() if n_public else None, n_public, k,
+                                                   ptr(_rho_limbs(rho)), d_ok.data_ptr(),
+                                                   None if stream is None else stream.cuda_stream))
+    return d_ok

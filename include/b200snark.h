@@ -71,7 +71,8 @@ int b200_version(void);
  * memory, 27 F_q^2 products of a tower multiplication on 27 lanes; csrc/pairing_warp.cuh); 0 = auto: a warp per
  * pairing up to 2048 pairings per call (latency), a thread per pairing above (throughput).
  * Bit-identical F_q^12 values.  b200_groth16_verify always runs four warps.  The same rule picks the Miller-loop
- * kernel of b200_groth16_verify_batch(_device) over its k_reg + 3 pairs.                                               */
+ * kernel of b200_groth16_verify_batch(_device) over its k_reg + 3 pairs and of b200_pinocchio_verify_batch(_device)
+ * over its k_reg + 6.                                                                                                  */
 #define B200_CFG_PAIRING_KERNEL 5
 /* Partition tuning of SHARDED proving keys loaded afterwards (defaults = the measured best for one proof at a time):
  * cost weight x100 of an A / B1 term (10) and of a G2 term (11) in C||PTD terms, and the
@@ -353,6 +354,49 @@ int b200_groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint
                                      const uint64_t gamma2[24], const uint64_t delta2[24], const void* d_proofs,
                                      const void* d_public, size_t n_public, size_t k, const uint64_t* rho, void* d_ok,
                                      void* stream);
+/* ok[i] = snark.VerifyProof(vk, proof_i, publicSignals_i) (snark.go:292-372) for k Pinocchio proofs under one Vk, by one
+ * random linear combination of the five checks of every proof (check c of proof i raised to rho_ic):
+ *   prod_i e(P_i, PiB_i) * e(sum rho_i1 PiA_i, Vka) * e(sum rho_i3 PiC_i, Vkc) * e(-sum rho_i4 PiH_i, Vkz)
+ *     * e(sum rho_i5 T_i, G2Kbg) * e(-sum rho_i5 PiKp_i, G2Kg)
+ *     * e(-sum (rho_i1 PiAp_i + rho_i2 PiBp_i + rho_i3 PiCp_i + rho_i4 PiC_i), g2) == 1,
+ *   P_i = rho_i2 Vkb + rho_i4 S_i + rho_i5 G1Kbg,
+ * over the REGULAR proofs: k_reg + 6 Miller loops, one F_q^12 product and ONE final exponentiation for the batch.
+ * Vkx_i = IC[0] + sum_j pub_ij IC[j+1], S_i = Add(Vkx_i, PiA_i) and T_i = Add(S_i, PiC_i) are the reference's sums, in its
+ * order and with its Add (no doubling branch: Vkx_i == PiA_i makes S_i infinity).
+ * A proof is regular when every G1 point one of its checks pairs (PiA, PiAp, PiBp, PiC, PiCp, PiH, PiKp, S_i, T_i) is on
+ * y^2 = x^3 + 3 and not infinity, and PiB is on the twist and in the order-r subgroup; under a Vk whose Vkb, G1Kbg (as G1
+ * points) or Vka, Vkc, G2Kbg, G2Kg, Vkz (as G2 points) fail the same tests no proof is regular.  The contract:
+ *   - every irregular proof gets exactly snark.VerifyProof's verdict (the reference pairs a G1 infinity as (0, 0), which
+ *     is not bilinear, so such proofs never enter the aggregate);
+ *   - when the aggregate fails, every proof gets exactly snark.VerifyProof's verdict (the per-proof check runs);
+ *   - when it passes, every regular proof is accepted.  A batch holding an invalid regular proof passes with probability
+ *     below 2^-127 over that proof's rho_ic, PROVIDED the randomisers are unpredictable to whoever made the proofs: draw
+ *     them from a cryptographic source per call.  The caller supplies them so that runs are reproducible.
+ * vk_g1 = Vkb | G1Kbg and vk_g2 = Vka | Vkc | G2Kbg | G2Kg | Vkz, as b200_pinocchio_setup / b200_pinocchio_setup_pk return
+ * them; ic = A[0..n_ic).  out_g1: k x 84 (PiA, PiAp, PiBp, PiC, PiCp, PiH, PiKp) and pi_b: k x 24, exactly
+ * b200_pinocchio_prove_witness_batch's outputs; public_signals: k x n_public x 4; standard-form Jacobian / scalars.
+ * rho: k x 5 x 2 limbs, rho[10 i + 2 (c - 1)] the low word of rho_ic, each 1 <= rho_ic < 2^128.  1 <= k <= 65536.
+ * status (may be NULL): bit 0 the aggregate ran over at least one proof and passed; bit 1 the per-proof check ran for
+ * some proof; bit 2 an irregular proof or Vk was routed around the aggregate.
+ * Errors: B200_ERANGE for a coordinate >= q (proofs, Vk, IC) or a public signal >= r; B200_EINVAL for PiB or a Vk G2 point
+ * at infinity (the reference panics, bn128.go:238-241), a null pointer, n_ic < n_public + 1, k outside 1..65536, or a
+ * rho_ic of 0.  Runs on context 0's main stream; synchronous.
+ * Launches: a fixed sequence of 9 kernels (8 when n_public = 0), whatever k and whatever the outcome.              */
+int b200_pinocchio_verify_batch(const uint64_t* ic, size_t n_ic, const uint64_t vk_g1[24], const uint64_t vk_g2[120],
+                                const uint64_t* out_g1, const uint64_t* pi_b, const uint64_t* public_signals, size_t n_public,
+                                size_t k, const uint64_t* rho, int* ok, uint32_t* status);
+/* b200_pinocchio_verify_batch on proofs already in device memory, queued on `stream` (NULL: context 0's main stream)
+ * without waiting: d_proofs is k x 108 uint64, the seven G1 points and then PiB per proof — exactly
+ * b200_pinocchio_prove_witness_batch_device's d_out, so a batch is verified where it lies; d_public is k x n_public x 4
+ * (standard form); d_ok receives k int32 verdicts followed by one uint32 status word (bits 0..2 as above; bit 3: an
+ * out-of-range input was seen).  The Vk, IC and rho are host arguments and are checked as b200_pinocchio_verify_batch
+ * checks them (B200_ERANGE / B200_EINVAL).  A proof coordinate >= q or a public signal >= r gives that proof verdict 0
+ * and sets status bit 3; a PiB at infinity gives verdict 0.  Neither returns an error code, and nothing of either reaches
+ * a later call.  Scratch is stream-ordered device memory (cudaMallocAsync), freed behind the work.  The same 9 (8)
+ * launches.                                                                                                          */
+int b200_pinocchio_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t vk_g1[24], const uint64_t vk_g2[120],
+                                       const void* d_proofs, const void* d_public, size_t n_public, size_t k,
+                                       const uint64_t* rho, void* d_ok, void* stream);
 
 /* ---- dense QAP API upstream of GenerateProofs (small n; the prove path consumes px) ---- */
 /* PolynomialField.R1CSToQAP (r1csqap/r1csqap.go:161-188).  a, b, c: n x m row-major R1CS matrices (coefficients
