@@ -46,9 +46,14 @@ int g_device = -1;
 // flight beside a proof on a context-0 key (two proofs pipelined on two caller streams: the latency-bound sort / tail /
 // product chains of one overlap the accumulation of the other).  Every other library call runs on context 0's main stream
 // and polynomial workspace.
+// A context's shared scratch is its PolyCtx (buffers and transform plans) and its R1csWork on every R1CS.  Proofs on the
+// context's keys use it on their side stream 3 while the caller's stream runs on; library calls use context 0's on its
+// main stream.  Every enqueue that touches it first makes its stream wait on `scratch_free` and records `scratch_free`
+// behind its last use (scratch_acquire / scratch_release), under the library mutex: the uses run in the host's order.
 struct ProveCtx {
   cudaStream_t main = nullptr;   // host-pointer proofs on this context's keys
   cudaStream_t side[3] = {nullptr, nullptr, nullptr};   // side streams: independent MSMs of one proof overlap
+  cudaEvent_t scratch_free = nullptr;   // behind the last enqueued use of the shared scratch
   std::unique_ptr<PolyCtx> poly;
   // NCCL communicator of the all-gathers (b200_comm_init).  Context 1 gathers on its own (ncclCommSplit of context 0's):
   // NCCL matches collectives by issue order per communicator, and two host threads proving on the two contexts reach
@@ -150,6 +155,7 @@ int init_locked(int device) {
   for (auto& c : g_ctx) {
     CU(cudaStreamCreateWithFlags(&c.main, cudaStreamNonBlocking));
     for (auto& sd : c.side) CU(cudaStreamCreateWithFlags(&sd, cudaStreamNonBlocking));  // (stream priorities: no measurable effect)
+    CU(cudaEventCreateWithFlags(&c.scratch_free, cudaEventDisableTiming));
     c.poly = std::make_unique<PolyCtx>();
     c.poly->launch_counter = &g_launches;
   }
@@ -157,6 +163,16 @@ int init_locked(int device) {
   CU(cudaMemset(g_d_err, 0, sizeof(int)));
   g_device = device;
   g_init = true;
+  return B200_OK;
+}
+
+// Order `st` behind the last enqueued use of context c's shared scratch / mark the end of this stream's use (ProveCtx).
+int scratch_acquire(ProveCtx& c, cudaStream_t st) {
+  CU(cudaStreamWaitEvent(st, c.scratch_free, 0));
+  return B200_OK;
+}
+int scratch_release(ProveCtx& c, cudaStream_t st) {
+  CU(cudaEventRecord(c.scratch_free, st));
   return B200_OK;
 }
 
@@ -240,8 +256,9 @@ int check_err_flag(const char* what, int* d_err, cudaStream_t st = nullptr, std:
     CU(cudaMemsetAsync(d_err, 0, sizeof(int), st));
     if (h & 16) return fail(B200_EINVAL, "%s: tau is one of the interpolation points 1..n", what);
     if (h & 8) return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (G2 point at infinity; the reference panics, bn128.go:238-241)", what);
-    if (h & 4) return fail(B200_EDIVZERO, "%s: divisor has a zero leading coefficient", what);
-    return fail(B200_ERANGE, "%s: %s", what, (h & 1) ? "point coordinate >= q" : "scalar / coefficient >= r");
+    // before the zero divisor: a leading coefficient >= r is read as 0 and also sets bit 2; the input is what is wrong
+    if (h & 3) return fail(B200_ERANGE, "%s: %s", what, (h & 1) ? "point coordinate >= q" : "scalar / coefficient >= r");
+    return fail(B200_EDIVZERO, "%s: divisor has a zero leading coefficient", what);
   }
   return B200_OK;
 }
@@ -359,7 +376,9 @@ int poly_mul_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, ui
   CU(dout.alloc((na + nb - 1) * sizeof(Fr)));
   CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
   CU(cudaMemcpyAsync(db.p, b, nb * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  if (int rc = scratch_acquire(g_ctx[0], g_ctx[0].main)) return rc;
   CU(poly_mul_device(*g_ctx[0].poly, da.as<Fr>(), na, 0, db.as<Fr>(), nb, 0, dout.as<Fr>(), g_d_err, g_ctx[0].main));
+  if (int rc = scratch_release(g_ctx[0], g_ctx[0].main)) return rc;
   CU(cudaMemcpyAsync(out, dout.p, (na + nb - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
   return check_err_flag("poly_mul", g_d_err);
 }
@@ -396,7 +415,9 @@ int poly_div_host(const uint64_t* a, size_t na, const uint64_t* b, size_t nb, ui
   CU(dq.alloc(nq * sizeof(Fr)));
   if (rem && nb > 1) CU(dr.alloc((nb - 1) * sizeof(Fr)));
   CU(cudaMemcpyAsync(da.p, a, na * sizeof(Fr), cudaMemcpyHostToDevice, g_ctx[0].main));
+  if ((rc = scratch_acquire(g_ctx[0], g_ctx[0].main))) return rc;
   CU(poly_div_device(*g_ctx[0].poly, dv, da.as<Fr>(), na, 0, dq.as<Fr>(), dr.as<Fr>(), g_d_err, g_ctx[0].main));
+  if ((rc = scratch_release(g_ctx[0], g_ctx[0].main))) return rc;
   CU(cudaMemcpyAsync(q, dq.p, nq * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
   if (rem && nb > 1) CU(cudaMemcpyAsync(rem, dr.p, (nb - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, g_ctx[0].main));
   return check_err_flag("poly_div", g_d_err);
@@ -424,8 +445,10 @@ int groth16_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, const uint6
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
-  const Fr *h, *px;   // h itself, or px for groth16_enqueue's division
-  int rc = qap_quotient_enqueue(r1, pk->Z.nb, pk->ctx, *pk->pctx().poly, d_w, err, sq, &h, &px);
+  const Fr *h, *px;   // h itself, or px for groth16_enqueue's division; that releases the scratch behind its last read
+  int rc = scratch_acquire(pk->pctx(), sq);
+  if (rc) return rc;
+  rc = qap_quotient_enqueue(r1, pk->Z.nb, pk->ctx, *pk->pctx().poly, d_w, err, sq, &h, &px);
   if (rc) return rc;
   return groth16_enqueue(pk, d_w, pk->m, px, npx, r, s, d_out, st, err, /*px_mont=*/1, h);
 }
@@ -584,9 +607,13 @@ int groth16_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, const
   // --- side stream 3: the quotients into the C||PTD vectors (h_p[p_lo, p_lo + n_p), zeros beyond len(h), -r_p s_p with
   // the tail), then the C||PTD MSMs
   EV_WAIT(s3, e_in);
-  if (quotient && (rc = qap_quotient_batch_enqueue(r1, ws, fb, *pk->pctx().poly, pk->Z, pk->h_full.as<Fr>(), d_w, k, CH + n_c, nch,
-                                                   n_p, sl.p_lo, sl.tail[3] ? rs + 3 : nullptr, s3, err)))
-    return rc;
+  if (quotient) {
+    if ((rc = scratch_acquire(pk->pctx(), s3))) return rc;
+    if ((rc = qap_quotient_batch_enqueue(r1, ws, fb, *pk->pctx().poly, pk->Z, pk->h_full.as<Fr>(), d_w, k, CH + n_c, nch, n_p,
+                                         sl.p_lo, sl.tail[3] ? rs + 3 : nullptr, s3, err)))
+      return rc;
+    if ((rc = scratch_release(pk->pctx(), s3))) return rc;
+  }
   MsmShape sh;
   if (Bases* gch = pk->g[3].get()) {
     sh = gch->sh;
@@ -715,8 +742,10 @@ int pinocchio_witness_enqueue(ProvingKey* pk, R1cs* r1, const Fr* d_w, Fq* d_out
     CU(cudaEventRecord(pk->ev[0], st));
     CU(cudaStreamWaitEvent(sq, pk->ev[0], 0));
   }
-  const Fr *h, *px;   // h itself, or px for pinocchio_enqueue's division
-  int rc = qap_quotient_enqueue(r1, pk->Z.nb, pk->ctx, *pk->pctx().poly, d_w, err, sq, &h, &px);
+  const Fr *h, *px;   // h itself, or px for pinocchio_enqueue's division; that releases the scratch behind its last read
+  int rc = scratch_acquire(pk->pctx(), sq);
+  if (rc) return rc;
+  rc = qap_quotient_enqueue(r1, pk->Z.nb, pk->ctx, *pk->pctx().poly, d_w, err, sq, &h, &px);
   if (rc) return rc;
   return pinocchio_enqueue(pk, d_w, px, npx, /*px_mont=*/1, h, d_out, record, st, err);
 }
@@ -844,8 +873,10 @@ int pinocchio_batch_parts(ProvingKey* pk, R1cs* r1, const Fr* d_w, size_t k, Fq*
   if (pk->g[7]) {
     if (s3 != st) EV_WAIT(s3, e_in);
     Fr* H = b.CH.as<Fr>();   // len(h) <= len(G1T) (pinocchio_check_px): every quotient is divided straight into its vector
+    if ((rc = scratch_acquire(pk->pctx(), s3))) return rc;
     if ((rc = qap_quotient_batch_enqueue(r1, ws, fb, *pk->pctx().poly, pk->Z, nullptr, d_w, k, H, ng, ng, 0, nullptr, s3, err)))
       return rc;
+    if ((rc = scratch_release(pk->pctx(), s3))) return rc;
     if ((rc = sort_of(7, H, ng, s3))) return rc;
     if ((rc = buckets_of(7, s3))) return rc;
   }
@@ -993,7 +1024,9 @@ int combine_polynomials_host(const uint64_t* r, size_t m, const uint64_t* ap, co
     CU(cudaStreamSynchronize(st));
   }
   // px = ax*bx - cx   (r1csqap.go:208)
+  if (int rc = scratch_acquire(g_ctx[0], st)) return rc;
   CU(poly_mul_device(*g_ctx[0].poly, mont[0].as<Fr>(), n, 1, mont[1].as<Fr>(), n, 1, prod.as<Fr>(), g_d_err, st));
+  if (int rc = scratch_release(g_ctx[0], st)) return rc;
   k_poly_addsub<<<nblk(2 * n - 1, 256), 256, 0, st>>>(prod.as<Fr>(), (uint32_t)(2 * n - 1), stdv[2].as<Fr>(), (uint32_t)n, 1,
                                                       prod.as<Fr>(), g_d_err);
   CU(cudaMemcpyAsync(px, prod.p, (2 * n - 1) * sizeof(Fr), cudaMemcpyDeviceToHost, st));

@@ -560,8 +560,11 @@ int groth16_enqueue(ProvingKey* pk, const Fr* d_w, size_t nw, const Fr* d_px, si
       bool direct = p_lo == 0 && nq <= n_p;
       Fr* h_dst = direct ? sCH + n_c : pk->h_full.as<Fr>();
       if (!direct && !pk->h_full.p) CU(pk->h_full.alloc((pk->m + pk->n_h_bases + 4) * sizeof(Fr)));
+      // the division's workspace, or the witness front end's R1csWork that holds h / px: the context's shared scratch
+      if ((rc = scratch_acquire(pk->pctx(), s3))) return rc;
       if (d_h_std) CU(cudaMemcpyAsync(h_dst, d_h_std, nq * sizeof(Fr), cudaMemcpyDeviceToDevice, s3));
       else CU(poly_div_device(*pk->pctx().poly, pk->Z, d_px, npx, px_mont, h_dst, nullptr, err, s3));
+      if ((rc = scratch_release(pk->pctx(), s3))) return rc;
       size_t have = nq > p_lo ? (nq < p_hi ? nq - p_lo : n_p) : 0;   // valid h coefficients inside [p_lo, p_hi)
       if (!direct && have)
         CU(cudaMemcpyAsync(sCH + n_c, pk->h_full.as<Fr>() + p_lo, have * sizeof(Fr), cudaMemcpyDeviceToDevice, s3));
@@ -833,11 +836,14 @@ int pinocchio_enqueue(ProvingKey* pk, const Fr* d_w, const Fr* d_px, size_t npx,
     used[2] = true;
     EV_WAIT(s3, e_in);
     const Fr* dh = d_h_std;
+    // the division's workspace, or the witness front end's R1csWork that holds h / px: the context's shared scratch
+    if ((rc = scratch_acquire(pk->pctx(), s3))) return rc;
     if (!dh) {
       CU(poly_div_device(*pk->pctx().poly, pk->Z, d_px, npx, px_mont, pk->s3.as<Fr>(), nullptr, err, s3));
       dh = pk->s3.as<Fr>();
     }
     if ((rc = msm_enqueue<Fq>(pk->g[7].get(), dh, nq, 0, slot_g1(7), err, s3))) return rc;
+    if ((rc = scratch_release(pk->pctx(), s3))) return rc;
   }
   // two scalar vectors: w[l+1..m) feeds PiA, PiAp (snark.go:265-268); w feeds PiB, PiBp, PiC, PiCp, PiKp (:270-278).
   // Per vector ONE digit sort (held by the first owned set of the group), the bucket phases fan out over the streams.

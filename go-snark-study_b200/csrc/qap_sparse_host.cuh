@@ -263,8 +263,10 @@ int qap_px_host(b200_r1cs_t h, const uint64_t* w, size_t nw, uint64_t* ax, uint6
   CU(dabc.alloc(3 * n * sizeof(Fr)));
   CU(dpx.alloc((2 * n - 1) * sizeof(Fr)));
   CU(cudaMemcpyAsync(dw.p, w, nw * sizeof(Fr), cudaMemcpyHostToDevice, st));
+  if ((rc = scratch_acquire(g_ctx[0], st))) return rc;   // ws: context 0's, which its proofs' front ends share
   rc = qap_px_enqueue(r, *ws, *g_ctx[0].poly, dw.as<Fr>(), dabc.as<Fr>(), dpx.as<Fr>(), g_d_err, st);
   if (rc) return rc;
+  if ((rc = scratch_release(g_ctx[0], st))) return rc;
   uint64_t* outs[3] = {ax, bx, cx};
   for (int k = 0; k < 3; k++)
     if (outs[k]) CU(cudaMemcpyAsync(outs[k], dabc.as<Fr>() + k * n, n * sizeof(Fr), cudaMemcpyDeviceToHost, st));
@@ -288,7 +290,9 @@ int interpolate_host(const uint64_t* values, size_t n, uint64_t* coeffs) {
   CU(ds.alloc(n * sizeof(Fr)));
   CU(cudaMemcpyAsync(dv.p, values, n * sizeof(Fr), cudaMemcpyHostToDevice, st));
   k_poly_load<<<nblk(n, 256), 256, 0, st>>>(dv.as<Fr>(), (uint32_t)n, (uint32_t)n, 0, 0, dm.as<Fr>(), (uint32_t)n, g_d_err);
+  if ((rc = scratch_acquire(g_ctx[0], st))) return rc;
   CU(interpolate_ap(*g_ctx[0].poly, *dom, wk, dm.as<Fr>(), n, n, 1, dc.as<Fr>(), st));
+  if ((rc = scratch_release(g_ctx[0], st))) return rc;
   k_poly_store<<<nblk(n, 256), 256, 0, st>>>(dc.as<Fr>(), (uint32_t)n, 0, 1, ds.as<Fr>());
   CU(cudaMemcpyAsync(coeffs, ds.p, n * sizeof(Fr), cudaMemcpyDeviceToHost, st));
   return check_err_flag("interpolate", g_d_err);
@@ -315,7 +319,9 @@ int zero_poly_device(size_t n, DevBuf& d_out, cudaStream_t st) {
   CU(cudaMemsetAsync(P.p, 0, N * sizeof(Fr), st));
   Fr one = Fr::one();
   CU(cudaMemcpyAsync(P.as<Fr>() + n, &one, sizeof(Fr), cudaMemcpyHostToDevice, st));
+  if ((rc = scratch_acquire(g_ctx[0], st))) return rc;
   CU(newton_to_monomial(*g_ctx[0].poly, *dom, P.as<Fr>(), X.as<Fr>(), 1, st));
+  if ((rc = scratch_release(g_ctx[0], st))) return rc;
   CU(cudaMemcpyAsync(o, P.p, (n + 1) * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
   CU(cudaStreamSynchronize(st));
   return B200_OK;

@@ -64,7 +64,9 @@ int b200_version(void);
  * keeps two proofs in flight hides the latency-bound sort / bucket-tail / blinding-product chains of one behind the
  * accumulation of the other (bench.py `proofs_in_flight`; the keys are independent objects, each with its own tables,
  * scratch and error words).  Host-pointer proofs run on their key's context and report only their own input errors, also
- * when two host threads prove at once.  Other calls run on context 0.                                                 */
+ * when two host threads prove at once.  Other calls run on context 0 and share its scratch with its proofs: each use
+ * of a context's scratch waits for the previous one on the device, in the order the calls were made, so a library call
+ * made while a context-0 proof is in flight on another stream waits on the device for that proof's quotient.          */
 #define B200_CFG_PK_CONTEXT 4
 /* B200_CFG_PAIRING_KERNEL: b200_pairing_batch with one THREAD per pairing (1: the step-by-step restatement of
  * bn128.go:179-421, a long chain of dependent multiplications per pairing) or one WARP per pairing (2: F_q^12 in shared
