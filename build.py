@@ -201,8 +201,8 @@ def build_host_setup_key(force=False):
 
 
 def build_host_verify_batch(force=False):
-    """g++ build of the batched Groth16 verifier's kernels (split pairings, G2 subgroup test, classification, the
-    aggregate in launch order) over csrc/host_stub (CPU test vehicle, tests/test_host_verify_batch.py)."""
+    """g++ build of the batched Groth16 verifier's kernels (split pairings, G2 subgroup test, classification) and of its
+    aggregate stage through verify_host.cuh over csrc/host_stub (CPU test vehicle, tests/test_host_verify_batch.py)."""
     os.makedirs(LIBDIR, exist_ok=True)
     target = os.path.join(LIBDIR, "libb200_host_verify_batch.so")
     if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):
@@ -213,8 +213,9 @@ def build_host_verify_batch(force=False):
 
 
 def build_host_pinocchio_verify_batch(force=False):
-    """g++ build of the batched Pinocchio verifier's kernels (classification, the reference sums S_i and T_i, the aggregate
-    in launch order) over csrc/host_stub (CPU test vehicle, tests/test_host_pinocchio_verify_batch.py)."""
+    """g++ build of the batched Pinocchio verifier's classification kernel and of its aggregate stage (the reference sums
+    S_i and T_i included) through verify_host.cuh over csrc/host_stub (CPU test vehicle,
+    tests/test_host_pinocchio_verify_batch.py)."""
     os.makedirs(LIBDIR, exist_ok=True)
     target = os.path.join(LIBDIR, "libb200_host_pinocchio_verify_batch.so")
     if not force and not _newer(target, _all_sources() + [os.path.join(HOSTTEST, "host_stub", "cuda_runtime.h")]):

@@ -27,12 +27,7 @@
 #include "glv.cuh"
 #include "pinocchio_batch.cuh"
 #include "shard_batch.cuh"
-#ifndef B200_NO_PAIRING
-#include "pairing.cuh"
-#include "pairing_warp.cuh"
-#include "verify_batch.cuh"
-#include "verify_batch_pinocchio.cuh"
-#endif
+#include "verify_host.cuh"
 
 using namespace b200;
 
@@ -1102,222 +1097,13 @@ int zero_poly_host(size_t n, uint64_t* out) {   // coefficients of prod_{i=1..n}
   return check_err_flag("zero_poly", g_d_err);
 }
 
-#ifndef B200_NO_PAIRING
-// ---- pairing / verification (SURVEY §8f row 2) -------------------------------------------------------
-template <bool FAST_FE>
-__device__ void pairing_from_jacobian(const Fq* g1, const Fq2* g2, F12& out, int* err) {
-  bool bad = false;
-  for (int k = 0; k < 3; k++) bad = bad || g1[k].geq_modulus() || g2[k].c0.geq_modulus() || g2[k].c1.geq_modulus();
-  Jacobian<Fq> p{g1[0].to_mont(), g1[1].to_mont(), g1[2].to_mont()};
-  Jacobian<Fq2> q{g2[0].to_mont(), g2[1].to_mont(), g2[2].to_mont()};
-  if (bad || q.is_inf()) {  // G2 infinity: preComputeG2 panics "q1[2] != Fq2.One()" (bn128.go:238-241)
-    atomicOr(err, bad ? 1 : 8);
-    out = F12::one();
-    return;
-  }
-  Affine<Fq> pa = jac_to_affine(p);                      // preComputeG1: G1.Affine, infinity -> (0, 0)
-  Affine<Fq2> qa = jac_to_affine(q);
-  F2::B px, py;
-#pragma unroll
-  for (int i = 0; i < 8; i++) { px.l[i] = pa.x.l[i]; py.l[i] = pa.y.l[i]; }
-  out = pairing_affine_t<FAST_FE>(px, py, qa.x, qa.y);
-}
-__device__ void store_f12_std(const F12& f, Fq2* out) {
-  out[0] = f.a.a.from_mont(); out[1] = f.a.b.from_mont(); out[2] = f.a.c.from_mont();
-  out[3] = f.b.a.from_mont(); out[4] = f.b.b.from_mont(); out[5] = f.b.c.from_mont();
-}
-// out[i] = a[i] * b[i] in F_q^12 (fields/fq12.go:72-84), standard form in/out, [2][3][2] order
-__global__ void __launch_bounds__(32) k_fq12_mul_batch(const Fq2* a, const Fq2* b, size_t n, Fq2* out, int* err) {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  F12 x, y;
-  Fq2* xs = &x.a.a;
-  Fq2* ys = &y.a.a;
-  bool bad = false;
-  for (int k = 0; k < 6; k++) {
-    Fq2 u = a[6 * i + k], v = b[6 * i + k];
-    bad = bad || u.geq_modulus() || v.geq_modulus();
-    xs[k] = u.to_mont();
-    ys[k] = v.to_mont();
-  }
-  if (bad) atomicOr(err, 1);
-  store_f12_std(f12_mul(x, y), out + 6 * i);
-}
-template <bool FAST_FE>
-__global__ void __launch_bounds__(32) k_pairing_batch(const Fq* g1, const Fq2* g2, size_t n, Fq2* out, int* err) {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  F12 f;
-  pairing_from_jacobian<FAST_FE>(g1 + 3 * i, g2 + 3 * i, f, err);
-  store_f12_std(f, out + 6 * i);
-}
-// ---- one warp per pairing (pairing_warp.cuh) ----------------------------------------------------------------------
-constexpr int kPairWarps = 4;   // warps (pairings) per CTA: 4 x 9.5 KB of shared memory
-// lane 0 validates and normalises the Jacobian inputs (preComputeG1 / G2.Affine); returns warp-uniformly whether a pairing
-// is to be computed (false: out-of-range coordinate or G2 infinity — the reference panics, bn128.go:238-241 — result = one)
-__device__ bool warp_pairing_inputs(wp::Ws& ws, const Fq* g1, const Fq2* g2, F2::B& px, F2::B& py, F2& qx, F2& qy, int* err) {
-  int go = 1;
-  if ((threadIdx.x & 31u) == 0) {
-    bool bad = false;
-    for (int k = 0; k < 3; k++) bad = bad || g1[k].geq_modulus() || g2[k].c0.geq_modulus() || g2[k].c1.geq_modulus();
-    Jacobian<Fq> p{g1[0].to_mont(), g1[1].to_mont(), g1[2].to_mont()};
-    Jacobian<Fq2> q{g2[0].to_mont(), g2[1].to_mont(), g2[2].to_mont()};
-    if (bad || q.is_inf()) {
-      atomicOr(err, bad ? 1 : 8);
-      go = 0;
-    } else {
-      Affine<Fq> pa = jac_to_affine(p);
-      Affine<Fq2> qa = jac_to_affine(q);
-#pragma unroll
-      for (int i = 0; i < 8; i++) { px.l[i] = pa.x.l[i]; py.l[i] = pa.y.l[i]; }
-      qx = qa.x;
-      qy = qa.y;
-    }
-  }
-  (void)ws;
-  return __shfl_sync(0xffffffffu, go, 0) != 0;
-}
-__global__ void __launch_bounds__(32 * kPairWarps) k_pairing_batch_warp(const Fq* g1, const Fq2* g2, size_t n, Fq2* out, int* err) {
-  __shared__ wp::Ws wss[kPairWarps];
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-  const size_t i = (size_t)blockIdx.x * kPairWarps + warp;
-  if (i >= n) return;
-  wp::Ws& ws = wss[warp];
-  F2::B px, py;
-  F2 qx, qy;
-  if (warp_pairing_inputs(ws, g1 + 3 * i, g2 + 3 * i, px, py, qx, qy, err)) wp::pairing(ws, px, py, qx, qy);
-  else wp::f12_set_one(ws, wp::RF);
-  if (lane < 12) {  // standard form out, [2][3][2] order: one F_q component per lane
-    const F2& c = ws.r[wp::RF][lane >> 1];
-    F2::B v = ((lane & 1) ? c.c1 : c.c0).from_mont();
-    Fq2* o = out + 6 * i + (lane >> 1);
-    if (lane & 1) o->c1 = v;
-    else o->c0 = v;
-  }
-}
-// groth16.VerifyProof (groth16/groth16.go:281-305): e(A,B) == e(alpha,beta) * (e(icPubl,gamma) * e(C,delta)).
-// Warp w of a 128-thread CTA pairs g1 with g2, the w-th of (A, alpha1, icPubl, C) and (B, beta2, gamma2, delta2) (Jacobian
-// standard form); warp 0 then forms the right-hand side with two warp-wide F_q^12 products and compares.
-__device__ void groth16_verify_cta(wp::Ws* wss, const Fq* g1, const Fq2* g2, int* ok, int* err) {
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-  wp::Ws& ws = wss[warp];
-  F2::B px, py;
-  F2 qx, qy;
-  if (warp_pairing_inputs(ws, g1, g2, px, py, qx, qy, err)) wp::pairing(ws, px, py, qx, qy);
-  else wp::f12_set_one(ws, wp::RF);
-  __syncthreads();
-  if (warp == 0) {
-    if (lane < 6) {
-      ws.r[2][lane] = wss[1].r[wp::RF][lane];
-      ws.r[3][lane] = wss[2].r[wp::RF][lane];
-      ws.r[4][lane] = wss[3].r[wp::RF][lane];
-    }
-    wp::wsync();
-    wp::f12_mul(ws, 3, 3, 4);
-    wp::f12_mul(ws, 2, 2, 3);
-    const int same = lane < 6 ? (ws.r[0][lane] == ws.r[2][lane] ? 1 : 0) : 1;
-    const unsigned all = __ballot_sync(0xffffffffu, same);
-    if (lane == 0) *ok = all == 0xffffffffu ? 1 : 0;
-  }
-}
-// pts1: A, alpha1, icPubl, C ; pts2: B, beta2, gamma2, delta2
-__global__ void __launch_bounds__(128) k_groth16_verify(const Fq* pts1, const Fq2* pts2, int* ok, int* err) {
-  __shared__ wp::Ws wss[4];
-  const uint32_t warp = threadIdx.x >> 5;
-  groth16_verify_cta(wss, pts1 + 3 * warp, pts2 + 3 * warp, ok, err);
-}
-// k_groth16_verify over a batch, one CTA per proof (verify_batch.cuh): a regular proof under a passed aggregate is accepted
-// at once, a bad one (coordinate >= q, signal >= r, PiB at infinity) gets 0, every other proof the single call's verdict.
-__global__ void __launch_bounds__(128) k_vb_verify_each(const uint64_t* proofs, const vb::Vk* vk, const Fq* icp,
-                                                        const uint32_t* flags, const uint32_t* agg, size_t k, int* ok,
-                                                        uint32_t* status, int* err) {
-  __shared__ wp::Ws wss[4];
-  const size_t p = blockIdx.x;
-  const uint32_t f = flags[p] | flags[k];
-  if ((f & vb::kBad) || (!f && *agg)) {
-    if (threadIdx.x == 0) ok[p] = (f & vb::kBad) ? 0 : 1;
-    return;
-  }
-  if (threadIdx.x == 0) atomicOr(status, vb::kStPerProof);
-  const uint32_t warp = threadIdx.x >> 5;
-  const vb::ProofView v = vb::proof_at(proofs, p);
-  const Fq* g1 = warp == 0 ? v.a : (warp == 1 ? vk->alpha : (warp == 2 ? icp + 3 * p : v.c));
-  const Fq2* g2 = warp == 0 ? v.b : (warp == 1 ? vk->beta : (warp == 2 ? vk->gamma : vk->delta));
-  groth16_verify_cta(wss, g1, g2, ok + p, err);
-}
-// snark.VerifyProof over a batch, one CTA per proof (verify_batch_pinocchio.cuh): a regular proof under a passed aggregate
-// is accepted at once, a bad one (coordinate >= q, signal >= r, PiB at infinity) gets 0, every other proof the reference's
-// verdict: its twelve pairings (warp w runs pairings 3w .. 3w + 2 with warp_pairing_inputs' semantics), the two F_q^12
-// products e7 e8 and e9 e10, and the five comparisons of snark.go:292-372.
-__global__ void __launch_bounds__(128) k_pvb_verify_each(const uint64_t* proofs, const vb::PVk* vk, const Fq* st,
-                                                         const uint32_t* flags, const uint32_t* agg, size_t k, int* ok,
-                                                         uint32_t* status, int* err) {
-  __shared__ wp::Ws wss[4];
-  __shared__ F2 e[vb::kPvbPairings][6];
-  const size_t p = blockIdx.x;
-  const uint32_t f = flags[p] | flags[k];
-  if ((f & vb::kBad) || (!f && *agg)) {
-    if (threadIdx.x == 0) ok[p] = (f & vb::kBad) ? 0 : 1;
-    return;
-  }
-  if (threadIdx.x == 0) atomicOr(status, vb::kStPerProof);
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-  wp::Ws& ws = wss[warp];
-  for (int j = 3 * (int)warp; j < 3 * (int)warp + 3; j++) {
-    F2::B px, py;
-    F2 qx, qy;
-    if (warp_pairing_inputs(ws, vb::pvb_pairing_g1(proofs, vk, st, p, j), vb::pvb_pairing_g2(proofs, vk, p, j), px, py, qx, qy, err))
-      wp::pairing(ws, px, py, qx, qy);
-    else
-      wp::f12_set_one(ws, wp::RF);
-    if (lane < 6) e[j][lane] = ws.r[wp::RF][lane];
-    wp::wsync();
-  }
-  __syncthreads();
-  if (warp != 0) return;
-  if (lane < 6) {
-    ws.r[2][lane] = e[7][lane];
-    ws.r[3][lane] = e[8][lane];
-    ws.r[4][lane] = e[9][lane];
-    ws.r[5][lane] = e[10][lane];
-  }
-  wp::wsync();
-  wp::f12_mul(ws, 2, 2, 3);   // e(PiH, Vkz) e(PiC, g2)
-  wp::f12_mul(ws, 4, 4, 5);   // e(T, G2Kbg) e(G1Kbg, PiB)
-  int same = 1;
-  if (lane < 6)
-    same = e[0][lane] == e[1][lane] && e[2][lane] == e[3][lane] && e[4][lane] == e[5][lane] && e[6][lane] == ws.r[2][lane] &&
-           ws.r[4][lane] == e[11][lane];
-  const unsigned all = __ballot_sync(0xffffffffu, same);
-  if (lane == 0) ok[p] = all == 0xffffffffu ? 1 : 0;
-}
-// icPubl = IC[0] + sum publicSignals[i] * IC[i+1] (groth16.go:283-286).  The products are independent: one half-warp each,
-// with the GLV split of prove_host.cuh (128 doublings + ~12 additions deep instead of the 254 + ~127 of MulScalar's
-// double-and-add; the same group element, which is all the pairing — it normalises its inputs — can see); the sum then runs
-// in the reference's order with the reference's Add, so its degenerate cases (equal operands give Z = 0) are the reference's.
-struct GlvScalar {
-  uint64_t k[4];
-  uint32_t neg[2];
-};
-__global__ void __launch_bounds__(32) k_ic_terms(const Fq* ic, const GlvScalar* gs, size_t npub, Jacobian<Fq>* terms, int* err) {
-  const uint32_t t = threadIdx.x & 31u;
-  const size_t i = (size_t)blockIdx.x * 2 + (t >> 4);
-  const size_t ii = i < npub ? i : npub - 1;   // an odd count leaves the last half-warp a duplicate: every lane joins the shuffles
-  const Fq* src = ic + 3 * (ii + 1);
-  if (src[0].geq_modulus() || src[1].geq_modulus() || src[2].geq_modulus()) atomicOr(err, 1);
-  Jacobian<Fq> p{src[0].to_mont(), src[1].to_mont(), src[2].to_mont()};
-  GlvScalar g = gs[ii];
-  Jacobian<Fq> r = glv_mul_halfwarp(p, g.k, g.neg, t);
-  if (i < npub && (t & 15u) == 0) terms[i] = r;
-}
-__global__ void k_ic_sum(const Fq* ic, const Jacobian<Fq>* terms, size_t npub, Fq* out, int* err) {
-  if (threadIdx.x | blockIdx.x) return;
-  if (ic[0].geq_modulus() || ic[1].geq_modulus() || ic[2].geq_modulus()) atomicOr(err, 1);
-  Jacobian<Fq> acc{ic[0].to_mont(), ic[1].to_mont(), ic[2].to_mont()};
-  for (size_t i = 0; i < npub; i++) acc = jac_add_ref(acc, terms[i]);
-  out[0] = acc.X.from_mont();
-  out[1] = acc.Y.from_mont();
-  out[2] = acc.Z.from_mont();
+// ---- pairing / verification (verify_host.cuh) -------------------------------------------------------------------------
+// The verification engine under the library's settings, read at every call (b200_config B200_CFG_PAIRING_KERNEL).
+VbEnv vb_env() {
+  VbEnv env;
+  env.launch_counter = &g_launches;
+  env.pairing_kernel = g_pairing_kernel;
+  return env;
 }
 
 // Final exponentiation: Devegili-Scott-Dahab (easy part + hard part by the BN parameter), the SAME F_q^12 value as the
@@ -1334,10 +1120,7 @@ int pairing_batch_host(const uint64_t* g1, const uint64_t* g2, size_t n, uint64_
   CU(dout.alloc(n * 6 * sizeof(Fq2)));
   CU(cudaMemcpyAsync(d1.p, g1, n * 3 * sizeof(Fq), cudaMemcpyHostToDevice, g_ctx[0].main));
   CU(cudaMemcpyAsync(d2.p, g2, n * 3 * sizeof(Fq2), cudaMemcpyHostToDevice, g_ctx[0].main));
-  // auto: a warp per pairing has the much shorter latency and wins for small calls; above that the thread-per-pairing
-  // kernel keeps more pairings resident and has the higher throughput
-  const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
-  if (thread_kernel) k_pairing_batch<kFastFinalExp><<<nblk(n, 32), 32, 0, g_ctx[0].main>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
+  if (vb_env().thread_pairings(n)) k_pairing_batch<kFastFinalExp><<<nblk(n, 32), 32, 0, g_ctx[0].main>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
   else k_pairing_batch_warp<<<nblk(n, kPairWarps), 32 * kPairWarps, 0, g_ctx[0].main>>>(d1.as<Fq>(), d2.as<Fq2>(), n, dout.as<Fq2>(), g_d_err);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, dout.p, n * 6 * sizeof(Fq2), cudaMemcpyDeviceToHost, g_ctx[0].main));
@@ -1400,7 +1183,7 @@ int groth16_verify_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1,
   return check_err_flag("groth16_verify", g_d_err);
 }
 
-// ---- batched verification (verify_batch.cuh) ----------------------------------------------------------------------------
+// ---- batched verification (verify_host.cuh) -----------------------------------------------------------------------------
 // Stream-ordered device memory: freed behind the work queued on its stream, so a _device call returns without waiting.
 struct StreamBuf {
   void* p = nullptr;
@@ -1414,56 +1197,6 @@ struct StreamBuf {
     return cudaMallocAsync(&p, b, s);
   }
 };
-// per-call scratch of verify_batch_enqueue, carved from one allocation
-struct VbScratch {
-  size_t off[10];
-  size_t bytes;
-  VbScratch(size_t k, size_t npub) {
-    const size_t n = k + 3, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
-    const size_t sz[10] = {(k + 1) * 4, 4, 4, 4, 3 * k * sizeof(Fq), (npub ? npub * k : 1) * sizeof(Jacobian<Fq>),
-                           3 * k * sizeof(Jacobian<Fq>), 3 * sizeof(Jacobian<Fq>), 6 * n * sizeof(F2), 6 * nparts * sizeof(F2)};
-    bytes = 0;
-    for (int i = 0; i < 10; i++) {
-      off[i] = bytes;
-      bytes += (sz[i] + 255) & ~(size_t)255;
-    }
-  }
-};
-// Every launch of a batch verification, on `st`: d_ok[0..k) verdicts, *d_status the status bits (zeroed here first).
-// A fixed launch sequence: no step waits for the host, whatever k and whatever the outcome.
-int verify_batch_enqueue(const Fq* d_ic, const vb::Vk* d_vk, const uint64_t* d_proofs, const uint64_t* d_pub, size_t npub,
-                         size_t k, const uint64_t* d_rho, int* d_ok, uint32_t* d_status, uint8_t* scratch, cudaStream_t st) {
-  const VbScratch L(k, npub);
-  uint32_t* flags = (uint32_t*)(scratch + L.off[0]);
-  uint32_t* k_reg = (uint32_t*)(scratch + L.off[1]);
-  uint32_t* agg = (uint32_t*)(scratch + L.off[2]);
-  int* err = (int*)(scratch + L.off[3]);
-  Fq* icp = (Fq*)(scratch + L.off[4]);
-  Jacobian<Fq>* terms = (Jacobian<Fq>*)(scratch + L.off[5]);
-  Jacobian<Fq>* rterms = (Jacobian<Fq>*)(scratch + L.off[6]);
-  Jacobian<Fq>* sums = (Jacobian<Fq>*)(scratch + L.off[7]);
-  F2* mvals = (F2*)(scratch + L.off[8]);
-  F2* parts = (F2*)(scratch + L.off[9]);
-  const size_t n = k + 3, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
-  CU(cudaMemsetAsync(scratch, 0, L.off[4], st));
-  CU(cudaMemsetAsync(d_status, 0, sizeof(uint32_t), st));
-  vb::k_vb_classify<<<nblk(k + 1, 64), 64, 0, st>>>(d_proofs, d_vk, k, flags, d_status);
-  if (npub) vb::k_vb_ic_terms<<<nblk(npub * k, 2), 32, 0, st>>>(d_ic, d_pub, npub, k, terms, flags, d_status);
-  vb::k_vb_ic_sum<<<nblk(k, 64), 64, 0, st>>>(d_ic, terms, npub, k, icp, flags, d_status);
-  vb::k_vb_rho_terms<<<nblk(3 * k, 2), 32, 0, st>>>(d_proofs, icp, d_rho, k, rterms);
-  vb::k_vb_sums<<<1, vb::kSumThreads, 0, st>>>(d_vk, rterms, d_rho, flags, k, sums, k_reg);
-  const vb::MlArgs ma{d_proofs, d_vk, rterms, sums, flags, k_reg, k};
-  // the kernel rule of b200_pairing_batch (B200_CFG_PAIRING_KERNEL; auto: a warp per pair up to 2048 pairs)
-  const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
-  if (thread_kernel) vb::k_vb_miller_thread<<<nblk(n, 32), 32, 0, st>>>(ma, n, mvals);
-  else vb::k_vb_miller_warp<<<nblk(n, vb::kMlWarps), 32 * vb::kMlWarps, 0, st>>>(ma, n, mvals);
-  vb::k_vb_product<<<(unsigned)nparts, 32 * vb::kProdWarps, 0, st>>>(mvals, n, parts);
-  vb::k_vb_final<<<1, 32 * vb::kProdWarps, 0, st>>>(parts, nparts, k_reg, agg, d_status);
-  k_vb_verify_each<<<(unsigned)k, 128, 0, st>>>(d_proofs, d_vk, icp, flags, agg, k, d_ok, d_status, err);
-  g_launches += npub ? 9 : 8;
-  CU(cudaGetLastError());
-  return B200_OK;
-}
 Fq fq_load_std(const uint64_t* v) {
   Fq r;
   memcpy(&r, v, sizeof(Fq));
@@ -1490,142 +1223,6 @@ int verify_batch_check_vk(const char* what, const uint64_t* ic, size_t n_ic, con
       return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (Vk G2 point at infinity; the reference panics, bn128.go:238-241)", what);
   return B200_OK;
 }
-// device image of the Vk, IC and rho: vb::Vk | IC | rho
-size_t vb_vk_bytes(size_t n_ic, size_t k) { return sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq) + 2 * k * sizeof(uint64_t); }
-int vb_upload_vk(uint8_t* d, const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2, const uint64_t* gamma2,
-                 const uint64_t* delta2, size_t k, const uint64_t* rho, cudaStream_t st) {
-  std::vector<uint8_t> h(vb_vk_bytes(n_ic, k));
-  vb::Vk* v = (vb::Vk*)h.data();
-  std::memcpy(v->alpha, alpha1, sizeof v->alpha);
-  std::memcpy(v->beta, beta2, sizeof v->beta);
-  std::memcpy(v->gamma, gamma2, sizeof v->gamma);
-  std::memcpy(v->delta, delta2, sizeof v->delta);
-  std::memcpy(h.data() + sizeof(vb::Vk), ic, n_ic * 3 * sizeof(Fq));
-  std::memcpy(h.data() + sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq), rho, 2 * k * sizeof(uint64_t));
-  CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, st));
-  return B200_OK;
-}
-int groth16_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2, const uint64_t* gamma2,
-                              const uint64_t* delta2, const uint64_t* pi_a, const uint64_t* pi_b, const uint64_t* pi_c,
-                              const uint64_t* pub, size_t npub, size_t k, const uint64_t* rho, int* ok, uint32_t* status) {
-  const char* what = "groth16_verify_batch";
-  if (!pi_a || !pi_b || !pi_c || !ok || (npub && !pub)) return fail(B200_EINVAL, "%s: null pointer", what);
-  int rc = verify_batch_check_vk(what, ic, n_ic, alpha1, beta2, gamma2, delta2, npub, k, rho);
-  if (rc) return rc;
-  for (size_t i = 0; i < k * npub; i++)
-    if (fr_load_std(pub + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: scalar / coefficient >= r", what);
-  // the batch prover's layout, PiA | PiC | PiB per proof
-  std::vector<uint64_t> proofs(48 * k);
-  for (size_t p = 0; p < k; p++) {
-    std::memcpy(&proofs[48 * p], pi_a + 12 * p, 12 * sizeof(uint64_t));
-    std::memcpy(&proofs[48 * p + 12], pi_c + 12 * p, 12 * sizeof(uint64_t));
-    std::memcpy(&proofs[48 * p + 24], pi_b + 24 * p, 24 * sizeof(uint64_t));
-  }
-  for (size_t i = 0; i < 12 * k; i++)
-    if (fq_load_std(&proofs[4 * i]).geq_modulus()) return fail(B200_ERANGE, "%s: point coordinate >= q", what);
-  for (size_t p = 0; p < k; p++) {
-    const uint64_t* z = &proofs[48 * p + 40];
-    if (!(z[0] | z[1] | z[2] | z[3] | z[4] | z[5] | z[6] | z[7]))
-      return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (PiB of proof %zu at infinity; the reference panics, bn128.go:238-241)", what, p);
-  }
-  cudaStream_t st = g_ctx[0].main;
-  const size_t vkb = vb_vk_bytes(n_ic, k), pb = proofs.size() * sizeof(uint64_t), ub = (npub ? npub : 1) * k * 32,
-               okb = (k + 1) * sizeof(int);
-  const VbScratch L(k, npub);
-  StreamBuf buf;
-  CU(buf.alloc(vkb + pb + ub + okb + L.bytes + 1024, st));
-  uint8_t* d = (uint8_t*)buf.p;
-  auto carve = [&](size_t b) { uint8_t* r = d; d += (b + 255) & ~(size_t)255; return r; };
-  uint8_t* d_vk = carve(vkb);
-  uint64_t* d_proofs = (uint64_t*)carve(pb);
-  uint64_t* d_pub = (uint64_t*)carve(ub);
-  int* d_ok = (int*)carve(okb);
-  uint8_t* d_scratch = carve(L.bytes);
-  if ((rc = vb_upload_vk(d_vk, ic, n_ic, alpha1, beta2, gamma2, delta2, k, rho, st))) return rc;
-  CU(cudaMemcpyAsync(d_proofs, proofs.data(), pb, cudaMemcpyHostToDevice, st));
-  if (npub) CU(cudaMemcpyAsync(d_pub, pub, npub * k * 32, cudaMemcpyHostToDevice, st));
-  const Fq* d_ic = (const Fq*)(d_vk + sizeof(vb::Vk));
-  const uint64_t* d_rho = (const uint64_t*)(d_vk + sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq));
-  if ((rc = verify_batch_enqueue(d_ic, (const vb::Vk*)d_vk, d_proofs, d_pub, npub, k, d_rho, d_ok, (uint32_t*)(d_ok + k),
-                                 d_scratch, st)))
-    return rc;
-  std::vector<int> h_ok(k + 1);
-  CU(cudaMemcpyAsync(h_ok.data(), d_ok, okb, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  std::memcpy(ok, h_ok.data(), k * sizeof(int));
-  if (status) *status = (uint32_t)h_ok[k];
-  return B200_OK;
-}
-int groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2,
-                                const uint64_t* gamma2, const uint64_t* delta2, const void* d_proofs, const void* d_public,
-                                size_t npub, size_t k, const uint64_t* rho, void* d_ok, cudaStream_t st) {
-  const char* what = "groth16_verify_batch_device";
-  if (!d_proofs || !d_ok || (npub && !d_public)) return fail(B200_EINVAL, "%s: null pointer", what);
-  int rc = verify_batch_check_vk(what, ic, n_ic, alpha1, beta2, gamma2, delta2, npub, k, rho);
-  if (rc) return rc;
-  const size_t vkb = (vb_vk_bytes(n_ic, k) + 255) & ~(size_t)255;
-  const VbScratch L(k, npub);
-  StreamBuf buf;
-  CU(buf.alloc(vkb + L.bytes, st));
-  uint8_t* d = (uint8_t*)buf.p;
-  if ((rc = vb_upload_vk(d, ic, n_ic, alpha1, beta2, gamma2, delta2, k, rho, st))) return rc;
-  return verify_batch_enqueue((const Fq*)(d + sizeof(vb::Vk)), (const vb::Vk*)d, (const uint64_t*)d_proofs,
-                              (const uint64_t*)d_public, npub, k, (const uint64_t*)(d + sizeof(vb::Vk) + n_ic * 3 * sizeof(Fq)),
-                              (int*)d_ok, (uint32_t*)((int*)d_ok + k), d + vkb, st);
-}
-
-// ---- batched Pinocchio verification (verify_batch_pinocchio.cuh) ------------------------------------------------------
-// per-call scratch of pvb_enqueue, carved from one allocation
-struct PvbScratch {
-  size_t off[10];
-  size_t bytes;
-  PvbScratch(size_t k, size_t npub) {
-    const size_t n = k + vb::kPvbSums, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
-    const size_t sz[10] = {(k + 1) * 4, 4, 4, 4, 6 * k * sizeof(Fq), (npub ? npub * k : 1) * sizeof(Jacobian<Fq>),
-                           vb::kPvbRhoTerms * k * sizeof(Jacobian<Fq>), vb::kPvbSums * sizeof(Jacobian<Fq>),
-                           6 * n * sizeof(F2), 6 * nparts * sizeof(F2)};
-    bytes = 0;
-    for (int i = 0; i < 10; i++) {
-      off[i] = bytes;
-      bytes += (sz[i] + 255) & ~(size_t)255;
-    }
-  }
-};
-// Every launch of a batched Pinocchio verification, on `st`: d_ok[0..k) verdicts, *d_status the status bits (zeroed here
-// first).  A fixed launch sequence: no step waits for the host, whatever k and whatever the outcome.
-int pvb_enqueue(const Fq* d_ic, const vb::PVk* d_vk, const uint64_t* d_proofs, const uint64_t* d_pub, size_t npub, size_t k,
-                const uint64_t* d_rho, int* d_ok, uint32_t* d_status, uint8_t* scratch, cudaStream_t st) {
-  const PvbScratch L(k, npub);
-  uint32_t* flags = (uint32_t*)(scratch + L.off[0]);
-  uint32_t* k_reg = (uint32_t*)(scratch + L.off[1]);
-  uint32_t* agg = (uint32_t*)(scratch + L.off[2]);
-  int* err = (int*)(scratch + L.off[3]);
-  Fq* sts = (Fq*)(scratch + L.off[4]);
-  Jacobian<Fq>* terms = (Jacobian<Fq>*)(scratch + L.off[5]);
-  Jacobian<Fq>* rterms = (Jacobian<Fq>*)(scratch + L.off[6]);
-  Jacobian<Fq>* sums = (Jacobian<Fq>*)(scratch + L.off[7]);
-  F2* mvals = (F2*)(scratch + L.off[8]);
-  F2* parts = (F2*)(scratch + L.off[9]);
-  const size_t n = k + vb::kPvbSums, nparts = (n + vb::kProdPerCta - 1) / vb::kProdPerCta;
-  CU(cudaMemsetAsync(scratch, 0, L.off[4], st));
-  CU(cudaMemsetAsync(d_status, 0, sizeof(uint32_t), st));
-  vb::k_pvb_classify<<<nblk(k + 7, 64), 64, 0, st>>>(d_proofs, d_vk, k, flags, d_status);
-  if (npub) vb::k_vb_ic_terms<<<nblk(npub * k, 2), 32, 0, st>>>(d_ic, d_pub, npub, k, terms, flags, d_status);
-  vb::k_pvb_st<<<nblk(k, 64), 64, 0, st>>>(d_ic, terms, d_proofs, npub, k, sts, flags, d_status);
-  vb::k_pvb_rho_terms<<<nblk(vb::kPvbRhoTerms * k, 2), 32, 0, st>>>(d_proofs, d_vk, sts, d_rho, k, rterms);
-  vb::k_pvb_sums<<<vb::kPvbSums, vb::kSumThreads, 0, st>>>(rterms, flags, k, sums, k_reg);
-  const vb::PvbMlArgs ma{d_proofs, d_vk, rterms, sums, flags, k_reg, k};
-  // the kernel rule of b200_pairing_batch (B200_CFG_PAIRING_KERNEL; auto: a warp per pair up to 2048 pairs)
-  const bool thread_kernel = g_pairing_kernel == 1 || (g_pairing_kernel == 0 && n > 2048);
-  if (thread_kernel) vb::k_vb_miller_thread<<<nblk(n, 32), 32, 0, st>>>(ma, n, mvals);
-  else vb::k_vb_miller_warp<<<nblk(n, vb::kMlWarps), 32 * vb::kMlWarps, 0, st>>>(ma, n, mvals);
-  vb::k_vb_product<<<(unsigned)nparts, 32 * vb::kProdWarps, 0, st>>>(mvals, n, parts);
-  vb::k_vb_final<<<1, 32 * vb::kProdWarps, 0, st>>>(parts, nparts, k_reg, agg, d_status);
-  k_pvb_verify_each<<<(unsigned)k, 128, 0, st>>>(d_proofs, d_vk, sts, flags, agg, k, d_ok, d_status, err);
-  g_launches += npub ? 9 : 8;
-  CU(cudaGetLastError());
-  return B200_OK;
-}
 // The checks both entries make on the host arguments of the Vk, IC and rho.
 int pvb_check_vk(const char* what, const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2, size_t npub,
                  size_t k, const uint64_t* rho) {
@@ -1647,46 +1244,26 @@ int pvb_check_vk(const char* what, const uint64_t* ic, size_t n_ic, const uint64
   }
   return B200_OK;
 }
-// device image of the Vk, IC and rho: vb::PVk | IC | rho
-size_t pvb_vk_bytes(size_t n_ic, size_t k) { return sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq) + 10 * k * sizeof(uint64_t); }
-int pvb_upload_vk(uint8_t* d, const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2, size_t k,
-                  const uint64_t* rho, cudaStream_t st) {
-  static_assert(sizeof(vb::PVk) == (24 + 120 + 24) * sizeof(uint64_t), "PVk is vk_g1 | vk_g2 | g2");
-  std::vector<uint8_t> h(pvb_vk_bytes(n_ic, k));
-  std::memcpy(h.data(), vk_g1, 24 * sizeof(uint64_t));
-  std::memcpy(h.data() + 24 * sizeof(uint64_t), vk_g2, 120 * sizeof(uint64_t));
-  std::memcpy(h.data() + 144 * sizeof(uint64_t), kG2GenJacStd, 24 * sizeof(uint64_t));
-  std::memcpy(h.data() + sizeof(vb::PVk), ic, n_ic * 3 * sizeof(Fq));
-  std::memcpy(h.data() + sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq), rho, 10 * k * sizeof(uint64_t));
-  CU(cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, st));
-  return B200_OK;
-}
-int pinocchio_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2,
-                                const uint64_t* out_g1, const uint64_t* pi_b, const uint64_t* pub, size_t npub, size_t k,
-                                const uint64_t* rho, int* ok, uint32_t* status) {
-  const char* what = "pinocchio_verify_batch";
-  if (!out_g1 || !pi_b || !ok || (npub && !pub)) return fail(B200_EINVAL, "%s: null pointer", what);
-  int rc = pvb_check_vk(what, ic, n_ic, vk_g1, vk_g2, npub, k, rho);
-  if (rc) return rc;
+// The host entries past their Vk checks: the signals' range, the proofs (packed as the batch provers lay them out, PiB's
+// 24 words last in each) checked for range and for PiB at infinity, one upload of the Vk image, the proofs and the
+// signals, the launches, and the verdicts and the status word copied back.
+template <class Vk>
+int verify_batch_host(const char* what, const std::vector<uint8_t>& img, size_t n_ic, const std::vector<uint64_t>& proofs,
+                      const uint64_t* pub, size_t npub, size_t k, int* ok, uint32_t* status) {
   for (size_t i = 0; i < k * npub; i++)
     if (fr_load_std(pub + 4 * i).geq_modulus()) return fail(B200_ERANGE, "%s: scalar / coefficient >= r", what);
-  // the batch prover's device layout: the seven G1 points, then PiB, per proof
-  std::vector<uint64_t> proofs(vb::kPvbProofWords * k);
-  for (size_t p = 0; p < k; p++) {
-    std::memcpy(&proofs[vb::kPvbProofWords * p], out_g1 + 84 * p, 84 * sizeof(uint64_t));
-    std::memcpy(&proofs[vb::kPvbProofWords * p + 84], pi_b + 24 * p, 24 * sizeof(uint64_t));
-  }
-  for (size_t i = 0; i < 27 * k; i++)
+  for (size_t i = 0; i < proofs.size() / 4; i++)
     if (fq_load_std(&proofs[4 * i]).geq_modulus()) return fail(B200_ERANGE, "%s: point coordinate >= q", what);
+  const size_t pw = proofs.size() / k;
   for (size_t p = 0; p < k; p++) {
-    const uint64_t* z = &proofs[vb::kPvbProofWords * p + 100];
+    const uint64_t* z = &proofs[pw * (p + 1) - 8];
     if (!(z[0] | z[1] | z[2] | z[3] | z[4] | z[5] | z[6] | z[7]))
       return fail(B200_EINVAL, "%s: q1[2] != Fq2.One() (PiB of proof %zu at infinity; the reference panics, bn128.go:238-241)", what, p);
   }
   cudaStream_t st = g_ctx[0].main;
-  const size_t vkb = pvb_vk_bytes(n_ic, k), pb = proofs.size() * sizeof(uint64_t), ub = (npub ? npub : 1) * k * 32,
+  const size_t vkb = img.size(), pb = proofs.size() * sizeof(uint64_t), ub = (npub ? npub : 1) * k * 32,
                okb = (k + 1) * sizeof(int);
-  const PvbScratch L(k, npub);
+  const VbScratch<Vk> L(k, npub);
   StreamBuf buf;
   CU(buf.alloc(vkb + pb + ub + okb + L.bytes + 1024, st));
   uint8_t* d = (uint8_t*)buf.p;
@@ -1696,19 +1273,74 @@ int pinocchio_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t*
   uint64_t* d_pub = (uint64_t*)carve(ub);
   int* d_ok = (int*)carve(okb);
   uint8_t* d_scratch = carve(L.bytes);
-  if ((rc = pvb_upload_vk(d_vk, ic, n_ic, vk_g1, vk_g2, k, rho, st))) return rc;
+  CU(cudaMemcpyAsync(d_vk, img.data(), vkb, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(d_proofs, proofs.data(), pb, cudaMemcpyHostToDevice, st));
   if (npub) CU(cudaMemcpyAsync(d_pub, pub, npub * k * 32, cudaMemcpyHostToDevice, st));
-  const Fq* d_ic = (const Fq*)(d_vk + sizeof(vb::PVk));
-  const uint64_t* d_rho = (const uint64_t*)(d_vk + sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq));
-  if ((rc = pvb_enqueue(d_ic, (const vb::PVk*)d_vk, d_proofs, d_pub, npub, k, d_rho, d_ok, (uint32_t*)(d_ok + k), d_scratch, st)))
-    return rc;
+  CU(verify_batch_enqueue(vb_env(), VbCall<Vk>{d_vk, n_ic, d_proofs, d_pub, npub, k, d_scratch, (uint32_t*)(d_ok + k)}, d_ok, st));
   std::vector<int> h_ok(k + 1);
   CU(cudaMemcpyAsync(h_ok.data(), d_ok, okb, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   std::memcpy(ok, h_ok.data(), k * sizeof(int));
   if (status) *status = (uint32_t)h_ok[k];
   return B200_OK;
+}
+// The _device entries past their Vk checks: the Vk image and the scratch in one stream-ordered allocation, then the
+// launches on `st`; returns without waiting.
+template <class Vk>
+int verify_batch_device(const std::vector<uint8_t>& img, size_t n_ic, const void* d_proofs, const void* d_public, size_t npub,
+                        size_t k, void* d_ok, cudaStream_t st) {
+  const size_t vkb = (img.size() + 255) & ~(size_t)255;
+  const VbScratch<Vk> L(k, npub);
+  StreamBuf buf;
+  CU(buf.alloc(vkb + L.bytes, st));
+  uint8_t* d = (uint8_t*)buf.p;
+  CU(cudaMemcpyAsync(d, img.data(), img.size(), cudaMemcpyHostToDevice, st));
+  const VbCall<Vk> c{d, n_ic, (const uint64_t*)d_proofs, (const uint64_t*)d_public, npub, k, d + vkb, (uint32_t*)((int*)d_ok + k)};
+  CU(verify_batch_enqueue(vb_env(), c, (int*)d_ok, st));
+  return B200_OK;
+}
+
+int groth16_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2, const uint64_t* gamma2,
+                              const uint64_t* delta2, const uint64_t* pi_a, const uint64_t* pi_b, const uint64_t* pi_c,
+                              const uint64_t* pub, size_t npub, size_t k, const uint64_t* rho, int* ok, uint32_t* status) {
+  const char* what = "groth16_verify_batch";
+  if (!pi_a || !pi_b || !pi_c || !ok || (npub && !pub)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = verify_batch_check_vk(what, ic, n_ic, alpha1, beta2, gamma2, delta2, npub, k, rho);
+  if (rc) return rc;
+  // the batch prover's layout, PiA | PiC | PiB per proof
+  std::vector<uint64_t> proofs(48 * k);
+  for (size_t p = 0; p < k; p++) {
+    std::memcpy(&proofs[48 * p], pi_a + 12 * p, 12 * sizeof(uint64_t));
+    std::memcpy(&proofs[48 * p + 12], pi_c + 12 * p, 12 * sizeof(uint64_t));
+    std::memcpy(&proofs[48 * p + 24], pi_b + 24 * p, 24 * sizeof(uint64_t));
+  }
+  return verify_batch_host<vb::Vk>(what, vb_vk_image(ic, n_ic, alpha1, beta2, gamma2, delta2, k, rho), n_ic, proofs, pub, npub, k,
+                                   ok, status);
+}
+int groth16_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t* alpha1, const uint64_t* beta2,
+                                const uint64_t* gamma2, const uint64_t* delta2, const void* d_proofs, const void* d_public,
+                                size_t npub, size_t k, const uint64_t* rho, void* d_ok, cudaStream_t st) {
+  const char* what = "groth16_verify_batch_device";
+  if (!d_proofs || !d_ok || (npub && !d_public)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = verify_batch_check_vk(what, ic, n_ic, alpha1, beta2, gamma2, delta2, npub, k, rho);
+  if (rc) return rc;
+  return verify_batch_device<vb::Vk>(vb_vk_image(ic, n_ic, alpha1, beta2, gamma2, delta2, k, rho), n_ic, d_proofs, d_public, npub,
+                                     k, d_ok, st);
+}
+int pinocchio_verify_batch_host(const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2,
+                                const uint64_t* out_g1, const uint64_t* pi_b, const uint64_t* pub, size_t npub, size_t k,
+                                const uint64_t* rho, int* ok, uint32_t* status) {
+  const char* what = "pinocchio_verify_batch";
+  if (!out_g1 || !pi_b || !ok || (npub && !pub)) return fail(B200_EINVAL, "%s: null pointer", what);
+  int rc = pvb_check_vk(what, ic, n_ic, vk_g1, vk_g2, npub, k, rho);
+  if (rc) return rc;
+  // the batch prover's device layout: the seven G1 points, then PiB, per proof
+  std::vector<uint64_t> proofs(vb::kPvbProofWords * k);
+  for (size_t p = 0; p < k; p++) {
+    std::memcpy(&proofs[vb::kPvbProofWords * p], out_g1 + 84 * p, 84 * sizeof(uint64_t));
+    std::memcpy(&proofs[vb::kPvbProofWords * p + 84], pi_b + 24 * p, 24 * sizeof(uint64_t));
+  }
+  return verify_batch_host<vb::PVk>(what, pvb_vk_image(ic, n_ic, vk_g1, vk_g2, k, rho), n_ic, proofs, pub, npub, k, ok, status);
 }
 int pinocchio_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_t* vk_g1, const uint64_t* vk_g2,
                                   const void* d_proofs, const void* d_public, size_t npub, size_t k, const uint64_t* rho,
@@ -1717,42 +1349,8 @@ int pinocchio_verify_batch_device(const uint64_t* ic, size_t n_ic, const uint64_
   if (!d_proofs || !d_ok || (npub && !d_public)) return fail(B200_EINVAL, "%s: null pointer", what);
   int rc = pvb_check_vk(what, ic, n_ic, vk_g1, vk_g2, npub, k, rho);
   if (rc) return rc;
-  const size_t vkb = (pvb_vk_bytes(n_ic, k) + 255) & ~(size_t)255;
-  const PvbScratch L(k, npub);
-  StreamBuf buf;
-  CU(buf.alloc(vkb + L.bytes, st));
-  uint8_t* d = (uint8_t*)buf.p;
-  if ((rc = pvb_upload_vk(d, ic, n_ic, vk_g1, vk_g2, k, rho, st))) return rc;
-  return pvb_enqueue((const Fq*)(d + sizeof(vb::PVk)), (const vb::PVk*)d, (const uint64_t*)d_proofs, (const uint64_t*)d_public,
-                     npub, k, (const uint64_t*)(d + sizeof(vb::PVk) + n_ic * 3 * sizeof(Fq)), (int*)d_ok,
-                     (uint32_t*)((int*)d_ok + k), d + vkb, st);
+  return verify_batch_device<vb::PVk>(pvb_vk_image(ic, n_ic, vk_g1, vk_g2, k, rho), n_ic, d_proofs, d_public, npub, k, d_ok, st);
 }
-
-#else  // experiment builds without the verifier side (ptxas 12.9 crashes on the pairing kernels under -DB200_KARATSUBA)
-int pairing_batch_host(const uint64_t*, const uint64_t*, size_t, uint64_t*) { return fail(B200_EINVAL, "pairing: not in this build variant"); }
-int groth16_verify_batch_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
-                              const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*, size_t, size_t, const uint64_t*,
-                              int*, uint32_t*) {
-  return fail(B200_EINVAL, "groth16_verify_batch: not in this build variant");
-}
-int groth16_verify_batch_device(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
-                                const void*, const void*, size_t, size_t, const uint64_t*, void*, cudaStream_t) {
-  return fail(B200_EINVAL, "groth16_verify_batch_device: not in this build variant");
-}
-int pinocchio_verify_batch_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
-                                const uint64_t*, size_t, size_t, const uint64_t*, int*, uint32_t*) {
-  return fail(B200_EINVAL, "pinocchio_verify_batch: not in this build variant");
-}
-int pinocchio_verify_batch_device(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const void*, const void*, size_t,
-                                  size_t, const uint64_t*, void*, cudaStream_t) {
-  return fail(B200_EINVAL, "pinocchio_verify_batch_device: not in this build variant");
-}
-int fq12_mul_batch_host(const uint64_t*, const uint64_t*, size_t, uint64_t*) { return fail(B200_EINVAL, "fq12_mul: not in this build variant"); }
-int groth16_verify_host(const uint64_t*, size_t, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*, const uint64_t*,
-                        const uint64_t*, const uint64_t*, const uint64_t*, size_t, int*) {
-  return fail(B200_EINVAL, "groth16_verify: not in this build variant");
-}
-#endif
 
 template <class F>
 int group_op_host(int op, const uint64_t* p, const uint64_t* q, size_t n, uint64_t* out) {

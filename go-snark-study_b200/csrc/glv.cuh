@@ -1,6 +1,6 @@
 // GLV scalar multiplication on BN254 G1 by the sixteen lanes of a half-warp, and the host-side lattice decomposition it
 // consumes.  Used by the prover's blinding products s*A, r*B1 (groth16.go:272-273; k_groth16_products in prove_host.cuh) and
-// by the verifier's public-input sum (groth16.go:283-286; k_ic_terms in capi.cu).  Kept free of runtime-API calls so that the
+// by the verifier's public-input sum (groth16.go:283-286; k_ic_terms in verify_host.cuh).  Kept free of runtime-API calls so that the
 // CPU emulation (tests/host/host_kernel_test.cpp: 32 OS threads, barrier shuffles) runs the very same lanes against the oracle.
 #pragma once
 #include <cstdint>

@@ -8,9 +8,9 @@
 // the curve and not infinity, B_i on the twist and in the order-r subgroup, icPubl_i not infinity, every input in range —
 // and only under a regular Vk: for anything else the reference's verdict is not that of the bilinear check (it pairs a
 // G1 infinity as the affine point (0, 0), bn128.go preComputeG1), so such proofs take the per-proof check (k_vb_verify_each
-// in capi.cu), which is b200_groth16_verify's kernel for one proof per CTA.
+// below), which is b200_groth16_verify's kernel for one proof per CTA.
 //
-// Launch order (capi.cu verify_batch_enqueue), a fixed sequence whatever k and whatever the outcome:
+// Launch order (verify_host.cuh: vb_aggregate, then vb_verdicts), a fixed sequence whatever k and whatever the outcome:
 //   k_vb_classify      range, curve and subgroup tests of every proof and of the Vk -> per-proof flags
 //   k_vb_ic_terms      pub_ij * IC[j+1] by the GLV half-warp product, the signals split on the device (skipped if npub = 0)
 //   k_vb_ic_sum        icPubl_i = IC[0] + sum_j terms in the reference's order with its Add (as k_ic_sum)
@@ -20,7 +20,8 @@
 //   k_vb_product       partial products of 64 Miller values per CTA
 //   k_vb_final         product of the partials, one final exponentiation, == 1 -> aggregate bit
 //   k_vb_verify_each   per-proof verdicts: regular proofs under a passed aggregate exit at once
-// Host/device: tests/host/verify_batch_test.cpp runs these kernels on the CPU emulation against the oracle.
+// Host/device: tests/host/verify_batch_test.cpp runs these kernels, and the aggregate through verify_host.cuh, on the CPU
+// emulation against the oracle.
 #pragma once
 #include "glv.cuh"
 #include "pairing_warp.cuh"
@@ -357,6 +358,77 @@ __global__ void __launch_bounds__(32 * kProdWarps) k_vb_final(const F2* parts, s
     *agg = pass ? 1u : 0u;
     if (pass) atomicOr(status, kStAggregate);
   }
+}
+
+// The two per-proof helpers below have internal linkage (static): groth16_verify_cta is called, not inlined, and with
+// external linkage ptxas allocates the registers of its callers (k_groth16_verify, k_vb_verify_each) differently.
+// lane 0 validates and normalises the Jacobian inputs (preComputeG1 / G2.Affine); returns warp-uniformly whether a pairing
+// is to be computed (false: out-of-range coordinate or G2 infinity — the reference panics, bn128.go:238-241 — result = one)
+static __device__ bool warp_pairing_inputs(wp::Ws& ws, const Fq* g1, const Fq2* g2, F2::B& px, F2::B& py, F2& qx, F2& qy, int* err) {
+  int go = 1;
+  if ((threadIdx.x & 31u) == 0) {
+    bool bad = false;
+    for (int k = 0; k < 3; k++) bad = bad || g1[k].geq_modulus() || g2[k].c0.geq_modulus() || g2[k].c1.geq_modulus();
+    Jacobian<Fq> p{g1[0].to_mont(), g1[1].to_mont(), g1[2].to_mont()};
+    Jacobian<Fq2> q{g2[0].to_mont(), g2[1].to_mont(), g2[2].to_mont()};
+    if (bad || q.is_inf()) {
+      atomicOr(err, bad ? 1 : 8);
+      go = 0;
+    } else {
+      Affine<Fq> pa = jac_to_affine(p);
+      Affine<Fq2> qa = jac_to_affine(q);
+#pragma unroll
+      for (int i = 0; i < 8; i++) { px.l[i] = pa.x.l[i]; py.l[i] = pa.y.l[i]; }
+      qx = qa.x;
+      qy = qa.y;
+    }
+  }
+  (void)ws;
+  return __shfl_sync(0xffffffffu, go, 0) != 0;
+}
+// groth16.VerifyProof (groth16/groth16.go:281-305): e(A,B) == e(alpha,beta) * (e(icPubl,gamma) * e(C,delta)).
+// Warp w of a 128-thread CTA pairs g1 with g2, the w-th of (A, alpha1, icPubl, C) and (B, beta2, gamma2, delta2) (Jacobian
+// standard form); warp 0 then forms the right-hand side with two warp-wide F_q^12 products and compares.
+static __device__ void groth16_verify_cta(wp::Ws* wss, const Fq* g1, const Fq2* g2, int* ok, int* err) {
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  wp::Ws& ws = wss[warp];
+  F2::B px, py;
+  F2 qx, qy;
+  if (warp_pairing_inputs(ws, g1, g2, px, py, qx, qy, err)) wp::pairing(ws, px, py, qx, qy);
+  else wp::f12_set_one(ws, wp::RF);
+  __syncthreads();
+  if (warp == 0) {
+    if (lane < 6) {
+      ws.r[2][lane] = wss[1].r[wp::RF][lane];
+      ws.r[3][lane] = wss[2].r[wp::RF][lane];
+      ws.r[4][lane] = wss[3].r[wp::RF][lane];
+    }
+    wp::wsync();
+    wp::f12_mul(ws, 3, 3, 4);
+    wp::f12_mul(ws, 2, 2, 3);
+    const int same = lane < 6 ? (ws.r[0][lane] == ws.r[2][lane] ? 1 : 0) : 1;
+    const unsigned all = __ballot_sync(0xffffffffu, same);
+    if (lane == 0) *ok = all == 0xffffffffu ? 1 : 0;
+  }
+}
+// k_groth16_verify over a batch, one CTA per proof: a regular proof under a passed aggregate is accepted at once, a bad one
+// (coordinate >= q, signal >= r, PiB at infinity) gets 0, every other proof the single call's verdict.
+__global__ void __launch_bounds__(128) k_vb_verify_each(const uint64_t* proofs, const Vk* vk, const Fq* icp,
+                                                        const uint32_t* flags, const uint32_t* agg, size_t k, int* ok,
+                                                        uint32_t* status, int* err) {
+  __shared__ wp::Ws wss[4];
+  const size_t p = blockIdx.x;
+  const uint32_t f = flags[p] | flags[k];
+  if ((f & kBad) || (!f && *agg)) {
+    if (threadIdx.x == 0) ok[p] = (f & kBad) ? 0 : 1;
+    return;
+  }
+  if (threadIdx.x == 0) atomicOr(status, kStPerProof);
+  const uint32_t warp = threadIdx.x >> 5;
+  const ProofView v = proof_at(proofs, p);
+  const Fq* g1 = warp == 0 ? v.a : (warp == 1 ? vk->alpha : (warp == 2 ? icp + 3 * p : v.c));
+  const Fq2* g2 = warp == 0 ? v.b : (warp == 1 ? vk->beta : (warp == 2 ? vk->gamma : vk->delta));
+  groth16_verify_cta(wss, g1, g2, ok + p, err);
 }
 
 }  // namespace vb

@@ -17,9 +17,9 @@
 // with their own final exponentiations per proof for snark.VerifyProof.  Only *regular* proofs enter the sum — the seven
 // G1 points and S_i, T_i on the curve and not infinity, PiB on the twist and in the order-r subgroup, every input in range
 // — and only under a regular Vk (Vkb, G1Kbg as G1 points; Vka, Vkc, G2Kbg, G2Kg, Vkz as G2 points); any other proof takes
-// the per-proof check (k_pvb_verify_each in capi.cu: snark.VerifyProof's twelve pairings, one CTA per proof).
+// the per-proof check (k_pvb_verify_each below: snark.VerifyProof's twelve pairings, one CTA per proof).
 //
-// Launch order (capi.cu pvb_enqueue), a fixed sequence whatever k and whatever the outcome:
+// Launch order (verify_host.cuh: vb_aggregate, then vb_verdicts), a fixed sequence whatever k and whatever the outcome:
 //   k_pvb_classify       range, curve and subgroup tests of every proof and of the Vk -> per-proof flags
 //   k_vb_ic_terms        pub_ij * IC[j+1] (verify_batch.cuh; skipped if npub = 0)
 //   k_pvb_st             Vkx_i, S_i, T_i in the reference's order with its Add; S_i or T_i irregular -> proof irregular
@@ -28,7 +28,8 @@
 //   k_vb_miller_warp / _thread   Miller loops of the k_reg + 6 pairs (PvbMlArgs; irregular pairs contribute one)
 //   k_vb_product, k_vb_final     as for Groth16: product tree, one final exponentiation, == 1 -> aggregate bit
 //   k_pvb_verify_each    per-proof verdicts: regular proofs under a passed aggregate exit at once
-// Host/device: tests/host/pinocchio_verify_batch_test.cpp runs these kernels on the CPU emulation against the oracle.
+// Host/device: tests/host/pinocchio_verify_batch_test.cpp runs the classification kernel, and the aggregate through
+// verify_host.cuh, on the CPU emulation against the oracle.
 #pragma once
 #include "verify_batch.cuh"
 
@@ -247,6 +248,53 @@ DEV const Fq2* pvb_pairing_g2(const uint64_t* proofs, const PVk* vk, size_t p, i
     case 11: return vk->g2kg;
     default: return vk->g2;
   }
+}
+
+// snark.VerifyProof over a batch, one CTA per proof: a regular proof under a passed aggregate is accepted at once, a bad one
+// (coordinate >= q, signal >= r, PiB at infinity) gets 0, every other proof the reference's verdict: its twelve pairings
+// (warp w runs pairings 3w .. 3w + 2 with warp_pairing_inputs' semantics), the two F_q^12 products e7 e8 and e9 e10, and
+// the five comparisons of snark.go:292-372.
+__global__ void __launch_bounds__(128) k_pvb_verify_each(const uint64_t* proofs, const PVk* vk, const Fq* st,
+                                                         const uint32_t* flags, const uint32_t* agg, size_t k, int* ok,
+                                                         uint32_t* status, int* err) {
+  __shared__ wp::Ws wss[4];
+  __shared__ F2 e[kPvbPairings][6];
+  const size_t p = blockIdx.x;
+  const uint32_t f = flags[p] | flags[k];
+  if ((f & kBad) || (!f && *agg)) {
+    if (threadIdx.x == 0) ok[p] = (f & kBad) ? 0 : 1;
+    return;
+  }
+  if (threadIdx.x == 0) atomicOr(status, kStPerProof);
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  wp::Ws& ws = wss[warp];
+  for (int j = 3 * (int)warp; j < 3 * (int)warp + 3; j++) {
+    F2::B px, py;
+    F2 qx, qy;
+    if (warp_pairing_inputs(ws, pvb_pairing_g1(proofs, vk, st, p, j), pvb_pairing_g2(proofs, vk, p, j), px, py, qx, qy, err))
+      wp::pairing(ws, px, py, qx, qy);
+    else
+      wp::f12_set_one(ws, wp::RF);
+    if (lane < 6) e[j][lane] = ws.r[wp::RF][lane];
+    wp::wsync();
+  }
+  __syncthreads();
+  if (warp != 0) return;
+  if (lane < 6) {
+    ws.r[2][lane] = e[7][lane];
+    ws.r[3][lane] = e[8][lane];
+    ws.r[4][lane] = e[9][lane];
+    ws.r[5][lane] = e[10][lane];
+  }
+  wp::wsync();
+  wp::f12_mul(ws, 2, 2, 3);   // e(PiH, Vkz) e(PiC, g2)
+  wp::f12_mul(ws, 4, 4, 5);   // e(T, G2Kbg) e(G1Kbg, PiB)
+  int same = 1;
+  if (lane < 6)
+    same = e[0][lane] == e[1][lane] && e[2][lane] == e[3][lane] && e[4][lane] == e[5][lane] && e[6][lane] == ws.r[2][lane] &&
+           ws.r[4][lane] == e[11][lane];
+  const unsigned all = __ballot_sync(0xffffffffu, same);
+  if (lane == 0) ok[p] = all == 0xffffffffu ? 1 : 0;
 }
 
 }  // namespace vb
